@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
-"""Headline benchmark: MPix/s of guetzli::Process(RGB) (bit-exact JPEG) on B200.
+"""Headline benchmark: MPix/s of guetzli::Process(RGB) (bit-exact JPEG) on H100.
 
-    python bench.py --gpus N --steps K --warmup W          # this repo (CUDA, sm_100a)
+    python bench.py --gpus N --steps K --warmup W          # this repo (CUDA, sm_90a)
     python bench.py --impl reference --gpus N ...          # reference CPU arm (oracle/_ref)
     python bench.py --mode tiled --workload gradnoise8k_q95 --gpus N   # ONE image over N GPUs
 
@@ -12,7 +12,8 @@ scaling, no data-path collective; torch.distributed only for the barrier and the
 max-over-ranks time).  The same run also reports the latency of ONE image alone on the GPU
 (SURVEY.md §8(d)'s per-call definition) and, unless --no-tiled-leg, one 8K image tiled over
 all N ranks through the NCCL strip mode (BASELINE configs[3], strong scaling).
-Prints ONE JSON line on rank 0.  See DESIGN.md "Measurement".
+Prints ONE JSON line on rank 0.  See DESIGN.md "Measurement".  --dump-outputs DIR also writes the JPEGs of the
+last timed step (rank 0) as DIR/*.npy, so that two builds can be compared output for output.
 """
 import argparse
 import hashlib
@@ -72,17 +73,11 @@ COMPARE_KERNELS = {
 }
 COMPARE_FLOP_PER_PX = 2500.0  # SURVEY.md §8(d): un-fused FP32 instructions per pixel per Compare (no FMA)
 
-# dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed ncu
-# --set full captures (profiles/), bytes; None until captured.
-NCU_TRAFFIC = {
-    # profiles/r02_ncu_fused.csv (noise1080p, per launch: dram read + write)
-    "hf_fused": 74.76e6 + 47.16e6, "mf_fused_y": 58.22e6 + 12.7e6, "mask_y_combine": 74.77e6 + 3.22e6,
-    "malta_sums": 49.82e6 + 3.18e6, "opsin_fused": 24.96e6 + 0.08e6, "lf_fused_y": 49.82e6 + 10.12e6,
-    "noise_fused_y": 33.26e6, "final_fused": 8.32e6, "mask_pre": 41.48e6 + 0.33e6,
-    # profiles/r01_final2_ncu_full.csv / r01_ncu_full_malta_blur.csv (staged chain)
-    "malta_channel": 49.8e6 + 1.7e6 + 24.9e6,
-    "blur_x": 8.33e6, "blur_y": 8.32e6,
-}
+# H100 SXM: SMs x FP32 lanes per SM, and the data sheet's HBM3 bandwidth and max SM clock (fallbacks
+# when MEASURED_PEAKS.json or nvidia-smi is absent)
+H100_SMS, H100_FP32_LANES, H100_HBM_GBS, H100_MAX_SM_MHZ = 132, 128, 3350.0, 1980.0
+# --dump-outputs: total size of the .npy files
+DUMP_BYTES = 64 * 10**6
 
 
 def make_image(spec, index=0):
@@ -155,7 +150,7 @@ class DeviceTimer:
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -331,6 +326,21 @@ def run_tiled(args, wl, name, gb, dist, rank, world, local, steps, warmup):
     return out
 
 
+def dump_outputs(out_dir, jpegs):
+    """The JPEG bytes of each image as float32 (jpeg_NN.npy) and their lengths (jpeg_sizes.npy, float64).
+    A JPEG longer than its share of DUMP_BYTES is written as a fixed sample: the bytes at sorted positions
+    drawn by a generator seeded with the image's index, plus the first and the last byte."""
+    os.makedirs(out_dir, exist_ok=True)
+    cap = (DUMP_BYTES - 8 * len(jpegs) - 4096) // 4 // max(1, len(jpegs))
+    np.save(os.path.join(out_dir, "jpeg_sizes.npy"), np.array([len(b) for b in jpegs], dtype=np.float64))
+    for j, b in enumerate(jpegs):
+        a = np.frombuffer(b, dtype=np.uint8)
+        if a.size > cap:
+            pos = np.random.default_rng(j).choice(a.size - 2, size=cap - 2, replace=False) + 1
+            a = a[np.concatenate(([0], np.sort(pos), [a.size - 1]))]
+        np.save(os.path.join(out_dir, "jpeg_%02d.npy" % j), a.astype(np.float32))
+
+
 def claim_stdout():
     """The contract is ONE JSON line on stdout.  Libraries print there too (NCCL's version banner
     when NCCL_DEBUG is set on the box, warnings of child processes): everything this process and
@@ -363,6 +373,8 @@ def main():
                     help="skip the extra 8K image tiled over all ranks at the end of a batch-mode run")
     ap.add_argument("--tiled-leg-workload", default="gradnoise8k_q95", choices=sorted(WORKLOADS))
     ap.add_argument("--tiled-leg-timeout", type=float, default=900.0)
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="write the JPEGs of the last timed step (rank 0) to DIR as float32 .npy files")
     args = ap.parse_args()
     wl = WORKLOADS[args.workload]
 
@@ -378,7 +390,7 @@ def main():
     lib = gb.load_library()
     global HAVE_CUDA
     HAVE_CUDA = torch.cuda.is_available()
-    rehearsal = lib.gb200_backend_name() != b"cuda-sm_100a"
+    rehearsal = lib.gb200_backend_name() != b"cuda-sm_90a"
     if lib.gb200_device_count() < 1 or (not HAVE_CUDA and not rehearsal):
         raise SystemExit("bench.py: no CUDA device; the product has no CPU fallback")
     if HAVE_CUDA:
@@ -388,7 +400,7 @@ def main():
     if os.path.exists(peaks_path):
         peak, peak_kind = json.load(open(peaks_path))["hbm_gbs"], "measured (MEASURED_PEAKS.json hbm_gbs)"
     else:
-        peak, peak_kind = 6650.0, "fallback (B200_PROFILING.md)"
+        peak, peak_kind = H100_HBM_GBS, "fallback (H100 SXM data sheet)"
 
     if args.mode == "tiled":
         sampler = ClockSampler(local)
@@ -424,6 +436,7 @@ def main():
     px = h * w
     pool = ThreadPoolExecutor(M)
     shas = [set() for _ in range(M)]
+    last_jpeg = [b""] * M  # what the timed path returned for each image in its last step
 
     def encode_host(j):  # reference-facing call: host buffer in, JPEG bytes out
         st = gb.ProcessStats()
@@ -443,6 +456,7 @@ def main():
         if not ok:
             raise RuntimeError(f"gb200_image_process failed on image {j}: {gb.last_error()}")
         shas[j].add(hashlib.sha256(jpeg).hexdigest())
+        last_jpeg[j] = jpeg
         return st
 
     for _ in range(args.warmup):
@@ -469,6 +483,8 @@ def main():
         img.close()
     resident.clear()
     value = world * args.steps * M * px / dt / 1e6
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_jpeg)
 
     # ---- e2e: same job through the reference-facing call with HOST buffers ----
     gdist.barrier(dist, cuda=HAVE_CUDA)
@@ -550,8 +566,7 @@ def main():
         achieved = bpe * top["elements"] / (top["ms"] * 1e-3) / 1e9
         us_per_compare = cmp_ms * 1e3 / compares
         roofline = {"bound": "hbm", "kernel": top["name"], "achieved": achieved, "peak": peak,
-                    "unit": "GB/s", "frac": achieved / peak, "traffic": NCU_TRAFFIC.get(top["name"]),
-                    "peak_source": peak_kind, "avg_launch_us": top["ms"] / max(1, top["launches"]) * 1e3,
+                    "unit": "GB/s", "frac": achieved / peak, "peak_source": peak_kind, "avg_launch_us": top["ms"] / max(1, top["launches"]) * 1e3,
                     "share_of_gpu_time": top["ms"] / gpu_ms if gpu_ms else None,
                     "alg_bytes_per_element": bpe,
                     "measured_on": "one extra image encoded alone (single stream) after the timed region",
@@ -561,7 +576,7 @@ def main():
                         "compulsory_bytes_per_px": 50,
                         "hbm_frac": 50.0 * px / (us_per_compare * 1e-6) / 1e9 / peak if us_per_compare else None,
                         "fp32_issue_frac": (COMPARE_FLOP_PER_PX * px / (us_per_compare * 1e-6)) /
-                                           (148 * 128 * (clocks.get("sm_max_mhz") or 1965.0) * 1e6) if us_per_compare else None,
+                                           (H100_SMS * H100_FP32_LANES * (clocks.get("sm_max_mhz") or H100_MAX_SM_MHZ) * 1e6) if us_per_compare else None,
                         "note": "event times include ~2-5 us of event overhead per launch"}}
     st = stats_list[-1]
     line = {

@@ -1,4 +1,4 @@
-"""guetzli_b200: B200-native (sm_100a) implementation of Guetzli's hot path
+"""guetzli_b200: H100-native (sm_90a) implementation of Guetzli's hot path
 behind Guetzli's own API surface.  See DESIGN.md / INTEGRATION.md.
 
     from guetzli_b200 import Params, ProcessStats, process, butteraugli_score_for_quality

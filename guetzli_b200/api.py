@@ -48,7 +48,7 @@ def load_library(path=None):
     if not os.path.exists(path):
         raise RuntimeError(
             f"guetzli_b200: {path} is missing. Build it with __graft_entry__.build() "
-            "(nvcc, sm_100a); there is no CPU fallback.")
+            "(nvcc, sm_90a); there is no CPU fallback.")
     lib = C.CDLL(path)
     P = C.POINTER
     lib.gb200_butteraugli_score_for_quality.restype = C.c_double

@@ -41,7 +41,7 @@ struct Options {
       "  --nomemlimit - Do not limit memory usage.\n"
       "\n"
       "This build (guetzli_b200) encodes YUV444 only: JPEG input with 4:2:0 chroma\n"
-      "subsampling is refused (\"YUV420 JPEG input is outside the B200 hot path\");\n"
+      "subsampling is refused (\"YUV420 JPEG input is outside the GPU hot path\");\n"
       "convert such files to PNG first.\n";
   const Options defaults;
   fprintf(stderr, kText, defaults.quality, defaults.memlimit_mb);

@@ -1,4 +1,4 @@
-// Launch / memory abstraction shared by the product (CUDA, sm_100a) and the
+// Launch / memory abstraction shared by the product (CUDA, sm_90a) and the
 // CPU restatement (oracle/port, -DGB200_HOSTSIM).  See hd.h.
 //
 //   launch_2d(stream, f, w, h)  : f(x, y) for every 0<=x<w, 0<=y<h
@@ -61,7 +61,9 @@ void d2h(void* dst, const void* src, size_t n, Stream s);  // synchronous
 void d2d(void* dst, const void* src, size_t n, Stream s);
 void dev_zero(void* dst, size_t n, Stream s);
 void stream_sync(Stream s);
-inline const char* backend_name() { return "cuda-sm_100a"; }
+inline const char* backend_name() { return "cuda-sm_90a"; }
+// streaming multiprocessors of the target (H100 SXM); caps grid-stride launches
+constexpr int kTargetSMs = 132;
 
 // launch accounting (gpu_launches in bench.py; per-kernel-name CUDA-event timing)
 void note_launch(const char* name, Stream s, double elements);

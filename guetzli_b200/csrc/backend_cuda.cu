@@ -223,7 +223,7 @@ void select_device(int device) {
   cudaError_t e = cudaGetDeviceCount(&n);
   if (e != cudaSuccess || n == 0) {
     throw std::runtime_error(
-        "guetzli_b200: no CUDA device visible. This library has no CPU fallback; it needs a B200 (sm_100a).");
+        "guetzli_b200: no CUDA device visible. This library has no CPU fallback; it needs an H100 (sm_90a).");
   }
   GB_CUDA(cudaSetDevice(device));
 }

@@ -1,4 +1,4 @@
-// TMA-staged, fused kernels of ButteraugliComparator::Compare (a10) for sm_100a.
+// TMA-staged, fused kernels of ButteraugliComparator::Compare (a10) for sm_90a.
 //
 // Every image-plane stage of the metric is a separable Gaussian blur followed by
 // point-wise arithmetic (b/butteraugli.cc:324-366 opsin, :489-622 frequency split,

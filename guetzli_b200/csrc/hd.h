@@ -1,7 +1,7 @@
 // Host/device portability shims for the single-source kernel bodies.
 //
 // Every arithmetic body of the hot path is written once, as a functor whose
-// operator() is GB_HD.  The product compiles these with nvcc for sm_100a and
+// operator() is GB_HD.  The product compiles these with nvcc for sm_90a and
 // launches them as CUDA kernels (backend_cuda.cuh).  The CPU restatement under
 // oracle/port compiles the very same bodies with g++ (-DGB200_HOSTSIM) and
 // runs them in plain loops; that build is test infrastructure and is never

@@ -154,7 +154,7 @@ struct JpegUnitBits {  // 1D over nblocks * ncomp
 // 64-bit register and leave as whole words with one atomic OR each (the first and
 // last word of a unit are shared with its neighbours; the bits that belong to the
 // neighbours are zero in our word, so OR-ing is safe).  Plain stores for the words in
-// between were measured slower on the B200 (48 vs 37 us per 1080p launch).
+// between were measured slower.
 struct BitCursor {
   unsigned int* words;
   unsigned long long word;  // index of the next word to write

@@ -12,7 +12,7 @@
 //       element <= pivot from the right while they have not crossed, which is what the
 //       two rank lists reproduce.
 // Ranges below a threshold go back to the host replay.  Checked against the host replay on
-// the CPU port and on the B200 (tools/check_device_order.py); GB200_DEVICE_ORDER=0 disables.
+// the CPU port and on the GPU (tools/check_device_order.py); GB200_DEVICE_ORDER=0 disables.
 #pragma once
 #include "hd.h"
 #include "kernels.h"

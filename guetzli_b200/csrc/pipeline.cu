@@ -1,5 +1,5 @@
 // Kernel sequences of the hot path (see pipeline.h).  Compiled by nvcc for
-// sm_100a in the product, and by g++ -DGB200_HOSTSIM for the CPU port.
+// sm_90a in the product, and by g++ -DGB200_HOSTSIM for the CPU port.
 #include "pipeline.h"
 #include "exact_sort.h"
 #include "order_exact.h"
@@ -1864,7 +1864,7 @@ size_t ImageContext::walk_count_below(int direction, float limit) {
 #else
   int ctas = (entries + 256 * 8 - 1) / (256 * 8);
   if (ctas < 1) ctas = 1;
-  if (ctas > 1184) ctas = 1184;
+  if (ctas > 8 * kTargetSMs) ctas = 8 * kTargetSMs;
   note_launch("count_keys_below", s_, entries);
   k_count_keys_below<<<ctas, 256, 0, s_>>>(c, limit, entries, out);
   note_launch_end("count_keys_below", s_);
@@ -1926,7 +1926,7 @@ size_t ImageContext::walk_select_split(int direction, size_t rank_lo, size_t ran
   }
   int ctas = (entries + 256 * 8 - 1) / (256 * 8);
   if (ctas < 1) ctas = 1;
-  if (ctas > 1184) ctas = 1184;  // 148 SMs x 8 resident CTAs
+  if (ctas > 8 * kTargetSMs) ctas = 8 * kTargetSMs;  // 8 resident CTAs per SM
   note_launch("order_key_hist", s_, entries);
   k_order_hist0_keys<<<ctas, 256, 0, s_>>>(c, d_hist_, w_keys_, entries);
   note_launch_end("order_key_hist", s_);

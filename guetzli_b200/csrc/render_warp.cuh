@@ -1,4 +1,4 @@
-// a7 + a9 on sm_100a, one warp per 8x8 block: dequantised coefficients -> IDCT (the
+// a7 + a9 on sm_90a, one warp per 8x8 block: dequantised coefficients -> IDCT (the
 // integer transform of g/idct.cc, shared with the zeroing kernel) -> YCbCr to RGB ->
 // linear light, two pixels per lane.  Same arithmetic as the RenderBlocks functor in
 // kernels.h (one thread per block), which stays the CPU port's version; the dirty-block

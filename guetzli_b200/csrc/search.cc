@@ -1373,7 +1373,7 @@ bool process_resident_impl(const SearchParams& params, ImageContext* ctx, const 
   // grayscale image ignores try_420 and runs force_420 as a one-component pass (set_yuv420_gray).
   const bool gray = (params.force_420 || params.try_420) ? is_grayscale(ctx) : false;
   if (w >= 32 && h >= 32 && (params.force_420 || params.try_420) && !gray) {
-    *err = "guetzli_b200: YUV420 is outside the B200 hot path (DESIGN.md)\n";
+    *err = "guetzli_b200: YUV420 is outside the GPU hot path (DESIGN.md)\n";
     fputs(err->c_str(), stderr);
     return false;
   }
@@ -1443,7 +1443,7 @@ bool process_jpeg(const SearchParams& params, const uint8_t* data, size_t len, i
   if (!check_params(params, err)) return false;
   if (ncomp != 3 || !has_ycbcr_color_space(jpg)) return fail("Only YUV color space input jpeg is supported\n");
   if (!jpg.is_444())
-    return fail("guetzli_b200: YUV420 JPEG input is outside the B200 hot path (DESIGN.md); provide 4:4:4 or PNG\n");
+    return fail("guetzli_b200: YUV420 JPEG input is outside the GPU hot path (DESIGN.md); provide 4:4:4 or PNG\n");
 
   if (!image_size_supported(jpg.width, jpg.height, err)) return false;
   Clock::time_point t0 = Clock::now();

@@ -1,4 +1,4 @@
-// Hand-tiled sm_100a kernels of the STAGED Compare chain (round 1: one kernel per stage).  The
+// Hand-tiled sm_90a kernels of the STAGED Compare chain (round 1: one kernel per stage).  The
 // product runs the TMA-staged fused chain of fused_kernels.cuh; this chain stays in the library
 // behind GB200_COMPARE=staged as the second implementation that the fused one is checked
 // against on the GPU (tests/test_gpu_parity.py::test_fused_matches_staged), and it shares the
@@ -464,7 +464,7 @@ __global__ void __launch_bounds__(256) k_jpeg_hist(const int16_t* cand, const in
 inline void launch_jpeg_hist(Stream s, const int16_t* cand, const int* q, const int* zigzag, unsigned int* out,
                              unsigned int* chroma_nonzero, int nblocks) {
   int ctas = (3 * nblocks + 255) / 256;
-  if (ctas > 592) ctas = 592;  // 148 SMs x 4
+  if (ctas > 4 * kTargetSMs) ctas = 4 * kTargetSMs;
   note_launch("jpeg_hist", s, 3.0 * nblocks);
   k_jpeg_hist<<<ctas, 256, 0, s>>>(cand, q, zigzag, out, chroma_nonzero, nblocks);
   note_launch_end("jpeg_hist", s);
@@ -566,7 +566,7 @@ inline void launch_order_hist(Stream s, const OrderKeyCommon& c, unsigned int* h
                               int level, int entries) {
   int ctas = (entries + 256 * 8 - 1) / (256 * 8);
   if (ctas < 1) ctas = 1;
-  if (ctas > 1184) ctas = 1184;  // 148 SMs x 8 resident CTAs
+  if (ctas > 8 * kTargetSMs) ctas = 8 * kTargetSMs;  // 8 resident CTAs per SM
   note_launch("order_key_hist", s, entries);
   k_order_hist<<<ctas, 256, 0, s>>>(c, hist, st, level, entries);
   note_launch_end("order_key_hist", s);

@@ -1,5 +1,5 @@
 // TMA (cp.async.bulk.tensor) plumbing for the image-plane kernels: tensor maps over
-// float plane groups and the mbarrier / bulk-copy PTX of sm_100a.
+// float plane groups and the mbarrier / bulk-copy PTX of sm_90a.
 //
 // A plane group [n][h][pitch] is described to the TMA unit as a rank-3 tensor with
 // extents {w, h, n}: the TRUE width w, so that a box reaching past the image (x < 0,

@@ -1,4 +1,4 @@
-// a13/a14 on sm_100a: one warp per 8x8 block runs the whole greedy zeroing loop of
+// a13/a14 on sm_90a: one warp per 8x8 block runs the whole greedy zeroing loop of
 // Processor::ComputeBlockZeroingOrder (g/processor.cc:364-467) with every per-pixel /
 // per-transform step of CompareBlock (g/butteraugli_comparator.cc:457-488) spread
 // over the 32 lanes and all block state in shared memory.  Same helper arithmetic

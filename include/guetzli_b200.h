@@ -1,4 +1,4 @@
-/* guetzli_b200 -- C ABI of the B200-native Guetzli hot path.
+/* guetzli_b200 -- C ABI of the H100-native Guetzli hot path.
  *
  * Drop-in boundary: the reference's public entry point for this path is the
  * C++ free function
@@ -18,7 +18,7 @@
  * 0 = failure with gb200_last_error() set (thread-local), no exceptions across
  * the ABI, one image context = one host thread + one CUDA stream.
  * There is NO CPU fallback: every entry point that computes fails when no CUDA
- * device (sm_100a) is present.
+ * device (sm_90a) is present.
  */
 #ifndef GUETZLI_B200_H_
 #define GUETZLI_B200_H_
@@ -110,7 +110,7 @@ int gb200_process_rgb_tiled_threads(const gb200_params* params, const uint8_t* r
 
 void gb200_free(void* p);
 const char* gb200_last_error(void);
-const char* gb200_backend_name(void); /* "cuda-sm_100a" for the product library */
+const char* gb200_backend_name(void); /* "cuda-sm_90a" for the product library */
 int gb200_device_count(void);
 
 /* ---- device-resident stages (Comparator seam on device memory) ---------- */

@@ -1,6 +1,8 @@
 """Stage-by-stage and end-to-end parity checks shared by the CPU-port tests
 (oracle pinning) and the GPU tests (product vs oracle).  `lib` is a C-ABI
-library handle (product or port); `ref` is tests/reflib (the real reference)."""
+library handle (product or port); `ref` is tests/reflib (the real reference or its recorded answers).  The reference's
+outputs are compared, never computed on: where a stage's input is the previous stage's
+output, the library's own output, once checked equal to the reference's, is fed on."""
 import hashlib
 import json
 import os
@@ -8,6 +10,7 @@ import os
 import numpy as np
 
 import guetzli_b200 as gb
+import reflib
 from guetzli_b200 import synth
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -20,9 +23,17 @@ BLUR_SPECS = [(1.2, 0.0), (7.46953768697, -0.00457628248637), (3.734768843485, -
 
 
 def bits_equal(a, b):
+    """Same float32 bit patterns; `b` may be a recorded reference output (reflib.Digest)."""
     a = np.ascontiguousarray(a, dtype=np.float32)
+    if isinstance(b, reflib.Digest):
+        return b.dtype == a.dtype.str and b.matches(a)
     b = np.ascontiguousarray(b, dtype=np.float32)
     return a.shape == b.shape and np.array_equal(a.view(np.uint32), b.view(np.uint32))
+
+
+def same(a, b):
+    """np.array_equal(a, b); `b` may be a recorded reference output (reflib.Digest)."""
+    return b.matches(a) if isinstance(b, reflib.Digest) else np.array_equal(a, b)
 
 
 def gray(h, w, seed):
@@ -59,14 +70,13 @@ def check_integer_stages(lib, ref, rgb):
     """a2 FDCT, a8 quantise, a7+a9 render: bit-exact integers / float LUT values."""
     h, w, _ = rgb.shape
     img = gb.DeviceImage(rgb, lib=lib)
-    ref_c = ref.rgb_to_coeffs(rgb)
-    assert np.array_equal(img.orig_coeffs(), ref_c), "FDCT coefficients differ"
+    coeffs = img.orig_coeffs()
+    assert same(coeffs, ref.rgb_to_coeffs(rgb)), "FDCT coefficients differ"
     q = test_quant(1)
-    cq = ref.apply_global_quant(ref_c, w, h, q)
     img.apply_global_quant(q)
-    assert np.array_equal(img.download_candidate(), cq), "global quantisation differs"
-    _, lin = ref.render(cq, w, h)
-    assert bits_equal(img.debug_render(), lin), "rendered linear RGB differs"
+    cq = img.download_candidate()
+    assert same(cq, ref.apply_global_quant(coeffs, w, h, q)), "global quantisation differs"
+    assert bits_equal(img.debug_render(), ref.render(cq, w, h)[1]), "rendered linear RGB differs"
     img.close()
 
 
@@ -78,10 +88,13 @@ def check_butteraugli_stages(lib, ref, rgb):
     plane = (rng.random((h, w), dtype=np.float32) * 255).astype(np.float32)
     for i, (s, b) in enumerate(BLUR_SPECS):
         assert bits_equal(img.debug_blur(plane, i), ref.blur(plane, s, b)), f"blur {i} differs"
-    _, lin = ref.render(ref.rgb_to_coeffs(rgb), w, h)
-    xyb_ref = ref.opsin(lin)
-    assert bits_equal(img.debug_opsin(lin), xyb_ref), "opsin differs"
-    assert bits_equal(img.debug_separate(xyb_ref), ref.separate(xyb_ref)), "frequency split differs"
+    coeffs = img.orig_coeffs()
+    assert same(coeffs, ref.rgb_to_coeffs(rgb)), "FDCT coefficients differ"
+    lin = img.debug_render()
+    assert bits_equal(lin, ref.render(coeffs, w, h)[1]), "rendered linear RGB differs"
+    xyb = img.debug_opsin(lin)
+    assert bits_equal(xyb, ref.opsin(lin)), "opsin differs"
+    assert bits_equal(img.debug_separate(xyb), ref.separate(xyb)), "frequency split differs"
     img.close()
 
 
@@ -89,29 +102,29 @@ def check_compare_and_blocks(lib, ref, rgb, target=0.9):
     """a10 Compare (distmap + distance), a13 masks, a15 weights, a14 zeroing orders, a11 JPEG bytes."""
     h, w, _ = rgb.shape
     img = gb.DeviceImage(rgb, lib=lib)
-    ref_c = ref.rgb_to_coeffs(rgb)
+    coeffs = img.orig_coeffs()
+    assert same(coeffs, ref.rgb_to_coeffs(rgb)), "FDCT coefficients differ"
     q = test_quant(2)
-    cq = ref.apply_global_quant(ref_c, w, h, q)
     img.apply_global_quant(q)
+    cq = img.download_candidate()
+    assert same(cq, ref.apply_global_quant(coeffs, w, h, q)), "global quantisation differs"
     dist = img.compare()
     rdm, rdist = ref.compare_coeffs(rgb, cq, target)
     assert dist == rdist, f"distance {dist} vs {rdist}"
-    assert bits_equal(img.distmap(), rdm), "distmap differs"
-    rm = ref.block_mask(rgb)
-    rmc = np.stack([rm[c][::8, ::8].reshape(-1) for c in range(3)], axis=1)
-    assert bits_equal(img.debug_corner_mask(), rmc), "block-corner mask differs"
+    dm = img.distmap()
+    assert bits_equal(dm, rdm), "distmap differs"
+    assert bits_equal(img.debug_corner_mask(), ref.block_mask_corners(rgb)), "block-corner mask differs"
     for d, r, z in [(1, 1, True), (1, 2, False), (-1, 1, False), (-1, 4, False)]:
         mine = img.block_weights(d, r, target * 1.0, z)
-        theirs = ref.block_weights(w, h, target, d, r, 1.0, np.zeros_like(rdm) if z else rdm)
-        assert np.array_equal(mine, theirs), f"block weights differ (dir {d}, r {r})"
+        theirs = ref.block_weights(w, h, target, d, r, 1.0, np.zeros_like(dm) if z else dm)
+        assert same(mine, theirs), f"block weights differ (dir {d}, r {r})"
     idx, err, cnt = img.zeroing_orders(target, 3)
-    roffs, ridx, rerr = ref.zeroing_orders(rgb, ref_c, q, target)
-    assert np.array_equal(cnt, np.diff(roffs)), "zeroing-order list lengths differ"
-    for b in range(img.nblocks):
-        n = cnt[b]
-        assert np.array_equal(idx[b, :n], ridx[roffs[b]:roffs[b + 1]]), f"block {b}: order differs"
-        assert bits_equal(err[b, :n], rerr[roffs[b]:roffs[b + 1]]), f"block {b}: errors differ"
-    assert gb.write_jpeg(cq, w, h, q, lib=lib) == ref.write_jpeg(ref_c, w, h, q), "JPEG bytes differ"
+    roffs, ridx, rerr = ref.zeroing_orders(rgb, coeffs, q, target)
+    offs = np.concatenate(([0], np.cumsum(cnt))).astype(np.int32)
+    assert same(offs, roffs), "zeroing-order list lengths differ"
+    assert same(np.concatenate([idx[b, :cnt[b]] for b in range(img.nblocks)]), ridx), "zeroing orders differ"
+    assert bits_equal(np.concatenate([err[b, :cnt[b]] for b in range(img.nblocks)]), rerr), "zeroing errors differ"
+    assert gb.write_jpeg(cq, w, h, q, lib=lib) == ref.write_jpeg(coeffs, w, h, q), "JPEG bytes differ"
     img.close()
 
 
@@ -145,6 +158,7 @@ def check_process_vs_ref(lib, ref, rgb, quality, lookahead=3, new_zeroing_model=
                                                   new_zeroing_model=new_zeroing_model)
     assert ok == rok
     if trace != rtrace:
+        assert isinstance(rtrace, str), "verbose trace differs from the recorded one"
         a, b = trace.split("\n"), rtrace.split("\n")
         for i, (x, y) in enumerate(zip(a, b)):
             assert x == y, f"trace line {i}:\n  mine: {x}\n  ref : {y}"

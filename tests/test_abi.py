@@ -25,7 +25,7 @@ def test_product_library_exports_declared_abi():
     for n in names:
         assert hasattr(lib, n), f"{n} declared in include/guetzli_b200.h but not exported"
     lib.gb200_backend_name.restype = ctypes.c_char_p
-    assert lib.gb200_backend_name() == b"cuda-sm_100a"
+    assert lib.gb200_backend_name() == b"cuda-sm_90a"
 
 
 def test_product_has_no_cpu_fallback():

@@ -8,6 +8,7 @@ import os
 import pytest
 
 import guetzli_b200 as gb
+import parity
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 GOLDEN = json.load(open(os.path.join(HERE, "golden", "golden_jpeg.json")))
@@ -74,7 +75,7 @@ def test_reader_differential_on_damaged_files(port_lib, ref, name):
         assert ok == rok, (name, t)
         if ok:
             accepted += 1
-            assert dims == rdims and np.array_equal(coeffs, rcoeffs), (name, t)
+            assert dims == list(rdims) and parity.same(coeffs, rcoeffs), (name, t)
     assert accepted > 0
 
 
@@ -87,8 +88,8 @@ def test_reference_reproduces_jpeg_golden(ref):
     for name in ("prog444_q85", "meta_kept", "tiny444", "gray"):
         g = GOLDEN[name]
         ok, jpeg, trace, counters = ref.process_jpeg(fixture(name), g["quality"], clear_metadata=g["clear_metadata"])
-        assert ok == g["ok"] and hashlib.sha256(jpeg).hexdigest() == g["jpeg_sha256"]
-        assert hashlib.sha256(trace.encode()).hexdigest() == g["trace_sha256"] and counters == g["iterations"]
+        assert ok == g["ok"] and ref.sha256_matches(jpeg, g["jpeg_sha256"])
+        assert ref.sha256_matches(trace, g["trace_sha256"]) and list(counters) == g["iterations"]
 
 
 def test_rgb_input_without_metadata_stripping(port_lib, ref):
@@ -98,11 +99,7 @@ def test_rgb_input_without_metadata_stripping(port_lib, ref):
     rgb = synth.gradnoise(40, 48, 3)
     p = gb.Params(butteraugli_target=gb.butteraugli_score_for_quality(90, lib=port_lib), clear_metadata=False)
     ok, jpeg = gb.process(p, None, rgb, 48, 40, lib=port_lib)
-    ref.lib().gref_set_clear_metadata(0)
-    try:
-        rok, rjpeg, _, _, _ = ref.process_rgb(rgb, 90)
-    finally:
-        ref.lib().gref_set_clear_metadata(1)
+    rok, rjpeg, _, _, _ = ref.process_rgb(rgb, 90, clear_metadata=False)
     assert ok and rok and rjpeg == jpeg and jpeg[2:4] == b"\xff\xe0"
 
 
