@@ -16,7 +16,9 @@
 //  * the point-wise stage that consumes a blur runs in the y pass's epilogue on the
 //    values still in registers (Epi functors below), instead of as its own kernel
 //    over planes in HBM;
-//  * blurs of radius <= 5 do x and y in one kernel from one tile.
+//  * blurs of radius <= 5 do x and y in one kernel from one tile;
+//  * the lf and mf blurs roll a window down a column strip (k_roll_blur): the x pass goes
+//    to a shared-memory ring of rows instead of a plane in HBM.
 //
 // Border outputs (fewer than r samples to an image edge) use the raw taps and the
 // per-position scale of ConvolveBorderColumn (b/butteraugli.cc:156-181); tiles that
@@ -143,14 +145,6 @@ __device__ __forceinline__ void blur_x_tile(float* tile, uint64_t* bar, const CU
   }
 }
 
-template <int R>
-__global__ void __launch_bounds__(128) k_tma_blur_x(const __grid_constant__ CUtensorMap in_map, float* out,
-                                                    const float* scale_x, PlaneGeom g, BlurK<R> k) {
-  __shared__ __align__(128) float tile[GBX_TH * BlurXCfg<R>::SW];
-  __shared__ __align__(8) uint64_t bar;
-  blur_x_tile<R>(tile, &bar, &in_map, out, scale_x, g, k, blockIdx.z);
-}
-
 // Four single-plane x passes with different kernels in one launch (blockIdx.z picks the blur):
 // the noise blur and the three mask blurs all become ready after hf_fused / mask_pre, and each
 // alone is a one-wave launch whose ramp and tail cost as much as its arithmetic.
@@ -233,39 +227,6 @@ __global__ void __launch_bounds__(256, NP == 1 ? 3 : 2) k_tma_blur_y(const __gri
     }
   }
   constexpr int CH = Epi::kChunk;
-  if (NP > 1) {
-    // Multi-plane epilogues are long (EpiMf: two Malta pre-passes per pixel): 16 unrolled copies
-    // do not fit the instruction cache.  The blurred values go back to shared memory (over the
-    // input tiles, dead once every thread has finished its passes; each thread reads only its own
-    // slots again) and the epilogue becomes a rolled loop over chunks.
-    static_assert(NP == 1 || GBY_G * 256 <= (GBY_TH + 2 * R) * GBY_TW, "stash must fit in the tiles");
-    __syncthreads();
-    float* stash = dyn_smem + threadIdx.x;  // [NP][GBY_G][256]
-#pragma unroll
-    for (int p = 0; p < NP; ++p)
-#pragma unroll
-      for (int o = 0; o < GBY_G; ++o) stash[(p * GBY_G + o) * 256] = res[p][o];
-    if (x >= g.w) return;
-#pragma unroll 1
-    for (int o0 = 0; o0 < GBY_G; o0 += CH) {
-      typename Epi::Pre pre[CH];
-#pragma unroll
-      for (int i = 0; i < CH; ++i) {
-        const int y = yg + o0 + i;
-        if (y < g.y_end) epi.load(x, y, pz, pre[i]);
-      }
-#pragma unroll
-      for (int i = 0; i < CH; ++i) {
-        const int y = yg + o0 + i;
-        if (y >= g.y_end) continue;
-        float v[NP];
-#pragma unroll
-        for (int p = 0; p < NP; ++p) v[p] = stash[(p * GBY_G + o0 + i) * 256];
-        epi.apply(x, y, pz, v, pre[i]);
-      }
-    }
-    return;
-  }
   if (x >= g.w) return;
   // Epilogue in chunks: first every global operand of the chunk's pixels (read-only path,
   // all loads in flight together), then the arithmetic and the stores.
@@ -285,6 +246,183 @@ __global__ void __launch_bounds__(256, NP == 1 ? 3 : 2) k_tma_blur_y(const __gri
 #pragma unroll
       for (int p = 0; p < NP; ++p) v[p] = res[p][o0 + i];
       epi.apply(x, y, pz, v, pre[i]);
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------
+// Rolling-window separable blur (large radii): x and y pass in one kernel, the x pass
+// never leaves shared memory.  A CTA (128 threads) owns a GBR_TW-column strip of a
+// segment of `seg` output rows [ys, ye) and walks it top to bottom in steps of GBR_CH rows:
+//
+//   chunk c   = input rows [ys - R + c*CH, +CH) with their x halo, one TMA box per plane,
+//               in NS stages (one mbarrier each; the load of chunk c + NS is issued as soon
+//               as the x pass of chunk c is done)
+//   x pass    of chunk c -> ring position c % (RING / CH) of the x-output ring, with rows
+//               0 .. 2R-1 of the ring also written at RING + i, so that every window of
+//               CH + 2R ring rows is contiguous (stream_y's immediate-offset loads)
+//   y pass    of step b = c - D (output rows [ys + b*CH, +CH)) from the ring; warp w owns
+//               rows w*G .. w*G + G-1, lane = column; then the epilogue on the registers.
+//
+// D = ceil(2R / CH) chunks of look-ahead.  A ring of D + 2 chunks means the x pass of chunk
+// c + 1 never overwrites rows the y pass of step c - D reads (one barrier per step); a ring of
+// D + 1 chunks needs a second barrier (RollCfg::kLean).  The only recomputation is the D
+// chunks of x rows above each segment.  Rows outside the image are zero-filled by the TMA
+// unit (or, for chunks wholly below the image, written as zeros), so their x outputs are +0,
+// as the y kernels' zero fill made them.
+#define GBR_TW 32
+#define GBR_CH 32
+#define GBR_G 8    // 4 warps x 8 rows = GBR_CH
+#define GBR_SEG 288  // target segment length: 4 segments of 1080 rows, recompute D*CH rows each
+
+template <int R, int NP>
+struct RollCfg {
+  static constexpr int SW = GBR_TW - 4 + 4 * XTile<R>::NQ;  // input box width
+  static constexpr int D = (2 * R + GBR_CH - 1) / GBR_CH;
+  // Multi-plane (lean): one input stage and a ring of D + 1 chunks, so that four CTAs fit on
+  // an SM; paid with a second barrier per step (the next x pass overwrites the rows the
+  // current y pass reads).  Single plane: two stages, D + 2 chunks, one barrier per step.
+  static constexpr bool kLean = NP > 1;
+  static constexpr int NS = kLean ? 1 : 2;
+  static constexpr int RING = (D + (kLean ? 1 : 2)) * GBR_CH;
+  static constexpr int RBUF = RING + 2 * R;  // ring rows incl. the wrap copy
+  static constexpr int kStageFloats = NP * GBR_CH * SW;
+  static constexpr int kRingFloats = NP * RBUF * GBR_TW;
+  static constexpr size_t kSmemBytes = (NS * kStageFloats + kRingFloats) * sizeof(float) + 16;
+  static_assert(SW <= 256 && SW % 4 == 0, "TMA box width");
+  static_assert((GBR_CH * SW * 4) % 128 == 0, "TMA destinations must be 128-byte aligned");
+};
+
+// x pass of one staged chunk (NP planes of CH rows) into ring rows [row0, row0 + CH) of each plane
+template <int R, int NP>
+__device__ __forceinline__ void roll_x_chunk(const float* st, float* ring, int row0, bool live, bool edge_x, int x0,
+                                             const float* scale_x, int w, const BlurK<R>& k) {
+  typedef RollCfg<R, NP> C;
+  constexpr int SLOTS = GBR_TW / 4;
+#pragma unroll 1
+  for (int i = threadIdx.x; i < NP * GBR_CH * SLOTS; i += 128) {
+    const int slot = i % SLOTS, prow = i / SLOTS;  // prow = p * CH + r
+    const int p = prow / GBR_CH, r = prow % GBR_CH;
+    float acc[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+    if (live) {
+      const float* s = st + prow * C::SW + 4 * slot;
+      stream_x4<R, false>(s, k, acc);
+      if (edge_x) {
+        float raw[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+        stream_x4<R, true>(s, k, raw);
+#pragma unroll
+        for (int o = 0; o < 4; ++o) {
+          const int x = x0 + 4 * slot + o;
+          // columns beyond the image only feed outputs that are never stored
+          if (x < w && (x < R || x + R >= w)) acc[o] = raw[o] * scale_x[x];
+        }
+      }
+    }
+    const int rr = row0 + r;
+    float* d = ring + (p * C::RBUF + rr) * GBR_TW + 4 * slot;
+    const float4 v = make_float4(acc[0], acc[1], acc[2], acc[3]);
+    *reinterpret_cast<float4*>(d) = v;
+    if (rr < 2 * R) *reinterpret_cast<float4*>(d + C::RING * GBR_TW) = v;
+  }
+}
+
+// y pass of G rows of one column from the ring; s points at the window's first row
+template <int R>
+__device__ __forceinline__ void roll_y(const float* s, const BlurK<R>& k, const float* scale_y, int yg, int h,
+                                       float res[GBR_G]) {
+#pragma unroll
+  for (int o = 0; o < GBR_G; ++o) res[o] = 0.0f;
+  stream_y<R, GBR_G, GBR_TW, false>(s, k, res);
+  if ((yg < R) || (yg + GBR_G + R > h)) {  // warp-uniform: some row of this group takes the border rule
+    float raw[GBR_G];
+#pragma unroll
+    for (int o = 0; o < GBR_G; ++o) raw[o] = 0.0f;
+    stream_y<R, GBR_G, GBR_TW, true>(s, k, raw);
+#pragma unroll
+    for (int o = 0; o < GBR_G; ++o) {
+      const int y = yg + o;
+      if (y < h && (y < R || y + R >= h)) res[o] = raw[o] * scale_y[y];
+    }
+  }
+}
+
+// NP planes blurred by the same thread and handed to the epilogue as v[NP] per pixel
+// (NP == 1: blockIdx.z picks the plane).  grid (ceil(w / TW), ceil(rows / seg), NP == 1 ? planes : 1).
+template <int R, int NP, class Epi>
+__global__ void __launch_bounds__(128) k_roll_blur(const __grid_constant__ CUtensorMap in_map, const float* scale_x,
+                                                   const float* scale_y, PlaneGeom g, int seg, BlurK<R> k, Epi epi) {
+  typedef RollCfg<R, NP> C;
+  constexpr int D = C::D, RP = XTile<R>::RP, NS = C::NS, NPOS = C::RING / GBR_CH;
+  extern __shared__ __align__(128) float dyn_smem[];
+  float* stage = dyn_smem;                        // [NS][NP][CH][SW]
+  float* ring = dyn_smem + NS * C::kStageFloats;  // [NP][RBUF][TW]
+  uint64_t* bar = reinterpret_cast<uint64_t*>(ring + C::kRingFloats);
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, pz = blockIdx.z;
+  const int x0 = blockIdx.x * GBR_TW, x = x0 + lane;
+  const int ys = g.y0 + blockIdx.y * seg;
+  const int ye = min(ys + seg, g.y_end);
+  const int nsteps = (ye - ys + GBR_CH - 1) / GBR_CH, nchunks = nsteps + D;
+  const int yin = ys - R;  // first input row of chunk 0
+  // chunks that start below the image are not loaded (their rows are zeros)
+  const int nlive = min(nchunks, (g.h - yin + GBR_CH - 1) / GBR_CH);
+  if (tid == 0) {
+    mbar_init(&bar[0], 1);
+    mbar_init(&bar[1], 1);
+    mbar_fence_init();
+  }
+  __syncthreads();
+  if (tid == 0) {
+    for (int c = 0; c < NS && c < nlive; ++c) {
+      mbar_expect_tx(&bar[c], C::kStageFloats * 4);
+#pragma unroll
+      for (int p = 0; p < NP; ++p)
+        tma_load_box(stage + c * C::kStageFloats + p * GBR_CH * C::SW, &in_map, &bar[c], x0 - RP, yin + c * GBR_CH,
+                     NP == 1 ? pz : p);
+    }
+  }
+  const bool edge_x = (x0 < R) || (x0 + GBR_TW + R > g.w);
+#pragma unroll 1
+  for (int c = 0; c < nchunks; ++c) {
+    const int sidx = c % NS;
+    const bool live = c < nlive;
+    if (C::kLean && c > 0) __syncthreads();  // the y pass of the previous step is done with its rows
+    if (live) mbar_wait(&bar[sidx], (c / NS) & 1);
+    roll_x_chunk<R, NP>(stage + sidx * C::kStageFloats, ring, (c % NPOS) * GBR_CH, live, edge_x, x0, scale_x, g.w, k);
+    __syncthreads();  // ring rows of chunk c complete; stage sidx free
+    if (tid == 0 && c + NS < nlive) {
+      mbar_expect_tx(&bar[sidx], C::kStageFloats * 4);
+#pragma unroll
+      for (int p = 0; p < NP; ++p)
+        tma_load_box(stage + sidx * C::kStageFloats + p * GBR_CH * C::SW, &in_map, &bar[sidx], x0 - RP,
+                     yin + (c + NS) * GBR_CH, NP == 1 ? pz : p);
+    }
+    if (c < D) continue;
+    const int b = c - D;
+    const int yg = ys + b * GBR_CH + GBR_G * warp;
+    const float* win = ring + ((b % NPOS) * GBR_CH + GBR_G * warp) * GBR_TW + lane;
+    float res[NP][GBR_G];
+#pragma unroll
+    for (int p = 0; p < NP; ++p) roll_y<R>(win + p * C::RBUF * GBR_TW, k, scale_y, yg, g.h, res[p]);
+    if (x >= g.w) continue;
+    // Epilogue: first every global operand of the G pixels (read-only path, all loads in
+    // flight together), then the arithmetic and the stores.  One copy of G = 8 pixels is in
+    // the instruction stream, inside the rolled step loop: as small as the rolled 8-pixel
+    // chunks of the former multi-plane y kernel, so EpiMf's long epilogue fits the cache.
+    static_assert(Epi::kChunk >= GBR_G, "the epilogue takes the G pixels of a thread in one chunk");
+    typename Epi::Pre pre[GBR_G];
+#pragma unroll
+    for (int o = 0; o < GBR_G; ++o) {
+      const int y = yg + o;
+      if (y < ye) epi.load(x, y, pz, pre[o]);
+    }
+#pragma unroll
+    for (int o = 0; o < GBR_G; ++o) {
+      const int y = yg + o;
+      if (y >= ye) continue;
+      float v[NP];
+#pragma unroll
+      for (int p = 0; p < NP; ++p) v[p] = res[p][o];
+      epi.apply(x, y, pz, v, pre[o]);
     }
   }
 }
@@ -478,12 +616,15 @@ struct EpiMf {
     const float hy = p.iny - mby;
     const float mfx = remove_range_around_zero(static_cast<float>(0.120079806822), mbx);
     const float mfy = amplify_range_around_zero(static_cast<float>(0.03430529365), mby);
-    ps[kMfX * plane + o] = mfx;
-    ps[kMfY * plane + o] = mfy;
-    ps[kMfB * plane + o] = v[2];
     hf_raw[o] = suppress_x_by_y(hx, hy);
     hf_raw[plane + o] = hy;
-    if (ps0 != nullptr) {
+    // the candidate's mf planes are consumed here (Malta pre-pass) and nowhere else: stored
+    // only when building a full PsychoImage
+    if (ps0 == nullptr) {
+      ps[kMfX * plane + o] = mfx;
+      ps[kMfY * plane + o] = mfy;
+      ps[kMfB * plane + o] = v[2];
+    } else {
       diffs[2 * plane + o] = malta_diff(p.p0x, mfx, mp_x);
       diffs[5 * plane + o] = malta_diff(p.p0y, mfy, mp_y);
     }
@@ -552,7 +693,8 @@ struct EpiHf {
     uhfy = maximum_clamp(uhfy, static_cast<float>(5.8907152736));
     uhfy = suppress_in_bright_areas(uhfy, lfy, kMulSuppressUhf, kRegUhf);
     hfy = suppress_in_bright_areas(hfy, lfy, kMulSuppressHf, kRegHf);
-    ps[kUhfX * plane + o] = uhfx;
+    // against the original (ps0 given), uhf[X] and lf[Y] of the candidate are consumed here
+    // only; k_mask_pre reads hf[X], uhf[Y], hf[Y], the noise epilogue hf[Y], the combine lf[X], lf[B]
     ps[kHfX * plane + o] = hfx;
     ps[kUhfY * plane + o] = uhfy;
     ps[kHfY * plane + o] = hfy;
@@ -563,8 +705,10 @@ struct EpiHf {
     const float bb = lfb + y_to_b_mul * lfy;
     ps[kLfB * plane + o] = bb * bmul;
     ps[kLfX * plane + o] = lfx * xmul;
-    ps[kLfY * plane + o] = lfy * ymul;
-    if (ps0 != nullptr) {
+    if (ps0 == nullptr) {
+      ps[kUhfX * plane + o] = uhfx;
+      ps[kLfY * plane + o] = lfy * ymul;
+    } else {
       const float h0y = p.h0y;
       diffs[0 * plane + o] = malta_diff(p.u0x, uhfx, mp_uhf_x);
       diffs[1 * plane + o] = malta_diff(p.h0x, hfx, mp_hf_x);

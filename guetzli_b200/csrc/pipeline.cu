@@ -163,16 +163,23 @@ void allow_smem(K kernel, size_t bytes) {
 
 inline int cdiv(int a, int b) { return (a + b - 1) / b; }
 
-// x pass of `nplanes` planes: in -> out
-template <int R>
-void launch_tma_x(Stream s, const CUtensorMap& in_map, float* out, int nplanes, const BlurTab& tab, const PlaneGeom& pg,
-                  const HostTables& ht, int id) {
+// Rolling-window blur of a plane group with epilogue (k_roll_blur); `in_map` has boxes of
+// RollCfg<R, NP>::SW x GBR_CH.  The launch's rows are cut into segments of whole steps of
+// about GBR_SEG rows.
+template <int R, int NP, class Epi>
+void launch_roll(Stream s, const CUtensorMap& in_map, int planes_z, const BlurTab& tab, const PlaneGeom& pg,
+                 const HostTables& ht, int id, const Epi& epi, const char* name) {
   const int rows = pg.y_end - pg.y0;
   if (rows <= 0) return;
-  dim3 grid(cdiv(pg.w, GBX_TW), cdiv(rows, GBX_TH), nplanes);
-  note_launch("tma_blur_x", s, static_cast<double>(pg.w) * rows * nplanes);
-  k_tma_blur_x<R><<<grid, 128, 0, s>>>(in_map, out, tab.scale_x, pg, make_blurk<R>(ht, id));
-  note_launch_end("tma_blur_x", s);
+  typedef RollCfg<R, NP> C;
+  allow_smem(k_roll_blur<R, NP, Epi>, C::kSmemBytes);
+  const int nseg = cdiv(rows, GBR_SEG);
+  const int seg = cdiv(cdiv(rows, nseg), GBR_CH) * GBR_CH;
+  dim3 grid(cdiv(pg.w, GBR_TW), cdiv(rows, seg), planes_z);
+  note_launch(name, s, static_cast<double>(pg.w) * rows * (NP == 1 ? planes_z : NP));
+  k_roll_blur<R, NP, Epi><<<grid, 128, C::kSmemBytes, s>>>(in_map, tab.scale_x, tab.scale_y, pg, seg,
+                                                           make_blurk<R>(ht, id), epi);
+  note_launch_end(name, s);
 }
 
 template <int R, int NP, class Epi>
@@ -226,11 +233,10 @@ void ImageContext::fused_separate(const float* xyb, float* ps, bool with_diffs) 
   const PlaneGeom pg{g_.w, g_.h, g_.pitch, g_.plane, cr_lo_, cr_hi_};
   const size_t P = g_.plane;
   // S2: lf = Blur(xyb, 7.47); mf_in = xyb - lf
-  launch_tma_x<GB_R_LF>(s_, fused_->map(xyb, 3, BlurXCfg<GB_R_LF>::SW, GBX_TH, g_), tmp_, 3, t_.blur[kBlurLf], pg, ht_, kBlurLf);
-  launch_tma_y<GB_R_LF, 1>(s_, fused_->map(tmp_, 3, GBY_TW, GBY_TH + 2 * GB_R_LF, g_), 3, t_.blur[kBlurLf], pg, ht_, kBlurLf,
-                           EpiLf{xyb, lf_, mf_in_, g_.pitch, P}, "lf_fused_y");
+  // (launch names are those of the former y-pass kernels, which these replace)
+  launch_roll<GB_R_LF, 1>(s_, fused_->map(xyb, 3, RollCfg<GB_R_LF, 1>::SW, GBR_CH, g_), 3, t_.blur[kBlurLf], pg, ht_, kBlurLf,
+                          EpiLf{xyb, lf_, mf_in_, g_.pitch, P}, "lf_fused_y");
   // S3 + S4: mf = Blur(mf_in, 3.73); split, range tweaks, SuppressXByY (+ Malta pre-pass of the mf bands)
-  launch_tma_x<GB_R_MF>(s_, fused_->map(mf_in_, 3, BlurXCfg<GB_R_MF>::SW, GBX_TH, g_), tmp_, 3, t_.blur[kBlurMf], pg, ht_, kBlurMf);
   EpiMf em;
   em.mf_in = mf_in_;
   em.ps = ps;
@@ -241,8 +247,8 @@ void ImageContext::fused_separate(const float* xyb, float* ps, bool with_diffs) 
   em.mp_y = malta_[4];
   em.pitch = g_.pitch;
   em.plane = P;
-  launch_tma_y<GB_R_MF, 3>(s_, fused_->map(tmp_, 3, GBY_TW, GBY_TH + 2 * GB_R_MF, g_), 1, t_.blur[kBlurMf], pg, ht_, kBlurMf, em,
-                           "mf_fused_y");
+  launch_roll<GB_R_MF, 3>(s_, fused_->map(mf_in_, 3, RollCfg<GB_R_MF, 3>::SW, GBR_CH, g_), 1, t_.blur[kBlurMf], pg, ht_, kBlurMf,
+                          em, "mf_fused_y");
   // S5 + S6: hf = Blur(hf_raw, 1.87) in one kernel; uhf / hf / lf "vals" (+ Malta pre-pass, noise difference)
   EpiHf eh;
   eh.lf_raw = lf_;
@@ -275,11 +281,10 @@ void ImageContext::fused_sup0() {
 void ImageContext::fused_blur(const float* in, float* out, int nplanes, int id) {
   const PlaneGeom pg{g_.w, g_.h, g_.pitch, g_.plane, cr_lo_, cr_hi_};
   const EpiStore st{out, g_.pitch, g_.plane};
-#define GB_BLUR_CASE(R)                                                                                              \
-  case R:                                                                                                            \
-    launch_tma_x<R>(s_, fused_->map(in, nplanes, BlurXCfg<R>::SW, GBX_TH, g_), tmp_, nplanes, t_.blur[id], pg, ht_, id); \
-    launch_tma_y<R, 1>(s_, fused_->map(tmp_, nplanes, GBY_TW, GBY_TH + 2 * R, g_), nplanes, t_.blur[id], pg, ht_, id, st, \
-                       "tma_blur_y");                                                                              \
+#define GB_BLUR_CASE(R)                                                                                               \
+  case R:                                                                                                             \
+    launch_roll<R, 1>(s_, fused_->map(in, nplanes, RollCfg<R, 1>::SW, GBR_CH, g_), nplanes, t_.blur[id], pg, ht_, id, st, \
+                      "tma_blur_y");                                                                                  \
     break;
   switch (t_.blur[id].r) {
     GB_BLUR_CASE(2)
