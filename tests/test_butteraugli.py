@@ -86,7 +86,7 @@ def test_port_cli(port_lib, ref, tmp_path):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("h,w", SIZES + [(300, 411)])
+@pytest.mark.parametrize("h,w", SIZES + [(300, 411), (577, 70), (1080, 100)])
 def test_cuda_diffmap_matches_reference(cuda_lib, ref, h, w):
     check_api(cuda_lib, ref, h, w)
 

@@ -23,7 +23,7 @@ def test_butteraugli_stages(cuda_lib, ref, h, w, seed):
     parity.check_butteraugli_stages(cuda_lib, ref, synth.gradnoise(h, w, seed))
 
 
-@pytest.mark.parametrize("h,w,seed", SIZES + [(40, 33, 2)])
+@pytest.mark.parametrize("h,w,seed", SIZES + [(40, 33, 2), (577, 70, 9)])
 def test_compare_and_block_kernels(cuda_lib, ref, h, w, seed):
     parity.check_compare_and_blocks(cuda_lib, ref, synth.noise(h, w, seed))
 
@@ -173,7 +173,7 @@ def test_tiled_nccl_two_ranks():
 
 
 AB_IMAGES = [("noise", 40, 33, 2), ("gradnoise", 70, 51, 3), ("noise", 136, 200, 4), ("gradnoise", 32, 300, 5),
-             ("noise", 300, 32, 6), ("gradnoise", 260, 410, 8)]
+             ("noise", 300, 32, 6), ("gradnoise", 260, 410, 8), ("noise", 577, 70, 9), ("gradnoise", 1080, 100, 10)]
 
 
 @pytest.mark.parametrize("gen,h,w,seed", AB_IMAGES)
