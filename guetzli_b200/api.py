@@ -90,6 +90,14 @@ def load_library(path=None):
     lib.gb200_counters.argtypes = [P(C.c_long), P(C.c_longlong), P(C.c_longlong)]
     lib.gb200_profile_enable.argtypes = [C.c_int]
     lib.gb200_profile_get.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
+    lib.gb200_butteraugli_comparator_create.restype = C.c_void_p
+    lib.gb200_butteraugli_comparator_create.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int]
+    lib.gb200_butteraugli_comparator_diffmap.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, P(C.c_double)]
+    lib.gb200_butteraugli_comparator_diffmap_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, P(C.c_double),
+                                                                C.c_void_p]
+    lib.gb200_butteraugli_comparator_mask.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.gb200_butteraugli_comparator_destroy.argtypes = [C.c_void_p]
+    lib.gb200_butteraugli_adaptive_quantization.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]
     _libs[path] = lib
     return lib
 
@@ -235,6 +243,93 @@ def butteraugli_diffmap(rgb0, rgb1, device=0, lib=None):
     if not lib.gb200_butteraugli_diffmap(a.ctypes.data, b.ctypes.data, w, h, device, dm.ctypes.data, C.byref(score)):
         raise RuntimeError(_err(lib))
     return dm, score.value
+
+
+def _is_torch_tensor(x):
+    # without importing torch: a caller that passes a tensor has imported it already
+    return type(x).__module__.split(".")[0] == "torch"
+
+
+class Comparator:
+    """butteraugli::ButteraugliComparator (butteraugli.h:425) on one GPU: the original rgb0, planar
+    linear RGB float32 [3][h][w] in 0..255 and at least 8x8, stays resident and is scored against
+    any number of images.  Used by one thread at a time."""
+
+    def __init__(self, rgb0, device=0, lib=None):
+        self.lib = lib or load_library()
+        self._h = None
+        a = np.ascontiguousarray(rgb0, dtype=np.float32)
+        if a.ndim != 3 or a.shape[0] != 3:
+            raise ValueError(f"rgb0 must be planar [3][h][w], got shape {a.shape}")
+        _, self.h, self.w = a.shape
+        self.device = device
+        self._h = self.lib.gb200_butteraugli_comparator_create(a.ctypes.data, self.w, self.h, device)
+        if not self._h:
+            raise RuntimeError("gb200_butteraugli_comparator_create failed: " + _err(self.lib))
+
+    def close(self):
+        if self._h:
+            self.lib.gb200_butteraugli_comparator_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        self.close()
+
+    def _ck(self, ok):
+        if not ok:
+            raise RuntimeError(_err(self.lib))
+
+    def diffmap(self, rgb1):
+        """ButteraugliComparator::Diffmap + ButteraugliScoreFromDiffmap -> (diffmap [h][w], score).
+
+        A CUDA torch tensor (float32, [3][h][w]) is scored from device memory after the work queued
+        on its device's current torch stream, and the diffmap comes back as a tensor on that device.
+        Anything else is read as a numpy array in host memory."""
+        if _is_torch_tensor(rgb1) and rgb1.is_cuda:
+            return self._diffmap_device(rgb1)
+        a = np.ascontiguousarray(rgb1, dtype=np.float32)
+        if a.shape != (3, self.h, self.w):
+            raise ValueError(f"rgb1 must have shape {(3, self.h, self.w)}, got {a.shape}")
+        dm = np.empty((self.h, self.w), dtype=np.float32)
+        score = C.c_double()
+        self._ck(self.lib.gb200_butteraugli_comparator_diffmap(self._h, a.ctypes.data, dm.ctypes.data,
+                                                               C.byref(score)))
+        return dm, score.value
+
+    def _diffmap_device(self, t):
+        import torch
+        if t.dtype != torch.float32 or tuple(t.shape) != (3, self.h, self.w):
+            raise ValueError(f"rgb1 must be float32 of shape {(3, self.h, self.w)}, got {t.dtype} {tuple(t.shape)}")
+        t = t.contiguous()
+        dm = torch.empty((self.h, self.w), dtype=torch.float32, device=t.device)
+        score = C.c_double()
+        stream = torch.cuda.current_stream(t.device).cuda_stream
+        self._ck(self.lib.gb200_butteraugli_comparator_diffmap_device(self._h, t.data_ptr(), dm.data_ptr(),
+                                                                      C.byref(score), stream))
+        return dm, score.value
+
+    def mask(self):
+        """ButteraugliComparator::Mask -> (mask, mask_dc), float32 [3][h][w] each."""
+        m = np.empty((3, self.h, self.w), dtype=np.float32)
+        mdc = np.empty_like(m)
+        self._ck(self.lib.gb200_butteraugli_comparator_mask(self._h, m.ctypes.data, mdc.ctypes.data))
+        return m, mdc
+
+
+def adaptive_quantization(rgb, device=0, lib=None):
+    """butteraugli::ButteraugliAdaptiveQuantization: rgb planar linear RGB float32 [3][h][w] (0..255)
+    -> quant [h][w] float32.  Raises ValueError below 16x16, where the reference returns false."""
+    lib = lib or load_library()
+    a = np.ascontiguousarray(rgb, dtype=np.float32)
+    if a.ndim != 3 or a.shape[0] != 3:
+        raise ValueError(f"rgb must be planar [3][h][w], got shape {a.shape}")
+    _, h, w = a.shape
+    if w < 16 or h < 16:
+        raise ValueError(f"adaptive quantization needs at least 16x16 pixels, got {w}x{h}")
+    quant = np.empty((h, w), dtype=np.float32)
+    if not lib.gb200_butteraugli_adaptive_quantization(a.ctypes.data, w, h, device, quant.ctypes.data):
+        raise RuntimeError(_err(lib))
+    return quant
 
 
 def counters(lib=None):

@@ -13,6 +13,8 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <stdexcept>
+
 #include "hd.h"
 
 #if defined(GB200_HOSTSIM)
@@ -29,6 +31,12 @@ inline void d2d(void* dst, const void* src, size_t n, Stream = 0) { memcpy(dst, 
 inline void dev_zero(void* dst, size_t n, Stream = 0) { memset(dst, 0, n); }
 inline void stream_sync(Stream = 0) {}
 inline const char* backend_name() { return "hostsim"; }
+// caller-owned device memory and streams exist only on a GPU
+inline int pointer_device(const void*) { throw std::runtime_error("the CPU port has no device memory"); }
+inline void stream_wait(Stream, Stream) { throw std::runtime_error("the CPU port has no streams"); }
+inline void d2d_2d(void*, size_t, const void*, size_t, size_t, size_t, Stream) {
+  throw std::runtime_error("the CPU port has no device memory");
+}
 
 template <class F>
 inline void launch_2d(Stream, const F& f, int w, int h, const char* = nullptr) {
@@ -61,6 +69,12 @@ void d2h(void* dst, const void* src, size_t n, Stream s);  // synchronous
 void d2d(void* dst, const void* src, size_t n, Stream s);
 void dev_zero(void* dst, size_t n, Stream s);
 void stream_sync(Stream s);
+// device ordinal of device memory (cudaPointerGetAttributes); -1 for host, managed or unknown pointers
+int pointer_device(const void* p);
+// work queued on `waiter` from now on runs after the work queued so far on `signaller` (an event)
+void stream_wait(Stream waiter, Stream signaller);
+// rows of `width` bytes between device pitches (cudaMemcpy2DAsync)
+void d2d_2d(void* dst, size_t dpitch, const void* src, size_t spitch, size_t width, size_t rows, Stream s);
 inline const char* backend_name() { return "cuda-sm_90a"; }
 // streaming multiprocessors of the target (H100 SXM); caps grid-stride launches
 constexpr int kTargetSMs = 132;

@@ -212,6 +212,28 @@ void d2d(void* dst, const void* src, size_t n, Stream s) {
 void dev_zero(void* dst, size_t n, Stream s) { GB_CUDA(cudaMemsetAsync(dst, 0, n, s)); }
 void stream_sync(Stream s) { wait_stream(s); }
 
+int pointer_device(const void* p) {
+  cudaPointerAttributes a;
+  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+    cudaGetLastError();
+    return -1;
+  }
+  return a.type == cudaMemoryTypeDevice ? a.device : -1;
+}
+
+void stream_wait(Stream waiter, Stream signaller) {
+  cudaEvent_t ev;
+  GB_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+  cudaError_t e = cudaEventRecord(ev, signaller);
+  if (e == cudaSuccess) e = cudaStreamWaitEvent(waiter, ev, 0);
+  cudaEventDestroy(ev);  // the wait already queued keeps its meaning
+  if (e != cudaSuccess) cuda_fail(e, "stream_wait", __FILE__, __LINE__);
+}
+
+void d2d_2d(void* dst, size_t dpitch, const void* src, size_t spitch, size_t width, size_t rows, Stream s) {
+  GB_CUDA(cudaMemcpy2DAsync(dst, dpitch, src, spitch, width, rows, cudaMemcpyDeviceToDevice, s));
+}
+
 int cuda_device_count() {
   int n = 0;
   if (cudaGetDeviceCount(&n) != cudaSuccess) return 0;

@@ -64,6 +64,11 @@ struct gb200_image {
   gb200::ImageContext* ctx;
 };
 
+struct gb200_butteraugli_comparator {
+  gb200::ImageContext* ctx;  // metric-only context
+  int device;
+};
+
 namespace {
 gb200::SearchParams to_search_params(const gb200_params* params) {
   gb200::SearchParams sp;
@@ -202,6 +207,98 @@ int gb200_butteraugli_diffmap(const float* rgb0, const float* rgb1, int w, int h
       m = dmax;
     }
     if (score) *score = m;
+  });
+}
+
+// ---- butteraugli::ButteraugliComparator (b/butteraugli.h:425) ---------------------
+// butteraugli::ButteraugliComparator::ButteraugliComparator (b/butteraugli.cc:784)
+gb200_butteraugli_comparator* gb200_butteraugli_comparator_create(const float* rgb0, int w, int h, int device) {
+  gb200_butteraugli_comparator* c = nullptr;
+  guarded([&]() {
+    if (rgb0 == nullptr) throw std::runtime_error("butteraugli comparator: no image");
+    // the reference class computes nothing below 8 pixels in a dimension (b/butteraugli.cc:788)
+    if (w < 8 || h < 8 || w >= 65536 || h >= 65536)
+      throw std::runtime_error("butteraugli comparator: the image must be at least 8x8 (and below 65536)");
+    gb200::ImageContext* ctx = new gb200::ImageContext(rgb0, w, h, device);
+    c = new gb200_butteraugli_comparator;
+    c->ctx = ctx;
+    c->device = device;
+  });
+  return c;
+}
+
+void gb200_butteraugli_comparator_destroy(gb200_butteraugli_comparator* c) {
+  if (!c) return;
+  guarded([&]() { delete c->ctx; });
+  delete c;
+}
+
+// ButteraugliComparator::Diffmap (b/butteraugli.cc:799) + ButteraugliScoreFromDiffmap (:1623)
+int gb200_butteraugli_comparator_diffmap(gb200_butteraugli_comparator* c, const float* rgb1, float* diffmap,
+                                         double* score) {
+  if (c == nullptr || rgb1 == nullptr) {
+    g_err = "butteraugli comparator: no comparator or no image";
+    return 0;
+  }
+  return guarded([&]() {
+    const float m = c->ctx->compare_linear(rgb1);
+    if (diffmap) c->ctx->download_distmap(diffmap);
+    if (score) *score = m;
+  });
+}
+
+// The same with rgb1 and diffmap in device memory of the comparator's device.
+int gb200_butteraugli_comparator_diffmap_device(gb200_butteraugli_comparator* c, const float* rgb1_dev,
+                                                float* diffmap_dev, double* score, void* stream) {
+  if (c == nullptr || rgb1_dev == nullptr) {
+    g_err = "butteraugli comparator: no comparator or no image";
+    return 0;
+  }
+  return guarded([&]() {
+    c->ctx->bind();
+    const void* ptrs[2] = {rgb1_dev, diffmap_dev};
+    const char* what[2] = {"rgb1", "diffmap"};
+    for (int i = 0; i < 2; ++i) {
+      if (ptrs[i] == nullptr) continue;
+      const int dev = gb200::pointer_device(ptrs[i]);
+      if (dev != c->device)
+        throw std::runtime_error(std::string("butteraugli comparator: ") + what[i] + " is not device memory of device " +
+                                 std::to_string(c->device) +
+                                 (dev < 0 ? " (host or unknown memory)" : " (device " + std::to_string(dev) + ")"));
+    }
+#if defined(GB200_HOSTSIM)
+    const gb200::Stream caller = 0;  // not reached: the port has no device memory
+    (void)stream;
+#else
+    const gb200::Stream caller = static_cast<gb200::Stream>(stream);
+#endif
+    const float m = c->ctx->compare_linear_device(rgb1_dev, diffmap_dev, caller);
+    if (score) *score = m;
+  });
+}
+
+// ButteraugliComparator::Mask (b/butteraugli.cc:793)
+int gb200_butteraugli_comparator_mask(gb200_butteraugli_comparator* c, float* mask, float* mask_dc) {
+  if (c == nullptr || mask == nullptr || mask_dc == nullptr) {
+    g_err = "butteraugli comparator: no comparator or no output";
+    return 0;
+  }
+  return guarded([&]() { c->ctx->mask(mask, mask_dc); });
+}
+
+// butteraugli::ButteraugliAdaptiveQuantization (b/butteraugli.cc:1880)
+int gb200_butteraugli_adaptive_quantization(const float* rgb, int w, int h, int device, float* quant) {
+  if (rgb == nullptr || quant == nullptr) {
+    g_err = "butteraugli adaptive quantization: no image or no output";
+    return 0;
+  }
+  if (w < 16 || h < 16 || w >= 65536 || h >= 65536) {
+    g_err = "butteraugli adaptive quantization: the image must be at least 16x16 (and below 65536)";
+    return 0;
+  }
+  return guarded([&]() {
+    gb200::ImageContext ctx(rgb, w, h, device);
+    ctx.adaptive_quantization(rgb, quant);
   });
 }
 

@@ -416,21 +416,35 @@ struct NoiseAndAsymAcc {
 
 // ---------------------------------------------------------------------------
 // Mask (b/butteraugli.cc:753-782, 1699-1817).
-// DiffPrecompute of the combined planes m_c = a*uhf_c + b*hf_c, c in {X,Y},
-// for both images; neighbours mirror at the last column/row.
+// The planes MaskPsychoImage hands to Mask (:768-781): m_c = a*uhf_c + b*hf_c in
+// double, stored as float, c in {X,Y}.  a = 0 for X is multiplied as written.
+struct MaskPsychoMix {
+  const float* ps;  // PsychoImage group
+  float* out;       // [2] X, Y
+  Geom g;
+  GB_HD static float mix(const float* ps, int c, size_t o, size_t plane) {
+    // muls (:762-767): X: (0, 1.64178305129), Y: (0.831081703362, 3.23680933546)
+    const double a = c == 0 ? 0.0 : 0.831081703362;
+    const double b = c == 0 ? 1.64178305129 : 3.23680933546;
+    const float uhf = ps[(kUhfX + c) * plane + o];
+    const float hf = ps[(kHfX + c) * plane + o];
+    return static_cast<float>(a * uhf + b * hf);
+  }
+  GB_HD void operator()(int x, int y) const {
+    const size_t o = static_cast<size_t>(y) * g.pitch + x;
+    out[o] = mix(ps, 0, o, g.plane);
+    out[g.plane + o] = mix(ps, 1, o, g.plane);
+  }
+};
+
+// DiffPrecompute of the combined planes m_c (MaskPsychoMix) for both images;
+// neighbours mirror at the last column/row.
 struct MaskDiffPre {
   const float* ps0;  // PsychoImage group of the original
   const float* ps1;  // candidate
   float* out;        // [2] X, Y
   Geom g;
-  GB_HD float combo(const float* ps, int c, size_t o) const {
-    // muls (:762-767): X: (0, 1.64178305129), Y: (0.831081703362, 3.23680933546)
-    const double a = c == 0 ? 0.0 : 0.831081703362;
-    const double b = c == 0 ? 1.64178305129 : 3.23680933546;
-    const float uhf = ps[(kUhfX + c) * g.plane + o];
-    const float hf = ps[(kHfX + c) * g.plane + o];
-    return static_cast<float>(a * uhf + b * hf);
-  }
+  GB_HD float combo(const float* ps, int c, size_t o) const { return MaskPsychoMix::mix(ps, c, o, g.plane); }
   GB_HD void operator()(int x, int y) const {
     const int x2 = (x + 1 < g.w) ? x + 1 : (x > 0 ? x - 1 : x);
     const int y2 = (y + 1 < g.h) ? y + 1 : (y > 0 ? y - 1 : y);
@@ -499,6 +513,26 @@ struct BlockCornerMask {
     out[3 * b + 0] = m[0];
     out[3 * b + 1] = m[1];
     out[3 * b + 2] = m[2];
+  }
+};
+
+// The same at every pixel: the mask and mask_dc planes Mask returns (:1802-1815).
+struct MaskPlanes {
+  const float* sx;
+  const float* sy1;
+  const float* sy2;
+  float* mask;     // [3]
+  float* mask_dc;  // [3]
+  Geom g;
+  const double* luts;
+  GB_HD void operator()(int x, int y) const {
+    const size_t o = static_cast<size_t>(y) * g.pitch + x;
+    float m[3], mdc[3];
+    mask_from_activity(luts, sx[o], mask_y_activity(sy1[o], sy2[o]), m, mdc);
+    for (int c = 0; c < 3; ++c) {
+      mask[c * g.plane + o] = m[c];
+      mask_dc[c * g.plane + o] = mdc[c];
+    }
   }
 };
 

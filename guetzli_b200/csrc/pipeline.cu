@@ -499,6 +499,20 @@ float ImageContext::compare_linear(const float* linear_rgb) {
   return compare_tail();
 }
 
+float ImageContext::compare_linear_device(const float* linear_rgb, float* diffmap, Stream caller) {
+  bind();
+  const size_t row = sizeof(float) * g_.w, pitch = sizeof(float) * g_.pitch;
+  stream_wait(s_, caller);
+  // [3][h][w] -> [3][h][pitch]: a plane is h rows of pitch, so the three planes are 3h rows
+  d2d_2d(lin_, pitch, linear_rgb, row, row, static_cast<size_t>(3) * g_.h, s_);
+  const float m = compare_tail();
+  if (diffmap != nullptr) {
+    d2d_2d(diffmap, row, dm_, pitch, row, g_.h, s_);
+    stream_sync(s_);
+  }
+  return m;
+}
+
 void ImageContext::download_rgb(uint8_t* rgb) {
   bind();
   d2h(rgb, d_rgb_, static_cast<size_t>(3) * g_.w * g_.h, s_);
@@ -660,13 +674,43 @@ void ImageContext::prepare() {
   fused_sup0();
 
   // a13: mask_xyz_ = Mask(xyb0, xyb0), only its block-corner samples are ever read.
-  px(MaskDiffPreSelf{xyb_, mpre_, g_}, "mask_diff_pre_self");
-  blur(mpre_, sact_, 1, kBlurMaskX);
-  blur(mpre_ + g_.plane, sact_ + g_.plane, 1, kBlurMaskY0);
-  blur(mpre_ + g_.plane, sact_ + 2 * g_.plane, 1, kBlurMaskY1);
+  mask_activity(xyb_);
   block_rows(BlockCornerMask{sact_, sact_ + g_.plane, sact_ + 2 * g_.plane, corner_mask_, g_, t_.mask_lut},
              "block_corner_mask", by_lo_, by_hi_);
   stream_sync(s_);
+}
+
+void ImageContext::mask_activity(const float* xy) {
+  px(MaskDiffPreSelf{xy, mpre_, g_}, "mask_diff_pre_self");
+  blur(mpre_, sact_, 1, kBlurMaskX);
+  blur(mpre_ + g_.plane, sact_ + g_.plane, 1, kBlurMaskY0);
+  blur(mpre_ + g_.plane, sact_ + 2 * g_.plane, 1, kBlurMaskY1);
+}
+
+void ImageContext::mask_planes(const float* xy) {
+  if (mask_ == nullptr) mask_ = planes(6);
+  mask_activity(xy);
+  px(MaskPlanes{sact_, sact_ + g_.plane, sact_ + 2 * g_.plane, mask_, mask_ + 3 * g_.plane, g_, t_.mask_lut},
+     "mask_planes");
+}
+
+void ImageContext::mask(float* mask, float* mask_dc) {
+  if (!metric_only_) throw std::runtime_error("mask(): not a metric-only context");
+  bind();
+  // MaskPsychoImage(pi0_, pi0_) (b/butteraugli.cc:753): the mixed X and Y planes go to xyb_, which
+  // every Compare rewrites before reading it
+  px(MaskPsychoMix{ps0_, xyb_, g_}, "mask_psycho_mix");
+  mask_planes(xyb_);
+  download_planes(mask_, mask, 3);
+  download_planes(mask_ + 3 * g_.plane, mask_dc, 3);
+}
+
+void ImageContext::adaptive_quantization(const float* linear_rgb, float* quant) {
+  if (!metric_only_) throw std::runtime_error("adaptive_quantization(): not a metric-only context");
+  bind();
+  upload_planes(linear_rgb, lin_, 3);
+  mask_planes(lin_);
+  download_planes(mask_ + g_.plane, quant, 1);
 }
 
 ImageContext::~ImageContext() { release(); }

@@ -47,6 +47,17 @@ class ImageContext {
   // float planes [3][h][w]; compare_linear() scores a second one against it.
   ImageContext(const float* linear_rgb, int w, int h, int device);
   float compare_linear(const float* linear_rgb);
+  // The same with the second image in memory of this context's device, packed [3][h][w].  This
+  // context's stream first waits for the work queued so far on `caller`; the image is then copied
+  // into lin_ (the tensor maps and the captured graph are bound to lin_).  diffmap: device memory,
+  // packed [h][w], or null; it is written when the call returns.
+  float compare_linear_device(const float* linear_rgb, float* diffmap, Stream caller);
+  // ButteraugliComparator::Mask (b/butteraugli.cc:793) of the first image at every pixel, on the
+  // host: mask, mask_dc [3][h][w].  Leaves the resident PsychoImage as it is.
+  void mask(float* mask, float* mask_dc);
+  // Mask(rgb, rgb) of linear RGB planes [3][h][w] as ButteraugliAdaptiveQuantization
+  // (b/butteraugli.cc:1880) computes it: its Y plane -> quant [h][w] on the host.
+  void adaptive_quantization(const float* linear_rgb, float* quant);
   // the one-time kernels (idempotent); split from the upload so that a caller can
   // time the job with the image already resident in HBM
   void prepare();
@@ -193,6 +204,11 @@ class ImageContext {
   void gather_blocks(void* dev_buf, size_t elem_bytes_per_block);
   void opsin(const float* lin, float* xyb);
   void separate(const float* xyb, float* ps);
+  // Mask's DiffPrecompute of X and Y (planes xy[0], xy[1]) and its three blurs -> sact_
+  void mask_activity(const float* xy);
+  // Mask(xy, xy) at every pixel -> mask_ (mask [3], then mask_dc [3], allocated on first use)
+  void mask_planes(const float* xy);
+  float* mask_ = nullptr;
   void upload_planes(const float* packed, float* dst, int n);
   void download_planes(const float* src, float* packed, int n);
   float* planes(int n);

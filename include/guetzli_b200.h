@@ -85,6 +85,33 @@ int gb200_process_jpeg(const gb200_params* params, const uint8_t* jpeg_in, size_
 int gb200_butteraugli_diffmap(const float* rgb0, const float* rgb1, int w, int h, int device, float* diffmap,
                               double* score);
 
+/* ---- butteraugli::ButteraugliComparator (third_party/butteraugli/butteraugli/butteraugli.h:425) ----
+ * One original kept resident on one GPU (its PsychoImage, the neighbour sums of its mask) and scored
+ * against any number of images.  Images are planar linear RGB floats [3][h][w] in 0..255, the
+ * original at least 8x8 (the reference class computes nothing below that; gb200_butteraugli_diffmap
+ * pads small images).  One comparator is used by one thread at a time; separate comparators may run
+ * concurrently, each has its own stream.  Every call returns once its outputs are written. */
+typedef struct gb200_butteraugli_comparator gb200_butteraugli_comparator;
+/* ButteraugliComparator::ButteraugliComparator(rgb0) (butteraugli.cc:784); rgb0 in host memory.
+ * NULL on failure (gb200_last_error). */
+gb200_butteraugli_comparator* gb200_butteraugli_comparator_create(const float* rgb0, int w, int h, int device);
+/* ButteraugliComparator::Diffmap (butteraugli.cc:799) and ButteraugliScoreFromDiffmap (butteraugli.cc:1623):
+ * rgb1 [3][h][w] in host memory; diffmap (may be NULL) receives [h][w], *score its maximum. */
+int gb200_butteraugli_comparator_diffmap(gb200_butteraugli_comparator* c, const float* rgb1, float* diffmap,
+                                         double* score);
+/* The same with rgb1 [3][h][w] and diffmap [h][w] (may be NULL) in device memory of the comparator's
+ * device.  stream (a cudaStream_t, NULL = the legacy default stream): the comparator waits for the work
+ * queued on it so far, so rgb1 may still be in the making there.  rgb1 is copied into the comparator's
+ * own buffer before it is read.  A host pointer or memory of another device is refused, nothing runs. */
+int gb200_butteraugli_comparator_diffmap_device(gb200_butteraugli_comparator* c, const float* rgb1_dev,
+                                                float* diffmap_dev, double* score, void* stream);
+/* ButteraugliComparator::Mask (butteraugli.cc:793): mask and mask_dc, [3][h][w] each, host memory. */
+int gb200_butteraugli_comparator_mask(gb200_butteraugli_comparator* c, float* mask, float* mask_dc);
+void gb200_butteraugli_comparator_destroy(gb200_butteraugli_comparator* c);
+/* butteraugli::ButteraugliAdaptiveQuantization (butteraugli.cc:1880): the Y plane of Mask(rgb, rgb),
+ * [h][w] into quant.  rgb in host memory.  Fails below 16x16, where the reference returns false. */
+int gb200_butteraugli_adaptive_quantization(const float* rgb, int w, int h, int device, float* quant);
+
 /* ReadJpeg(JPEG_READ_HEADER) as the CLI uses it (guetzli/guetzli.cc:306): frame size only. */
 int gb200_jpeg_dimensions(const uint8_t* jpeg_in, size_t jpeg_len, int* width, int* height);
 

@@ -8,6 +8,7 @@
 #define GUETZLI_B200_COMPAT_H_
 
 #include <cstdio>
+#include <cstdlib>
 #include <map>
 #include <string>
 #include <vector>
@@ -124,5 +125,90 @@ inline bool Process(const Params& params, ProcessStats* stats, const std::string
 }
 
 }  // namespace guetzli
+
+namespace guetzli_b200 {
+
+// butteraugli::ButteraugliComparator (third_party/butteraugli/butteraugli/butteraugli.h:425) with
+// the original resident on one GPU.  Images are three planes of linear RGB (0..255), each w*h floats
+// row by row, as ButteraugliAdaptiveQuantization takes them; outputs are laid out the same way.
+// The methods return false on failure (gb200_last_error), where the reference's return nothing.
+// One comparator is used by one thread at a time.
+class ButteraugliComparator {
+ public:
+  ButteraugliComparator(const std::vector<std::vector<float> >& rgb0, int w, int h, int device = 0)
+      : w_(w), h_(h) {
+    if (Complete(rgb0)) {
+      const std::vector<float> flat = Flat(rgb0);
+      c_ = gb200_butteraugli_comparator_create(flat.data(), w, h, device);
+    }
+  }
+  ~ButteraugliComparator() { gb200_butteraugli_comparator_destroy(c_); }
+  ButteraugliComparator(const ButteraugliComparator&) = delete;
+  ButteraugliComparator& operator=(const ButteraugliComparator&) = delete;
+
+  // false when the original was refused (smaller than 8x8, no device, ...)
+  bool ok() const { return c_ != nullptr; }
+
+  // ButteraugliComparator::Diffmap (butteraugli.cc:799): result receives w*h floats.
+  bool Diffmap(const std::vector<std::vector<float> >& rgb1, std::vector<float>& result) {
+    if (!c_ || !Complete(rgb1)) return false;
+    const std::vector<float> flat = Flat(rgb1);
+    result.resize(static_cast<size_t>(w_) * h_);
+    return gb200_butteraugli_comparator_diffmap(c_, flat.data(), result.data(), nullptr) != 0;
+  }
+
+  // ButteraugliComparator::Mask (butteraugli.cc:793): three planes each.
+  bool Mask(std::vector<std::vector<float> >* mask, std::vector<std::vector<float> >* mask_dc) {
+    if (!c_) return false;
+    const size_t n = static_cast<size_t>(w_) * h_;
+    std::vector<float> m(3 * n), mdc(3 * n);
+    if (!gb200_butteraugli_comparator_mask(c_, m.data(), mdc.data())) return false;
+    mask->assign(3, std::vector<float>());
+    mask_dc->assign(3, std::vector<float>());
+    for (int c = 0; c < 3; ++c) {
+      (*mask)[c].assign(m.begin() + c * n, m.begin() + (c + 1) * n);
+      (*mask_dc)[c].assign(mdc.begin() + c * n, mdc.begin() + (c + 1) * n);
+    }
+    return true;
+  }
+
+ private:
+  bool Complete(const std::vector<std::vector<float> >& rgb) const {
+    if (rgb.size() != 3 || w_ < 1 || h_ < 1) return false;
+    for (int c = 0; c < 3; ++c)
+      if (rgb[c].size() != static_cast<size_t>(w_) * h_) return false;
+    return true;
+  }
+  static std::vector<float> Flat(const std::vector<std::vector<float> >& rgb) {
+    std::vector<float> flat;
+    for (int c = 0; c < 3; ++c) flat.insert(flat.end(), rgb[c].begin(), rgb[c].end());
+    return flat;
+  }
+  gb200_butteraugli_comparator* c_ = nullptr;
+  int w_, h_;
+};
+
+// butteraugli::ButteraugliAdaptiveQuantization (butteraugli.cc:1880), same signature; the device
+// is GUETZLI_B200_DEVICE (environment), default 0.  False below 16x16, as the reference.
+inline bool ButteraugliAdaptiveQuantization(size_t xsize, size_t ysize, const std::vector<std::vector<float> >& rgb,
+                                            std::vector<float>& quant) {
+  const size_t n = xsize * ysize;
+  if (xsize < 16 || ysize < 16 || rgb.size() != 3 || xsize >= 65536 || ysize >= 65536) return false;
+  std::vector<float> flat;
+  for (int c = 0; c < 3; ++c) {
+    if (rgb[c].size() != n) return false;
+    flat.insert(flat.end(), rgb[c].begin(), rgb[c].end());
+  }
+  int device = 0;
+  if (const char* e = getenv("GUETZLI_B200_DEVICE")) device = atoi(e);
+  std::vector<float> q(n);
+  if (!gb200_butteraugli_adaptive_quantization(flat.data(), static_cast<int>(xsize), static_cast<int>(ysize), device,
+                                               q.data()))
+    return false;
+  quant.insert(quant.end(), q.begin(), q.end());  // the reference appends too
+  return true;
+}
+
+}  // namespace guetzli_b200
 
 #endif  // GUETZLI_B200_COMPAT_H_
