@@ -98,6 +98,13 @@ def load_library(path=None):
     lib.gb200_butteraugli_comparator_mask.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
     lib.gb200_butteraugli_comparator_destroy.argtypes = [C.c_void_p]
     lib.gb200_butteraugli_adaptive_quantization.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]
+    lib.gb200_butteraugli_batch_create.restype = C.c_void_p
+    lib.gb200_butteraugli_batch_create.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int]
+    lib.gb200_butteraugli_batch_diffmap.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                                                    C.c_void_p]
+    lib.gb200_butteraugli_batch_diffmap_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                                                           C.c_void_p, C.c_void_p]
+    lib.gb200_butteraugli_batch_destroy.argtypes = [C.c_void_p]
     _libs[path] = lib
     return lib
 
@@ -314,6 +321,78 @@ class Comparator:
         mdc = np.empty_like(m)
         self._ck(self.lib.gb200_butteraugli_comparator_mask(self._h, m.ctypes.data, mdc.ctypes.data))
         return m, mdc
+
+
+class ButteraugliBatch:
+    """butteraugli::ButteraugliInterface on up to `capacity` same-size pairs per call, on one GPU: each
+    pair (rgb0[i], rgb1[i]) is scored as gb.butteraugli_diffmap scores it alone, bit for bit, with the
+    pairs going through the Compare chain together.  Images are planar linear RGB float32 in 0..255,
+    at least 8x8.  Used by one thread at a time."""
+
+    def __init__(self, h, w, capacity, device=0, lib=None):
+        self.lib = lib or load_library()
+        self._h = None
+        self.h, self.w, self.capacity, self.device = int(h), int(w), int(capacity), device
+        self._h = self.lib.gb200_butteraugli_batch_create(self.w, self.h, self.capacity, device)
+        if not self._h:
+            raise RuntimeError("gb200_butteraugli_batch_create failed: " + _err(self.lib))
+
+    def close(self):
+        if self._h:
+            self.lib.gb200_butteraugli_batch_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        self.close()
+
+    def _shape_of(self, shape):
+        if len(shape) != 4 or tuple(shape[1:]) != (3, self.h, self.w) or not 1 <= shape[0] <= self.capacity:
+            raise ValueError(f"rgb0 and rgb1 must have shape [n, 3, {self.h}, {self.w}] with 1 <= n <= "
+                             f"{self.capacity}, got {tuple(shape)}")
+        return shape[0]
+
+    def diffmap(self, rgb0, rgb1):
+        """-> (diffmaps [n][h][w], scores float64 [n]) for rgb0, rgb1 float32 [n][3][h][w].
+
+        CUDA torch tensors are scored from device memory after the work queued on their device's
+        current torch stream, and the diffmaps come back as a tensor on that device.  Anything else
+        is read as numpy arrays in host memory.  The scores are a numpy array either way."""
+        if _is_torch_tensor(rgb0) and _is_torch_tensor(rgb1) and rgb0.is_cuda and rgb1.is_cuda:
+            return self._diffmap_device(rgb0, rgb1)
+        if _is_torch_tensor(rgb0) or _is_torch_tensor(rgb1):
+            if getattr(rgb0, "is_cuda", False) or getattr(rgb1, "is_cuda", False):
+                raise ValueError("rgb0 and rgb1 must both be CUDA tensors or both host arrays")
+        a, b = np.asarray(rgb0), np.asarray(rgb1)
+        if a.dtype != np.float32 or b.dtype != np.float32:
+            raise ValueError(f"rgb0 and rgb1 must be float32, got {a.dtype} and {b.dtype}")
+        if a.shape != b.shape:
+            raise ValueError(f"rgb0 and rgb1 differ in shape: {a.shape} and {b.shape}")
+        n = self._shape_of(a.shape)
+        a, b = np.ascontiguousarray(a), np.ascontiguousarray(b)
+        dm = np.empty((n, self.h, self.w), dtype=np.float32)
+        score = np.empty(n, dtype=np.float64)
+        if not self.lib.gb200_butteraugli_batch_diffmap(self._h, a.ctypes.data, b.ctypes.data, n, dm.ctypes.data,
+                                                        score.ctypes.data):
+            raise RuntimeError(_err(self.lib))
+        return dm, score
+
+    def _diffmap_device(self, t0, t1):
+        import torch
+        if t0.dtype != torch.float32 or t1.dtype != torch.float32:
+            raise ValueError(f"rgb0 and rgb1 must be float32, got {t0.dtype} and {t1.dtype}")
+        if tuple(t0.shape) != tuple(t1.shape):
+            raise ValueError(f"rgb0 and rgb1 differ in shape: {tuple(t0.shape)} and {tuple(t1.shape)}")
+        if t0.device != t1.device:
+            raise ValueError(f"rgb0 and rgb1 are on different devices: {t0.device} and {t1.device}")
+        n = self._shape_of(tuple(t0.shape))
+        t0, t1 = t0.contiguous(), t1.contiguous()
+        dm = torch.empty((n, self.h, self.w), dtype=torch.float32, device=t0.device)
+        score = np.empty(n, dtype=np.float64)
+        stream = torch.cuda.current_stream(t0.device).cuda_stream
+        if not self.lib.gb200_butteraugli_batch_diffmap_device(self._h, t0.data_ptr(), t1.data_ptr(), n, dm.data_ptr(),
+                                                               score.ctypes.data, stream):
+            raise RuntimeError(_err(self.lib))
+        return dm, score
 
 
 def adaptive_quantization(rgb, device=0, lib=None):

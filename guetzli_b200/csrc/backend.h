@@ -37,6 +37,13 @@ inline void stream_wait(Stream, Stream) { throw std::runtime_error("the CPU port
 inline void d2d_2d(void*, size_t, const void*, size_t, size_t, size_t, Stream) {
   throw std::runtime_error("the CPU port has no device memory");
 }
+inline void copy_3d(void* dst, size_t dpitch, size_t drows, const void* src, size_t spitch, size_t srows, size_t width,
+                    size_t rows, size_t depth, Stream) {
+  for (size_t z = 0; z < depth; ++z)
+    for (size_t r = 0; r < rows; ++r)
+      memcpy(static_cast<char*>(dst) + (z * drows + r) * dpitch, static_cast<const char*>(src) + (z * srows + r) * spitch,
+             width);
+}
 
 template <class F>
 inline void launch_2d(Stream, const F& f, int w, int h, const char* = nullptr) {
@@ -75,6 +82,10 @@ int pointer_device(const void* p);
 void stream_wait(Stream waiter, Stream signaller);
 // rows of `width` bytes between device pitches (cudaMemcpy2DAsync)
 void d2d_2d(void* dst, size_t dpitch, const void* src, size_t spitch, size_t width, size_t rows, Stream s);
+// `depth` slices of `rows` rows of `width` bytes; a slice is drows (srows) rows of dpitch (spitch)
+// bytes; host or device memory on either side (one cudaMemcpy3DAsync)
+void copy_3d(void* dst, size_t dpitch, size_t drows, const void* src, size_t spitch, size_t srows, size_t width,
+             size_t rows, size_t depth, Stream s);
 inline const char* backend_name() { return "cuda-sm_90a"; }
 // streaming multiprocessors of the target (H100 SXM); caps grid-stride launches
 constexpr int kTargetSMs = 132;

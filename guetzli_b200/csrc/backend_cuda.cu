@@ -234,6 +234,16 @@ void d2d_2d(void* dst, size_t dpitch, const void* src, size_t spitch, size_t wid
   GB_CUDA(cudaMemcpy2DAsync(dst, dpitch, src, spitch, width, rows, cudaMemcpyDeviceToDevice, s));
 }
 
+void copy_3d(void* dst, size_t dpitch, size_t drows, const void* src, size_t spitch, size_t srows, size_t width,
+             size_t rows, size_t depth, Stream s) {
+  cudaMemcpy3DParms p = {};
+  p.srcPtr = make_cudaPitchedPtr(const_cast<void*>(src), spitch, width, srows);
+  p.dstPtr = make_cudaPitchedPtr(dst, dpitch, width, drows);
+  p.extent = make_cudaExtent(width, rows, depth);
+  p.kind = cudaMemcpyDefault;
+  GB_CUDA(cudaMemcpy3DAsync(&p, s));
+}
+
 int cuda_device_count() {
   int n = 0;
   if (cudaGetDeviceCount(&n) != cudaSuccess) return 0;

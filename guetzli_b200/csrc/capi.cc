@@ -69,6 +69,25 @@ struct gb200_butteraugli_comparator {
   int device;
 };
 
+struct gb200_butteraugli_batch {
+  gb200::ImageContext* ctx;  // batched metric-only context
+  int device;
+};
+
+namespace {
+// device pointers of a *_device entry: memory of `device`, else a message naming the argument
+void check_device_pointers(const char* who, int device, const void* const* ptrs, const char* const* what, int n) {
+  for (int i = 0; i < n; ++i) {
+    if (ptrs[i] == nullptr) continue;
+    const int dev = gb200::pointer_device(ptrs[i]);
+    if (dev != device)
+      throw std::runtime_error(std::string(who) + ": " + what[i] + " is not device memory of device " +
+                               std::to_string(device) +
+                               (dev < 0 ? " (host or unknown memory)" : " (device " + std::to_string(dev) + ")"));
+  }
+}
+}  // namespace
+
 namespace {
 gb200::SearchParams to_search_params(const gb200_params* params) {
   gb200::SearchParams sp;
@@ -258,14 +277,7 @@ int gb200_butteraugli_comparator_diffmap_device(gb200_butteraugli_comparator* c,
     c->ctx->bind();
     const void* ptrs[2] = {rgb1_dev, diffmap_dev};
     const char* what[2] = {"rgb1", "diffmap"};
-    for (int i = 0; i < 2; ++i) {
-      if (ptrs[i] == nullptr) continue;
-      const int dev = gb200::pointer_device(ptrs[i]);
-      if (dev != c->device)
-        throw std::runtime_error(std::string("butteraugli comparator: ") + what[i] + " is not device memory of device " +
-                                 std::to_string(c->device) +
-                                 (dev < 0 ? " (host or unknown memory)" : " (device " + std::to_string(dev) + ")"));
-    }
+    check_device_pointers("butteraugli comparator", c->device, ptrs, what, 2);
 #if defined(GB200_HOSTSIM)
     const gb200::Stream caller = 0;  // not reached: the port has no device memory
     (void)stream;
@@ -275,6 +287,71 @@ int gb200_butteraugli_comparator_diffmap_device(gb200_butteraugli_comparator* c,
     const float m = c->ctx->compare_linear_device(rgb1_dev, diffmap_dev, caller);
     if (score) *score = m;
   });
+}
+
+// ---- butteraugli::ButteraugliInterface (b/butteraugli.cc:1858) on N pairs per call ----------
+gb200_butteraugli_batch* gb200_butteraugli_batch_create(int w, int h, int capacity, int device) {
+  gb200_butteraugli_batch* b = nullptr;
+  guarded([&]() {
+    if (w < 8 || h < 8 || w >= 65536 || h >= 65536)
+      throw std::runtime_error("butteraugli batch: the images must be at least 8x8 (and below 65536)");
+    // the batched Compare chain folds the image into blockIdx.z, four z per image in its widest launch
+    if (capacity < 1 || capacity > 16383)
+      throw std::runtime_error("butteraugli batch: the capacity must be in 1..16383");
+    gb200::ImageContext* ctx = new gb200::ImageContext(w, h, capacity, device);
+    b = new gb200_butteraugli_batch;
+    b->ctx = ctx;
+    b->device = device;
+  });
+  return b;
+}
+
+void gb200_butteraugli_batch_destroy(gb200_butteraugli_batch* b) {
+  if (!b) return;
+  guarded([&]() { delete b->ctx; });
+  delete b;
+}
+
+namespace {
+int batch_diffmap(gb200_butteraugli_batch* b, const float* rgb0, const float* rgb1, int n, float* diffmap,
+                  double* score, bool device, void* stream) {
+  if (b == nullptr || rgb0 == nullptr || rgb1 == nullptr) {
+    g_err = "butteraugli batch: no batch or no images";
+    return 0;
+  }
+  if (n < 1 || n > b->ctx->capacity()) {
+    g_err = "butteraugli batch: n = " + std::to_string(n) + " pairs, the batch takes 1.." +
+            std::to_string(b->ctx->capacity());
+    return 0;
+  }
+  return guarded([&]() {
+    b->ctx->bind();
+    gb200::Stream caller = 0;
+    if (device) {
+      const void* ptrs[3] = {rgb0, rgb1, diffmap};
+      const char* what[3] = {"rgb0", "rgb1", "diffmap"};
+      check_device_pointers("butteraugli batch", b->device, ptrs, what, 3);
+#if !defined(GB200_HOSTSIM)
+      caller = static_cast<gb200::Stream>(stream);
+#endif
+    }
+    (void)stream;
+    std::vector<float> m(n);
+    b->ctx->compare_batch(rgb0, rgb1, n, diffmap, m.data(), device, caller);
+    if (score)
+      for (int i = 0; i < n; ++i) score[i] = m[i];
+  });
+}
+}  // namespace
+
+int gb200_butteraugli_batch_diffmap(gb200_butteraugli_batch* b, const float* rgb0, const float* rgb1, int n,
+                                    float* diffmap, double* score) {
+  return batch_diffmap(b, rgb0, rgb1, n, diffmap, score, false, nullptr);
+}
+
+int gb200_butteraugli_batch_diffmap_device(gb200_butteraugli_batch* b, const float* rgb0_dev, const float* rgb1_dev,
+                                           int n, float* diffmap_dev, double* score, void* stream) {
+  return batch_diffmap(b, rgb0_dev, rgb1_dev, n, diffmap_dev, score, true, stream);
 }
 
 // ButteraugliComparator::Mask (b/butteraugli.cc:793)

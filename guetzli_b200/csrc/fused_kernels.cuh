@@ -45,7 +45,21 @@ struct PlaneGeom {
   int w, h, pitch;
   size_t plane;   // floats per plane
   int y0, y_end;  // rows [y0, y_end) are produced (strip mode computes a sub-range)
+  // Batched launches (kernel template argument B): image n keeps its planes in arena slot n,
+  // kslot planes (kslot * plane floats) after slot 0, so every pointer moves by n * kslot * plane
+  // and every TMA plane coordinate by n * kslot.  The grid's z is n * zimg + (the single-image z).
+  // Single-image instantiations (B = false) read neither field.
+  int kslot, zimg;
 };
+
+// image index and single-image z of a block of a batched launch; (0, blockIdx.z) when B is false
+template <bool B>
+__device__ __forceinline__ int batch_image(const PlaneGeom& g) {
+  return B ? static_cast<int>(blockIdx.z) / g.zimg : 0;
+}
+__device__ __forceinline__ size_t slot_offset(const PlaneGeom& g, int n) {
+  return static_cast<size_t>(n) * g.kslot * g.plane;
+}
 
 // ---------------------------------------------------------------------------
 // Streaming inner loops.  `acc` must be zero on entry.
@@ -145,9 +159,10 @@ __device__ __forceinline__ void blur_x_tile(float* tile, uint64_t* bar, const CU
   }
 }
 
-// Four single-plane x passes with different kernels in one launch (blockIdx.z picks the blur):
-// the noise blur and the three mask blurs all become ready after hf_fused / mask_pre, and each
-// alone is a one-wave launch whose ramp and tail cost as much as its arithmetic.
+// Four single-plane x passes with different kernels in one launch (blockIdx.z picks the blur;
+// batched: z = n * 4 + blur): the noise blur and the three mask blurs all become ready after
+// hf_fused / mask_pre, and each alone is a one-wave launch whose ramp and tail cost as much as its
+// arithmetic.
 template <int R0, int R1, int R2, int R3>
 struct BlurX4Args {
   float* out[4];
@@ -158,7 +173,7 @@ struct BlurX4Args {
   BlurK<R3> k3;
 };
 
-template <int R0, int R1, int R2, int R3>
+template <bool B, int R0, int R1, int R2, int R3>
 __global__ void __launch_bounds__(128) k_tma_blur_x4(const __grid_constant__ CUtensorMap m0,
                                                      const __grid_constant__ CUtensorMap m1,
                                                      const __grid_constant__ CUtensorMap m2,
@@ -168,11 +183,13 @@ __global__ void __launch_bounds__(128) k_tma_blur_x4(const __grid_constant__ CUt
                                : (R1 > R2 ? (R1 > R3 ? R1 : R3) : (R2 > R3 ? R2 : R3));
   __shared__ __align__(128) float tile[GBX_TH * BlurXCfg<RMAX>::SW];
   __shared__ __align__(8) uint64_t bar;
-  switch (blockIdx.z) {  // uniform per CTA
-    case 0: blur_x_tile<R0>(tile, &bar, &m0, a.out[0], a.scale_x[0], g, a.k0, 0); break;
-    case 1: blur_x_tile<R1>(tile, &bar, &m1, a.out[1], a.scale_x[1], g, a.k1, 0); break;
-    case 2: blur_x_tile<R2>(tile, &bar, &m2, a.out[2], a.scale_x[2], g, a.k2, 0); break;
-    default: blur_x_tile<R3>(tile, &bar, &m3, a.out[3], a.scale_x[3], g, a.k3, 0); break;
+  // the image's first plane: blur_x_tile takes it as the TMA plane and as the output plane
+  const int n = B ? static_cast<int>(blockIdx.z) >> 2 : 0, pl = n * g.kslot;
+  switch (B ? blockIdx.z & 3 : blockIdx.z) {  // uniform per CTA
+    case 0: blur_x_tile<R0>(tile, &bar, &m0, a.out[0], a.scale_x[0], g, a.k0, pl); break;
+    case 1: blur_x_tile<R1>(tile, &bar, &m1, a.out[1], a.scale_x[1], g, a.k1, pl); break;
+    case 2: blur_x_tile<R2>(tile, &bar, &m2, a.out[2], a.scale_x[2], g, a.k2, pl); break;
+    default: blur_x_tile<R3>(tile, &bar, &m3, a.out[3], a.scale_x[3], g, a.k3, pl); break;
   }
 }
 
@@ -180,19 +197,20 @@ __global__ void __launch_bounds__(128) k_tma_blur_x4(const __grid_constant__ CUt
 // y pass with epilogue: tile of GBY_TW x GBY_TH outputs, 256 threads = 128 columns x
 // 2 groups of 16 rows.  NP planes are blurred by the same thread (their tiles arrive
 // together) and handed to the epilogue as v[NP] per pixel.
-// grid (ceil(w / TW), ceil(rows / TH), NP == 1 ? planes : 1).
+// grid (ceil(w / TW), ceil(rows / TH), NP == 1 ? planes : 1), times the images of a batched launch.
 #define GBY_TW 128
 #define GBY_TH 32
 #define GBY_G 16
 
-template <int R, int NP, class Epi>
+template <bool B, int R, int NP, class Epi>
 __global__ void __launch_bounds__(256, NP == 1 ? 3 : 2) k_tma_blur_y(const __grid_constant__ CUtensorMap in_map, const float* scale_y,
                                                     PlaneGeom g, BlurK<R> k, Epi epi) {
   constexpr int HI = GBY_TH + 2 * R;
   extern __shared__ __align__(128) float dyn_smem[];
   float* tile = dyn_smem;                                                     // [NP][HI][TW]
   uint64_t* bar = reinterpret_cast<uint64_t*>(dyn_smem + NP * HI * GBY_TW);  // 8-byte aligned: sizes are multiples of 128 B
-  const int x0 = blockIdx.x * GBY_TW, yb = g.y0 + blockIdx.y * GBY_TH, pz = blockIdx.z;
+  const int n = batch_image<B>(g);
+  const int x0 = blockIdx.x * GBY_TW, yb = g.y0 + blockIdx.y * GBY_TH, pz = blockIdx.z - n * g.zimg;
   if (threadIdx.x == 0) {
     mbar_init(bar, 1);
     mbar_fence_init();
@@ -201,7 +219,8 @@ __global__ void __launch_bounds__(256, NP == 1 ? 3 : 2) k_tma_blur_y(const __gri
   if (threadIdx.x == 0) {
     mbar_expect_tx(bar, NP * HI * GBY_TW * 4);
 #pragma unroll
-    for (int p = 0; p < NP; ++p) tma_load_box(tile + p * HI * GBY_TW, &in_map, bar, x0, yb - R, NP == 1 ? pz : p);
+    for (int p = 0; p < NP; ++p)
+      tma_load_box(tile + p * HI * GBY_TW, &in_map, bar, x0, yb - R, n * g.kslot + (NP == 1 ? pz : p));
   }
   const int c = threadIdx.x & (GBY_TW - 1), grp = threadIdx.x >> 7;
   const int x = x0 + c, yg = yb + GBY_G * grp;
@@ -236,7 +255,7 @@ __global__ void __launch_bounds__(256, NP == 1 ? 3 : 2) k_tma_blur_y(const __gri
 #pragma unroll
     for (int i = 0; i < CH; ++i) {
       const int y = yg + o0 + i;
-      if (y < g.y_end) epi.load(x, y, pz, pre[i]);
+      if (y < g.y_end) epi.load(x, y, n, pz, pre[i]);
     }
 #pragma unroll
     for (int i = 0; i < CH; ++i) {
@@ -245,7 +264,7 @@ __global__ void __launch_bounds__(256, NP == 1 ? 3 : 2) k_tma_blur_y(const __gri
       float v[NP];
 #pragma unroll
       for (int p = 0; p < NP; ++p) v[p] = res[p][o0 + i];
-      epi.apply(x, y, pz, v, pre[i]);
+      epi.apply(x, y, n, pz, v, pre[i]);
     }
   }
 }
@@ -347,8 +366,9 @@ __device__ __forceinline__ void roll_y(const float* s, const BlurK<R>& k, const 
 }
 
 // NP planes blurred by the same thread and handed to the epilogue as v[NP] per pixel
-// (NP == 1: blockIdx.z picks the plane).  grid (ceil(w / TW), ceil(rows / seg), NP == 1 ? planes : 1).
-template <int R, int NP, class Epi>
+// (NP == 1: blockIdx.z picks the plane).  grid (ceil(w / TW), ceil(rows / seg), NP == 1 ? planes : 1),
+// times the images of a batched launch.
+template <bool B, int R, int NP, class Epi>
 __global__ void __launch_bounds__(128) k_roll_blur(const __grid_constant__ CUtensorMap in_map, const float* scale_x,
                                                    const float* scale_y, PlaneGeom g, int seg, BlurK<R> k, Epi epi) {
   typedef RollCfg<R, NP> C;
@@ -357,7 +377,8 @@ __global__ void __launch_bounds__(128) k_roll_blur(const __grid_constant__ CUten
   float* stage = dyn_smem;                        // [NS][NP][CH][SW]
   float* ring = dyn_smem + NS * C::kStageFloats;  // [NP][RBUF][TW]
   uint64_t* bar = reinterpret_cast<uint64_t*>(ring + C::kRingFloats);
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, pz = blockIdx.z;
+  const int n = batch_image<B>(g), pl0 = n * g.kslot;  // image, its first TMA plane
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, pz = blockIdx.z - n * g.zimg;
   const int x0 = blockIdx.x * GBR_TW, x = x0 + lane;
   const int ys = g.y0 + blockIdx.y * seg;
   const int ye = min(ys + seg, g.y_end);
@@ -377,7 +398,7 @@ __global__ void __launch_bounds__(128) k_roll_blur(const __grid_constant__ CUten
 #pragma unroll
       for (int p = 0; p < NP; ++p)
         tma_load_box(stage + c * C::kStageFloats + p * GBR_CH * C::SW, &in_map, &bar[c], x0 - RP, yin + c * GBR_CH,
-                     NP == 1 ? pz : p);
+                     pl0 + (NP == 1 ? pz : p));
     }
   }
   const bool edge_x = (x0 < R) || (x0 + GBR_TW + R > g.w);
@@ -394,7 +415,7 @@ __global__ void __launch_bounds__(128) k_roll_blur(const __grid_constant__ CUten
 #pragma unroll
       for (int p = 0; p < NP; ++p)
         tma_load_box(stage + sidx * C::kStageFloats + p * GBR_CH * C::SW, &in_map, &bar[sidx], x0 - RP,
-                     yin + (c + NS) * GBR_CH, NP == 1 ? pz : p);
+                     yin + (c + NS) * GBR_CH, pl0 + (NP == 1 ? pz : p));
     }
     if (c < D) continue;
     const int b = c - D;
@@ -413,7 +434,7 @@ __global__ void __launch_bounds__(128) k_roll_blur(const __grid_constant__ CUten
 #pragma unroll
     for (int o = 0; o < GBR_G; ++o) {
       const int y = yg + o;
-      if (y < ye) epi.load(x, y, pz, pre[o]);
+      if (y < ye) epi.load(x, y, n, pz, pre[o]);
     }
 #pragma unroll
     for (int o = 0; o < GBR_G; ++o) {
@@ -422,7 +443,7 @@ __global__ void __launch_bounds__(128) k_roll_blur(const __grid_constant__ CUten
       float v[NP];
 #pragma unroll
       for (int p = 0; p < NP; ++p) v[p] = res[p][o];
-      epi.apply(x, y, pz, v, pre[o]);
+      epi.apply(x, y, n, pz, v, pre[o]);
     }
   }
 }
@@ -433,7 +454,7 @@ __global__ void __launch_bounds__(128) k_roll_blur(const __grid_constant__ CUten
 //   phase 1  x pass of all NP * (TH + 2R) tile rows -> tmp (shared), 4 outputs per item
 //   phase 2  thread = column x group of 8 rows: y pass from tmp, then the epilogue, which
 //            also sees the un-blurred samples of its pixel (`sharp`, from the input tile).
-// grid (ceil(w / TW), ceil(rows / TH), 1).
+// grid (ceil(w / TW), ceil(rows / TH), 1), or (..., images) batched.
 #define GB2_TW 64
 #define GB2_TH 32
 #define GB2_G 8
@@ -448,7 +469,7 @@ struct Blur2dCfg {
   static_assert(NP == 1 || (HI * SWI * 4) % 128 == 0, "TMA destinations must be 128-byte aligned");
 };
 
-template <int R, int NP, class Epi>
+template <bool B, int R, int NP, class Epi>
 __global__ void __launch_bounds__(256) k_tma_blur_2d(const __grid_constant__ CUtensorMap in_map, const float* scale_x,
                                                      const float* scale_y, PlaneGeom g, BlurK<R> k, Epi epi) {
   typedef Blur2dCfg<R, NP> C;
@@ -458,7 +479,7 @@ __global__ void __launch_bounds__(256) k_tma_blur_2d(const __grid_constant__ CUt
   float* tmp = dyn_smem + C::kInFloats;  // [NP][HI][TW]
   uint64_t* bar = reinterpret_cast<uint64_t*>(dyn_smem + C::kInFloats + C::kTmpFloats);
   const int x0 = blockIdx.x * GB2_TW, yb = g.y0 + blockIdx.y * GB2_TH;
-  const int tid = threadIdx.x;
+  const int tid = threadIdx.x, n = batch_image<B>(g);
   if (tid == 0) {
     mbar_init(bar, 1);
     mbar_fence_init();
@@ -467,7 +488,7 @@ __global__ void __launch_bounds__(256) k_tma_blur_2d(const __grid_constant__ CUt
   if (tid == 0) {
     mbar_expect_tx(bar, C::kInFloats * 4);
 #pragma unroll
-    for (int p = 0; p < NP; ++p) tma_load_box(in + p * HI * SWI, &in_map, bar, x0 - RP, yb - R, p);
+    for (int p = 0; p < NP; ++p) tma_load_box(in + p * HI * SWI, &in_map, bar, x0 - RP, yb - R, n * g.kslot + p);
   }
   const bool edge_x = (x0 < R) || (x0 + GB2_TW + R > g.w);
   const bool edge_y = (yb < R) || (yb + GB2_TH + R > g.h);
@@ -523,7 +544,7 @@ __global__ void __launch_bounds__(256) k_tma_blur_2d(const __grid_constant__ CUt
 #pragma unroll
     for (int i = 0; i < CH; ++i) {
       const int y = yg + o0 + i;
-      if (live_col && y < g.y_end) epi.load(x, y, pre[i]);
+      if (live_col && y < g.y_end) epi.load(x, y, n, pre[i]);
     }
 #pragma unroll
     for (int i = 0; i < CH; ++i) {
@@ -536,13 +557,14 @@ __global__ void __launch_bounds__(256) k_tma_blur_2d(const __grid_constant__ CUt
       }
       // every thread calls the epilogue (it may contain warp-wide reductions); `live` tells
       // whether (x, y) is a pixel this launch must produce
-      epi.apply(x, y, live_col && y < g.y_end, sharp, v, pre[i], carry);
+      epi.apply(x, y, n, live_col && y < g.y_end, sharp, v, pre[i], carry);
     }
   }
 }
 
 // ---------------------------------------------------------------------------
-// Epilogues.  Plane groups are addressed as base + plane_index * g.plane + y * pitch + x.
+// Epilogues.  Plane groups are addressed as base + n * slot + plane_index * g.plane + y * pitch + x,
+// where n is the image of a batched launch (0 otherwise) and slot the floats per arena slot.
 
 // Each epilogue has two halves: load() fetches the pixel's global operands through the
 // read-only path into a Pre, apply() does the arithmetic and the stores.  The kernels call
@@ -550,15 +572,15 @@ __global__ void __launch_bounds__(256) k_tma_blur_2d(const __grid_constant__ CUt
 // in flight together instead of queueing behind one another's dependent stores.
 struct NoPre {};
 
-// plain store (stand-alone blur: tests, the one-time mask of the original)
+// plain store (stand-alone blur: tests, the one-time mask of the original); single image only
 struct EpiStore {
   float* out;
   int pitch;
   size_t plane;
   typedef NoPre Pre;
   static constexpr int kChunk = 16;
-  __device__ __forceinline__ void load(int, int, int, Pre&) const {}
-  __device__ __forceinline__ void apply(int x, int y, int pz, const float v[1], const Pre&) const {
+  __device__ __forceinline__ void load(int, int, int, int, Pre&) const {}
+  __device__ __forceinline__ void apply(int x, int y, int, int pz, const float v[1], const Pre&) const {
     out[pz * plane + static_cast<size_t>(y) * pitch + x] = v[0];
   }
 };
@@ -569,16 +591,16 @@ struct EpiLf {
   float* lf;
   float* mf_in;
   int pitch;
-  size_t plane;
+  size_t plane, slot;
   struct Pre {
     float a;
   };
   static constexpr int kChunk = 8;
-  __device__ __forceinline__ void load(int x, int y, int pz, Pre& p) const {
-    p.a = __ldg(xyb + pz * plane + static_cast<size_t>(y) * pitch + x);
+  __device__ __forceinline__ void load(int x, int y, int n, int pz, Pre& p) const {
+    p.a = __ldg(xyb + n * slot + pz * plane + static_cast<size_t>(y) * pitch + x);
   }
-  __device__ __forceinline__ void apply(int x, int y, int pz, const float v[1], const Pre& p) const {
-    const size_t o = pz * plane + static_cast<size_t>(y) * pitch + x;
+  __device__ __forceinline__ void apply(int x, int y, int n, int pz, const float v[1], const Pre& p) const {
+    const size_t o = n * slot + pz * plane + static_cast<size_t>(y) * pitch + x;
     lf[o] = v[0];
     mf_in[o] = p.a - v[0];
   }
@@ -595,13 +617,13 @@ struct EpiMf {
   float* diffs;        // [6]: X uhf, hf, mf; Y uhf, hf, mf
   MaltaParams mp_x, mp_y;
   int pitch;
-  size_t plane;
+  size_t plane, slot;
   struct Pre {
     float inx, iny, p0x, p0y;
   };
   static constexpr int kChunk = 8;
-  __device__ __forceinline__ void load(int x, int y, int, Pre& p) const {
-    const size_t o = static_cast<size_t>(y) * pitch + x;
+  __device__ __forceinline__ void load(int x, int y, int n, int, Pre& p) const {
+    const size_t o = n * slot + static_cast<size_t>(y) * pitch + x;
     p.inx = __ldg(mf_in + o);
     p.iny = __ldg(mf_in + plane + o);
     if (ps0 != nullptr) {
@@ -609,8 +631,8 @@ struct EpiMf {
       p.p0y = __ldg(ps0 + kMfY * plane + o);
     }
   }
-  __device__ __forceinline__ void apply(int x, int y, int, const float v[3], const Pre& p) const {
-    const size_t o = static_cast<size_t>(y) * pitch + x;
+  __device__ __forceinline__ void apply(int x, int y, int n, int, const float v[3], const Pre& p) const {
+    const size_t o = n * slot + static_cast<size_t>(y) * pitch + x;
     const float mbx = v[0], mby = v[1];
     const float hx = p.inx - mbx;
     const float hy = p.iny - mby;
@@ -635,14 +657,14 @@ struct EpiMf {
 struct EpiOpsin {
   float* xyb;
   int pitch;
-  size_t plane;
+  size_t plane, slot;
   typedef NoPre Pre;
   static constexpr int kChunk = 8;
-  __device__ __forceinline__ void load(int, int, Pre&) const {}
-  __device__ __forceinline__ void apply(int x, int y, bool live, const float sharp[3], const float v[3], const Pre&,
+  __device__ __forceinline__ void load(int, int, int, Pre&) const {}
+  __device__ __forceinline__ void apply(int x, int y, int n, bool live, const float sharp[3], const float v[3], const Pre&,
                                         float&) const {
     if (!live) return;
-    const size_t o = static_cast<size_t>(y) * pitch + x;
+    const size_t o = n * slot + static_cast<size_t>(y) * pitch + x;
     opsin_pixel(sharp[0], sharp[1], sharp[2], v[0], v[1], v[2], &xyb[o], &xyb[plane + o], &xyb[2 * plane + o]);
   }
 };
@@ -658,13 +680,13 @@ struct EpiHf {
   float* noise;         // [1]
   MaltaParams mp_uhf_x, mp_uhf_y, mp_hf_x, mp_hf_y;
   int pitch;
-  size_t plane;
+  size_t plane, slot;
   struct Pre {
     float lfx, lfy, lfb, u0x, h0x, u0y, h0y;
   };
   static constexpr int kChunk = 4;
-  __device__ __forceinline__ void load(int x, int y, Pre& p) const {
-    const size_t o = static_cast<size_t>(y) * pitch + x;
+  __device__ __forceinline__ void load(int x, int y, int n, Pre& p) const {
+    const size_t o = n * slot + static_cast<size_t>(y) * pitch + x;
     p.lfx = __ldg(lf_raw + o);
     p.lfy = __ldg(lf_raw + plane + o);
     p.lfb = __ldg(lf_raw + 2 * plane + o);
@@ -675,10 +697,10 @@ struct EpiHf {
       p.h0y = __ldg(ps0 + kHfY * plane + o);
     }
   }
-  __device__ __forceinline__ void apply(int x, int y, bool live, const float sharp[2], const float v[2], const Pre& p,
-                                        float&) const {
+  __device__ __forceinline__ void apply(int x, int y, int n, bool live, const float sharp[2], const float v[2],
+                                        const Pre& p, float&) const {
     if (!live) return;
-    const size_t o = static_cast<size_t>(y) * pitch + x;
+    const size_t o = n * slot + static_cast<size_t>(y) * pitch + x;
     const float uhfx = sharp[0] - v[0];
     const float hfx = remove_range_around_zero(static_cast<float>(0.0287615200377), v[0]);
     const float lfx = p.lfx, lfy = p.lfy, lfb = p.lfb;
@@ -731,18 +753,19 @@ struct EpiNoise {
   float* acc;        // block_diff_ac[Y], read-modify-write (each pixel by exactly one thread)
   double w_0gt1, w_0lt1;
   int pitch;
+  size_t slot;
   struct Pre {
     float r0, r1, a;
   };
   static constexpr int kChunk = 8;
-  __device__ __forceinline__ void load(int x, int y, int, Pre& p) const {
-    const size_t o = static_cast<size_t>(y) * pitch + x;
+  __device__ __forceinline__ void load(int x, int y, int n, int, Pre& p) const {
+    const size_t o = n * slot + static_cast<size_t>(y) * pitch + x;
     p.r0 = __ldg(hf0 + o);
     p.r1 = __ldg(hf1 + o);
     p.a = acc[o];  // plain load: this launch writes the location later (same thread)
   }
-  __device__ __forceinline__ void apply(int x, int y, int, const float v[1], const Pre& p) const {
-    const size_t o = static_cast<size_t>(y) * pitch + x;
+  __device__ __forceinline__ void apply(int x, int y, int n, int, const float v[1], const Pre& p) const {
+    const size_t o = n * slot + static_cast<size_t>(y) * pitch + x;
     float a = p.a;
     {
       const double w = 884.809801415;
@@ -781,24 +804,27 @@ struct EpiNoise {
 // mixed with the sharp one; the lanes of an 8x8 block reduce their maximum with warp
 // shuffles (a thread holds 8 rows of one column, 8 adjacent lanes hold the block's
 // columns), and one lane per block stores it and folds it into the global maximum
-// (non-negative floats order like their bit patterns).
+// (non-negative floats order like their bit patterns).  Image n of a batch has its own
+// block_max (n * nblocks on) and global maximum (gmax[n]).
 struct EpiFinal {
   float* distmap;
   float* block_max;     // [nblocks], written for block rows [by_lo, by_hi)
   unsigned int* gmax;   // global maximum (float bits), or nullptr
   int pitch, bw, by_lo, by_hi;
+  size_t slot;
+  int nblocks;
   typedef NoPre Pre;
   static constexpr int kChunk = 8;
-  __device__ __forceinline__ void load(int, int, Pre&) const {}
+  __device__ __forceinline__ void load(int, int, int, Pre&) const {}
   // m: running maximum of the thread's pixels of the current block row (one block column)
-  __device__ __forceinline__ void apply(int x, int y, bool live, const float sharp[1], const float v[1], const Pre&,
-                                        float& m) const {
+  __device__ __forceinline__ void apply(int x, int y, int n, bool live, const float sharp[1], const float v[1],
+                                        const Pre&, float& m) const {
     if (live) {
       const double mul1 = 0.458794906198;
       const float scale = static_cast<float>(1.0f / (1.0f + mul1));
       float d = static_cast<float>(static_cast<double>(sharp[0]) + mul1 * v[0]);
       d *= scale;
-      distmap[static_cast<size_t>(y) * pitch + x] = d;
+      distmap[n * slot + static_cast<size_t>(y) * pitch + x] = d;
       m = (y & 7) == 0 ? hd_max(0.0f, d) : hd_max(m, d);
     } else if ((y & 7) == 0) {
       m = 0.0f;
@@ -810,8 +836,8 @@ struct EpiFinal {
       b = hd_max(b, __shfl_xor_sync(0xffffffffu, b, 4));
       const int by = y >> 3, bx = x >> 3;
       if ((x & 7) == 0 && bx < bw && by >= by_lo && by < by_hi) {
-        block_max[by * bw + bx] = b;
-        if (gmax != nullptr) atomicMax(gmax, __float_as_uint(b));
+        (block_max + static_cast<size_t>(n) * nblocks)[by * bw + bx] = b;
+        if (gmax != nullptr) atomicMax(gmax + n, __float_as_uint(b));
       }
     }
   }
@@ -855,7 +881,8 @@ struct CombineArgs {
   size_t plane;
 };
 
-template <int RA, int RB, int RC>
+// grid (ceil(w / TW), ceil(rows / TH), 1), or (..., images) batched.
+template <bool B, int RA, int RB, int RC>
 __global__ void __launch_bounds__(256) k_tma_mask_y(const __grid_constant__ CUtensorMap map_a,
                                                     const __grid_constant__ CUtensorMap map_b,
                                                     const __grid_constant__ CUtensorMap map_c, const float* sya,
@@ -868,6 +895,8 @@ __global__ void __launch_bounds__(256) k_tma_mask_y(const __grid_constant__ CUte
   float* tc = tb + C::HB * GBY_TW;
   uint64_t* bar = reinterpret_cast<uint64_t*>(tc + C::HC * GBY_TW);
   const int x0 = blockIdx.x * GBY_TW, yb = g.y0 + blockIdx.y * GBY_TH;
+  const int n = batch_image<B>(g);
+  const size_t so = slot_offset(g, n);
   if (threadIdx.x == 0) {
     mbar_init(bar, 1);
     mbar_fence_init();
@@ -875,9 +904,9 @@ __global__ void __launch_bounds__(256) k_tma_mask_y(const __grid_constant__ CUte
   __syncthreads();
   if (threadIdx.x == 0) {
     mbar_expect_tx(bar, (C::HA + C::HB + C::HC) * GBY_TW * 4);
-    tma_load_box(ta, &map_a, bar, x0, yb - RA, 0);
-    tma_load_box(tb, &map_b, bar, x0, yb - RB, 0);
-    tma_load_box(tc, &map_c, bar, x0, yb - RC, 0);
+    tma_load_box(ta, &map_a, bar, x0, yb - RA, n * g.kslot);
+    tma_load_box(tb, &map_b, bar, x0, yb - RB, n * g.kslot);
+    tma_load_box(tc, &map_c, bar, x0, yb - RC, n * g.kslot);
   }
   const int c = threadIdx.x & (GBY_TW - 1), grp = threadIdx.x >> 7;
   const int x = x0 + c, yg = yb + GBY_G * grp;
@@ -899,10 +928,10 @@ __global__ void __launch_bounds__(256) k_tma_mask_y(const __grid_constant__ CUte
   }
   if (x >= g.w) return;
   CombineAndSqrt comb;
-  comb.ps0 = ca.ps0;
-  comb.ps1 = ca.ps1;
-  comb.ac = ca.ac;
-  comb.out = ca.out;
+  comb.ps0 = ca.ps0 + so;
+  comb.ps1 = ca.ps1 + so;
+  comb.ac = ca.ac + so;
+  comb.out = ca.out + so;
   comb.luts = ca.luts;
   comb.g.pitch = ca.pitch;
   comb.g.plane = ca.plane;
@@ -914,7 +943,7 @@ __global__ void __launch_bounds__(256) k_tma_mask_y(const __grid_constant__ CUte
     for (int i = 0; i < CH; ++i) {
       const int y = yg + o0 + i;
       if (y >= g.y_end) continue;
-      const size_t o = static_cast<size_t>(y) * ca.pitch + x;
+      const size_t o = so + static_cast<size_t>(y) * ca.pitch + x;
       l0x[i] = __ldg(ca.ps0 + kLfX * ca.plane + o);
       l0b[i] = __ldg(ca.ps0 + kLfB * ca.plane + o);
       l1x[i] = __ldg(ca.ps1 + kLfX * ca.plane + o);
@@ -938,14 +967,17 @@ __global__ void __launch_bounds__(256) k_tma_mask_y(const __grid_constant__ CUte
 // copied as 72 x 40 boxes by the TMA unit, double-buffered over the three bands; the zero
 // fill outside the image is PaddedMaltaUnit's padding.  Line sums as in k_malta_sums
 // (tiled_kernels.cuh): a thread evaluates 2 x 4 pixels from a 9 x 12 register window.
-// grid (ceil(w / 64), ceil(rows / 32), 2 channels), 256 threads.
+// grid (ceil(w / 64), ceil(rows / 32), 2 channels), times the images of a batched launch; 256 threads.
+template <bool B>
 __global__ void __launch_bounds__(256, 2) k_tma_malta_sums(const __grid_constant__ CUtensorMap diffs_map, float* acc,
                                                            PlaneGeom g) {
   __shared__ __align__(128) float tile[2][GB_MALTA_SH * GB_MALTA_SW];
   __shared__ __align__(8) uint64_t bar[2];
   const int tx = threadIdx.x, ty = threadIdx.y;  // 16 x 16
   const int tid = ty * 16 + tx;
-  const int x0 = blockIdx.x * GB_MALTA_TILE_W, y0 = g.y0 + blockIdx.y * GB_MALTA_TILE_H, ch = blockIdx.z;
+  const int n = B ? static_cast<int>(blockIdx.z) >> 1 : 0;
+  const int x0 = blockIdx.x * GB_MALTA_TILE_W, y0 = g.y0 + blockIdx.y * GB_MALTA_TILE_H;
+  const int ch = B ? blockIdx.z & 1 : blockIdx.z, pl = n * g.kslot + 3 * ch;  // first plane of the channel's bands
   constexpr uint32_t kBytes = GB_MALTA_SH * GB_MALTA_SW * 4;
   if (tid == 0) {
     mbar_init(&bar[0], 1);
@@ -955,9 +987,9 @@ __global__ void __launch_bounds__(256, 2) k_tma_malta_sums(const __grid_constant
   __syncthreads();
   if (tid == 0) {
     mbar_expect_tx(&bar[0], kBytes);
-    tma_load_box(tile[0], &diffs_map, &bar[0], x0 - 4, y0 - 4, 3 * ch + 0);
+    tma_load_box(tile[0], &diffs_map, &bar[0], x0 - 4, y0 - 4, pl + 0);
     mbar_expect_tx(&bar[1], kBytes);
-    tma_load_box(tile[1], &diffs_map, &bar[1], x0 - 4, y0 - 4, 3 * ch + 1);
+    tma_load_box(tile[1], &diffs_map, &bar[1], x0 - 4, y0 - 4, pl + 1);
   }
   float r[2][4];
 #pragma unroll
@@ -970,7 +1002,7 @@ __global__ void __launch_bounds__(256, 2) k_tma_malta_sums(const __grid_constant
   __syncthreads();  // everybody is done with buffer 0
   if (tid == 0) {
     mbar_expect_tx(&bar[0], kBytes);
-    tma_load_box(tile[0], &diffs_map, &bar[0], x0 - 4, y0 - 4, 3 * ch + 2);
+    tma_load_box(tile[0], &diffs_map, &bar[0], x0 - 4, y0 - 4, pl + 2);
   }
   // band 1 (hf) from buffer 1, band 2 (mf) from buffer 0 again
   mbar_wait(&bar[1], 0);
@@ -978,7 +1010,7 @@ __global__ void __launch_bounds__(256, 2) k_tma_malta_sums(const __grid_constant
   mbar_wait(&bar[0], 1);
   malta_window_sums(tile[0], tx, ty, false, r);
   const int xb = x0 + 4 * tx;
-  float* aplane = acc + static_cast<size_t>(ch) * g.plane;
+  float* aplane = acc + slot_offset(g, n) + static_cast<size_t>(ch) * g.plane;
 #pragma unroll
   for (int k = 0; k < 2; ++k) {
     const int y = y0 + ty + 16 * k;
@@ -1008,9 +1040,14 @@ __device__ __forceinline__ float mask_combo_y(float uhf, float hf) {
 
 // sup = |v - v_right| + |v - v_down| (float magnitudes, float sum, widened by the consumer),
 // neighbours mirrored at the last column / row; one plane per channel: sup[0] = X, sup[1] = Y.
+// grid (ceil(w / 32), ceil(rows / 8), 1), or (..., images) batched; 32 x 8 threads.
+template <bool B>
 __global__ void __launch_bounds__(256) k_mask_sup(const float* ps, float* sup, PlaneGeom g) {
   const int x = blockIdx.x * 32 + threadIdx.x, y = g.y0 + blockIdx.y * 8 + threadIdx.y;
   if (x >= g.w || y >= g.y_end) return;
+  const size_t so = slot_offset(g, batch_image<B>(g));
+  ps += so;
+  sup += so;
   const int x2 = (x + 1 < g.w) ? x + 1 : (x > 0 ? x - 1 : x);
   const int y2 = (y + 1 < g.h) ? y + 1 : (y > 0 ? y - 1 : y);
   const size_t o = static_cast<size_t>(y) * g.pitch + x;
@@ -1025,10 +1062,15 @@ __global__ void __launch_bounds__(256) k_mask_sup(const float* ps, float* sup, P
   sup[g.plane + o] = hd_fabsf(b - bx) + hd_fabsf(b - by);
 }
 
-// mpre[c] = min(cutoff, mul0 * min(sup0_c, sup1_c)) for c = X, Y.
+// mpre[c] = min(cutoff, mul0 * min(sup0_c, sup1_c)) for c = X, Y.  Grid as k_mask_sup.
+template <bool B>
 __global__ void __launch_bounds__(256) k_mask_pre(const float* ps1, const float* sup0, float* mpre, PlaneGeom g) {
   const int x = blockIdx.x * 32 + threadIdx.x, y = g.y0 + blockIdx.y * 8 + threadIdx.y;
   if (x >= g.w || y >= g.y_end) return;
+  const size_t so = slot_offset(g, batch_image<B>(g));
+  ps1 += so;
+  sup0 += so;
+  mpre += so;
   const int x2 = (x + 1 < g.w) ? x + 1 : (x > 0 ? x - 1 : x);
   const int y2 = (y + 1 < g.h) ? y + 1 : (y > 0 ? y - 1 : y);
   const size_t o = static_cast<size_t>(y) * g.pitch + x;

@@ -17,6 +17,7 @@
 #include <mutex>
 #include <set>
 #include <tuple>
+#include <type_traits>
 
 #include "tiled_kernels.cuh"
 #include "zeroing_warp.cuh"
@@ -27,7 +28,7 @@
 namespace gb200 {
 
 #if defined(GB200_HOSTSIM)
-void ImageContext::fused_sup0() {}
+void ImageContext::fused_sup0(int, int) {}
 static void select_device(int) {}
 static Stream make_stream() { return 0; }
 static void destroy_stream(Stream) {}
@@ -126,6 +127,12 @@ struct ImageContext::Fused {
       it = maps.insert(std::make_pair(key, make_plane_map(base, g.w, g.h, g.pitch, g.plane, nplanes, box_w, box_h))).first;
     return it->second;
   }
+  // a group of nplanes planes in each of the `capacity` arena slots of a batched context, kslot
+  // planes apart (kslot = 0: the group alone)
+  int capacity = 1;
+  const CUtensorMap& slots(const float* base, int nplanes, int box_w, int box_h, int kslot, const Geom& g) {
+    return map(base, (capacity - 1) * kslot + nplanes, box_w, box_h, g);
+  }
 };
 
 namespace {
@@ -163,48 +170,76 @@ void allow_smem(K kernel, size_t bytes) {
 
 inline int cdiv(int a, int b) { return (a + b - 1) / b; }
 
+// f(std::true_type()) for a launch over several images (the kernels' batched instantiation, which
+// takes the image from blockIdx.z), f(std::false_type()) for one image.  EpiStore (stand-alone
+// blurs) has no batched form.
+template <class Epi, class F>
+void with_batch(int nimg, const F& f) {
+  if constexpr (!std::is_same<Epi, EpiStore>::value) {
+    if (nimg > 1) {
+      f(std::true_type());
+      return;
+    }
+  }
+  if (nimg != 1) throw std::runtime_error("with_batch: no batched form of this launch");
+  f(std::false_type());
+}
+
 // Rolling-window blur of a plane group with epilogue (k_roll_blur); `in_map` has boxes of
 // RollCfg<R, NP>::SW x GBR_CH.  The launch's rows are cut into segments of whole steps of
-// about GBR_SEG rows.
+// about GBR_SEG rows.  nimg images: arena slots 0 .. nimg - 1 (PlaneGeom::kslot).
 template <int R, int NP, class Epi>
-void launch_roll(Stream s, const CUtensorMap& in_map, int planes_z, const BlurTab& tab, const PlaneGeom& pg,
+void launch_roll(Stream s, const CUtensorMap& in_map, int planes_z, int nimg, const BlurTab& tab, PlaneGeom pg,
                  const HostTables& ht, int id, const Epi& epi, const char* name) {
   const int rows = pg.y_end - pg.y0;
   if (rows <= 0) return;
   typedef RollCfg<R, NP> C;
-  allow_smem(k_roll_blur<R, NP, Epi>, C::kSmemBytes);
   const int nseg = cdiv(rows, GBR_SEG);
   const int seg = cdiv(cdiv(rows, nseg), GBR_CH) * GBR_CH;
-  dim3 grid(cdiv(pg.w, GBR_TW), cdiv(rows, seg), planes_z);
-  note_launch(name, s, static_cast<double>(pg.w) * rows * (NP == 1 ? planes_z : NP));
-  k_roll_blur<R, NP, Epi><<<grid, 128, C::kSmemBytes, s>>>(in_map, tab.scale_x, tab.scale_y, pg, seg,
-                                                           make_blurk<R>(ht, id), epi);
+  pg.zimg = planes_z;
+  dim3 grid(cdiv(pg.w, GBR_TW), cdiv(rows, seg), planes_z * nimg);
+  note_launch(name, s, static_cast<double>(pg.w) * rows * (NP == 1 ? planes_z : NP) * nimg);
+  with_batch<Epi>(nimg, [&](auto b) {
+    constexpr bool B = decltype(b)::value;
+    allow_smem(k_roll_blur<B, R, NP, Epi>, C::kSmemBytes);
+    k_roll_blur<B, R, NP, Epi><<<grid, 128, C::kSmemBytes, s>>>(in_map, tab.scale_x, tab.scale_y, pg, seg,
+                                                                make_blurk<R>(ht, id), epi);
+  });
   note_launch_end(name, s);
 }
 
 template <int R, int NP, class Epi>
-void launch_tma_y(Stream s, const CUtensorMap& in_map, int planes_z, const BlurTab& tab, const PlaneGeom& pg,
+void launch_tma_y(Stream s, const CUtensorMap& in_map, int planes_z, int nimg, const BlurTab& tab, PlaneGeom pg,
                   const HostTables& ht, int id, const Epi& epi, const char* name) {
   const int rows = pg.y_end - pg.y0;
   if (rows <= 0) return;
   const size_t smem = static_cast<size_t>(NP) * (GBY_TH + 2 * R) * GBY_TW * sizeof(float) + 16;
-  allow_smem(k_tma_blur_y<R, NP, Epi>, smem);
-  dim3 grid(cdiv(pg.w, GBY_TW), cdiv(rows, GBY_TH), planes_z);
-  note_launch(name, s, static_cast<double>(pg.w) * rows * (NP == 1 ? planes_z : NP));
-  k_tma_blur_y<R, NP, Epi><<<grid, 256, smem, s>>>(in_map, tab.scale_y, pg, make_blurk<R>(ht, id), epi);
+  pg.zimg = planes_z;
+  dim3 grid(cdiv(pg.w, GBY_TW), cdiv(rows, GBY_TH), planes_z * nimg);
+  note_launch(name, s, static_cast<double>(pg.w) * rows * (NP == 1 ? planes_z : NP) * nimg);
+  with_batch<Epi>(nimg, [&](auto b) {
+    constexpr bool B = decltype(b)::value;
+    allow_smem(k_tma_blur_y<B, R, NP, Epi>, smem);
+    k_tma_blur_y<B, R, NP, Epi><<<grid, 256, smem, s>>>(in_map, tab.scale_y, pg, make_blurk<R>(ht, id), epi);
+  });
   note_launch_end(name, s);
 }
 
 template <int R, int NP, class Epi>
-void launch_tma_2d(Stream s, const CUtensorMap& in_map, const BlurTab& tab, const PlaneGeom& pg, const HostTables& ht,
-                   int id, const Epi& epi, const char* name) {
+void launch_tma_2d(Stream s, const CUtensorMap& in_map, int nimg, const BlurTab& tab, PlaneGeom pg,
+                   const HostTables& ht, int id, const Epi& epi, const char* name) {
   const int rows = pg.y_end - pg.y0;
   if (rows <= 0) return;
   typedef Blur2dCfg<R, NP> C;
-  allow_smem(k_tma_blur_2d<R, NP, Epi>, C::kSmemBytes);
-  dim3 grid(cdiv(pg.w, GB2_TW), cdiv(rows, GB2_TH), 1);
-  note_launch(name, s, static_cast<double>(pg.w) * rows);
-  k_tma_blur_2d<R, NP, Epi><<<grid, 256, C::kSmemBytes, s>>>(in_map, tab.scale_x, tab.scale_y, pg, make_blurk<R>(ht, id), epi);
+  pg.zimg = 1;
+  dim3 grid(cdiv(pg.w, GB2_TW), cdiv(rows, GB2_TH), nimg);
+  note_launch(name, s, static_cast<double>(pg.w) * rows * nimg);
+  with_batch<Epi>(nimg, [&](auto b) {
+    constexpr bool B = decltype(b)::value;
+    allow_smem(k_tma_blur_2d<B, R, NP, Epi>, C::kSmemBytes);
+    k_tma_blur_2d<B, R, NP, Epi><<<grid, 256, C::kSmemBytes, s>>>(in_map, tab.scale_x, tab.scale_y, pg,
+                                                                  make_blurk<R>(ht, id), epi);
+  });
   note_launch_end(name, s);
 }
 }  // namespace
@@ -220,22 +255,30 @@ void launch_tma_2d(Stream s, const CUtensorMap& in_map, const BlurTab& tab, cons
 #define GB_R_MASKY1 20
 #define GB_R_FINAL 3
 
-void ImageContext::fused_opsin(const float* lin, float* xyb) {
-  const PlaneGeom pg{g_.w, g_.h, g_.pitch, g_.plane, cr_lo_, cr_hi_};
+// Launches over nimg images take the planes of arena slots 0 .. nimg - 1, kslot planes apart
+// (kslot = 0 and nimg = 1 for a single-image context); their tensor maps cover every slot.
+namespace {
+PlaneGeom fused_geom(const Geom& g, int y0, int y_end, int kslot) {
+  return PlaneGeom{g.w, g.h, g.pitch, g.plane, y0, y_end, kslot, 1};
+}
+}  // namespace
+
+void ImageContext::fused_opsin(const float* lin, float* xyb, int nimg, int kslot) {
+  const PlaneGeom pg = fused_geom(g_, cr_lo_, cr_hi_, kslot);
   typedef Blur2dCfg<GB_R_OPSIN, 3> C;
-  const CUtensorMap& m = fused_->map(lin, 3, C::SWI, C::HI, g_);
-  launch_tma_2d<GB_R_OPSIN, 3>(s_, m, t_.blur[kBlurOpsin], pg, ht_, kBlurOpsin, EpiOpsin{xyb, g_.pitch, g_.plane},
-                               "opsin_fused");
+  const CUtensorMap& m = fused_->slots(lin, 3, C::SWI, C::HI, kslot, g_);
+  launch_tma_2d<GB_R_OPSIN, 3>(s_, m, nimg, t_.blur[kBlurOpsin], pg, ht_, kBlurOpsin,
+                               EpiOpsin{xyb, g_.pitch, g_.plane, kslot * g_.plane}, "opsin_fused");
 }
 
 // SeparateFrequencies; with_diffs: also the Malta pre-pass and the noise difference against ps0_.
-void ImageContext::fused_separate(const float* xyb, float* ps, bool with_diffs) {
-  const PlaneGeom pg{g_.w, g_.h, g_.pitch, g_.plane, cr_lo_, cr_hi_};
-  const size_t P = g_.plane;
+void ImageContext::fused_separate(const float* xyb, float* ps, bool with_diffs, int nimg, int kslot) {
+  const PlaneGeom pg = fused_geom(g_, cr_lo_, cr_hi_, kslot);
+  const size_t P = g_.plane, S = kslot * P;
   // S2: lf = Blur(xyb, 7.47); mf_in = xyb - lf
   // (launch names are those of the former y-pass kernels, which these replace)
-  launch_roll<GB_R_LF, 1>(s_, fused_->map(xyb, 3, RollCfg<GB_R_LF, 1>::SW, GBR_CH, g_), 3, t_.blur[kBlurLf], pg, ht_, kBlurLf,
-                          EpiLf{xyb, lf_, mf_in_, g_.pitch, P}, "lf_fused_y");
+  launch_roll<GB_R_LF, 1>(s_, fused_->slots(xyb, 3, RollCfg<GB_R_LF, 1>::SW, GBR_CH, kslot, g_), 3, nimg, t_.blur[kBlurLf], pg, ht_,
+                          kBlurLf, EpiLf{xyb, lf_, mf_in_, g_.pitch, P, S}, "lf_fused_y");
   // S3 + S4: mf = Blur(mf_in, 3.73); split, range tweaks, SuppressXByY (+ Malta pre-pass of the mf bands)
   EpiMf em;
   em.mf_in = mf_in_;
@@ -247,8 +290,9 @@ void ImageContext::fused_separate(const float* xyb, float* ps, bool with_diffs) 
   em.mp_y = malta_[4];
   em.pitch = g_.pitch;
   em.plane = P;
-  launch_roll<GB_R_MF, 3>(s_, fused_->map(mf_in_, 3, RollCfg<GB_R_MF, 3>::SW, GBR_CH, g_), 1, t_.blur[kBlurMf], pg, ht_, kBlurMf,
-                          em, "mf_fused_y");
+  em.slot = S;
+  launch_roll<GB_R_MF, 3>(s_, fused_->slots(mf_in_, 3, RollCfg<GB_R_MF, 3>::SW, GBR_CH, kslot, g_), 1, nimg, t_.blur[kBlurMf], pg,
+                          ht_, kBlurMf, em, "mf_fused_y");
   // S5 + S6: hf = Blur(hf_raw, 1.87) in one kernel; uhf / hf / lf "vals" (+ Malta pre-pass, noise difference)
   EpiHf eh;
   eh.lf_raw = lf_;
@@ -262,29 +306,31 @@ void ImageContext::fused_separate(const float* xyb, float* ps, bool with_diffs) 
   eh.mp_hf_x = malta_[3];
   eh.pitch = g_.pitch;
   eh.plane = P;
+  eh.slot = S;
   typedef Blur2dCfg<GB_R_HF, 2> C;
-  launch_tma_2d<GB_R_HF, 2>(s_, fused_->map(hf_raw_, 2, C::SWI, C::HI, g_), t_.blur[kBlurHf], pg, ht_, kBlurHf, eh, "hf_fused");
+  launch_tma_2d<GB_R_HF, 2>(s_, fused_->slots(hf_raw_, 2, C::SWI, C::HI, kslot, g_), nimg, t_.blur[kBlurHf], pg, ht_, kBlurHf, eh,
+                            "hf_fused");
 }
 
 // Neighbour sums of DiffPrecompute for the original's PsychoImage (constant during the search).
-void ImageContext::fused_sup0() {
+void ImageContext::fused_sup0(int nimg, int kslot) {
   if (!use_fused_) return;
-  const PlaneGeom pg{g_.w, g_.h, g_.pitch, g_.plane, cr_lo_, cr_hi_};
+  const PlaneGeom pg = fused_geom(g_, cr_lo_, cr_hi_, kslot);
   const int rows = cr_hi_ - cr_lo_;
-  dim3 block(32, 8), grid(cdiv(g_.w, 32), cdiv(rows, 8));
-  note_launch("mask_sup0", s_, static_cast<double>(g_.w) * rows);
-  k_mask_sup<<<grid, block, 0, s_>>>(ps0_, sup0_, pg);
+  dim3 block(32, 8), grid(cdiv(g_.w, 32), cdiv(rows, 8), nimg);
+  note_launch("mask_sup0", s_, static_cast<double>(g_.w) * rows * nimg);
+  with_batch<void>(nimg, [&](auto b) { k_mask_sup<decltype(b)::value><<<grid, block, 0, s_>>>(ps0_, sup0_, pg); });
   note_launch_end("mask_sup0", s_);
 }
 
 // One separable blur of a plane group (tests, one-time mask of the original).
 void ImageContext::fused_blur(const float* in, float* out, int nplanes, int id) {
-  const PlaneGeom pg{g_.w, g_.h, g_.pitch, g_.plane, cr_lo_, cr_hi_};
+  const PlaneGeom pg = fused_geom(g_, cr_lo_, cr_hi_, 0);
   const EpiStore st{out, g_.pitch, g_.plane};
 #define GB_BLUR_CASE(R)                                                                                               \
   case R:                                                                                                             \
-    launch_roll<R, 1>(s_, fused_->map(in, nplanes, RollCfg<R, 1>::SW, GBR_CH, g_), nplanes, t_.blur[id], pg, ht_, id, st, \
-                      "tma_blur_y");                                                                                  \
+    launch_roll<R, 1>(s_, fused_->map(in, nplanes, RollCfg<R, 1>::SW, GBR_CH, g_), nplanes, 1, t_.blur[id], pg, ht_, id, \
+                      st, "tma_blur_y");                                                                              \
     break;
   switch (t_.blur[id].r) {
     GB_BLUR_CASE(2)
@@ -330,7 +376,7 @@ void ImageContext::fused_compare_submit() {
     GB_CUDA(cudaStreamBeginCapture(s_, cudaStreamCaptureModeThreadLocal));
     cudaGraph_t graph = nullptr;
     try {
-      fused_compare_launches();
+      fused_compare_launches(1, 0);
     } catch (...) {
       cudaStreamEndCapture(s_, &graph);
       if (graph) cudaGraphDestroy(graph);
@@ -346,7 +392,7 @@ void ImageContext::fused_compare_submit() {
     GB_CUDA(cudaGraphLaunch(fused_->compare_graph, s_));
     add_launches(recorded);
   } else {
-    fused_compare_launches();
+    fused_compare_launches(1, 0);
   }
   ++fused_->compare_calls;
 }
@@ -369,17 +415,17 @@ float ImageContext::fused_compare_result() {
 }
 
 // the stream work of one Compare after the render: no host synchronisation inside
-void ImageContext::fused_compare_launches() {
-  const PlaneGeom pg{g_.w, g_.h, g_.pitch, g_.plane, cr_lo_, cr_hi_};
-  const size_t P = g_.plane;
+void ImageContext::fused_compare_launches(int nimg, int kslot) {
+  const PlaneGeom pg = fused_geom(g_, cr_lo_, cr_hi_, kslot);
+  const size_t P = g_.plane, S = kslot * P;
   const int rows = cr_hi_ - cr_lo_;
-  fused_opsin(lin_, xyb_);
-  fused_separate(xyb_, ps1_, true);
+  fused_opsin(lin_, xyb_, nimg, kslot);
+  fused_separate(xyb_, ps1_, true, nimg, kslot);
   // S10 mask: DiffPrecompute against the original's resident neighbour sums
   {
-    dim3 block(32, 8), grid(cdiv(g_.w, 32), cdiv(rows, 8));
-    note_launch("mask_pre", s_, static_cast<double>(g_.w) * rows);
-    k_mask_pre<<<grid, block, 0, s_>>>(ps1_, sup0_, mpre_, pg);
+    dim3 block(32, 8), grid(cdiv(g_.w, 32), cdiv(rows, 8), nimg);
+    note_launch("mask_pre", s_, static_cast<double>(g_.w) * rows * nimg);
+    with_batch<void>(nimg, [&](auto b) { k_mask_pre<decltype(b)::value><<<grid, block, 0, s_>>>(ps1_, sup0_, mpre_, pg); });
     note_launch_end("mask_pre", s_);
   }
   // x passes of the noise blur (S8) and of the three mask blurs in one launch:
@@ -399,47 +445,57 @@ void ImageContext::fused_compare_launches() {
     xa.k1 = make_blurk<GB_R_MASKX>(ht_, kBlurMaskX);
     xa.k2 = make_blurk<GB_R_MASKY1>(ht_, kBlurMaskY1);
     xa.k3 = make_blurk<GB_R_MASKY0>(ht_, kBlurMaskY0);
-    dim3 grid(cdiv(g_.w, GBX_TW), cdiv(rows, GBX_TH), 4);
-    note_launch("tma_blur_x", s_, 4.0 * g_.w * rows);
-    k_tma_blur_x4<GB_R_NOISE, GB_R_MASKX, GB_R_MASKY1, GB_R_MASKY0><<<grid, 128, 0, s_>>>(
-        fused_->map(noise_, 1, BlurXCfg<GB_R_NOISE>::SW, GBX_TH, g_), fused_->map(mpre_, 1, BlurXCfg<GB_R_MASKX>::SW, GBX_TH, g_),
-        fused_->map(mpre_ + P, 1, BlurXCfg<GB_R_MASKY1>::SW, GBX_TH, g_),
-        fused_->map(mpre_ + P, 1, BlurXCfg<GB_R_MASKY0>::SW, GBX_TH, g_), pg, xa);
+    dim3 grid(cdiv(g_.w, GBX_TW), cdiv(rows, GBX_TH), 4 * nimg);
+    note_launch("tma_blur_x", s_, 4.0 * g_.w * rows * nimg);
+    with_batch<void>(nimg, [&](auto b) {
+      k_tma_blur_x4<decltype(b)::value, GB_R_NOISE, GB_R_MASKX, GB_R_MASKY1, GB_R_MASKY0><<<grid, 128, 0, s_>>>(
+          fused_->slots(noise_, 1, BlurXCfg<GB_R_NOISE>::SW, GBX_TH, kslot, g_),
+          fused_->slots(mpre_, 1, BlurXCfg<GB_R_MASKX>::SW, GBX_TH, kslot, g_),
+          fused_->slots(mpre_ + P, 1, BlurXCfg<GB_R_MASKY1>::SW, GBX_TH, kslot, g_),
+          fused_->slots(mpre_ + P, 1, BlurXCfg<GB_R_MASKY0>::SW, GBX_TH, kslot, g_), pg, xa);
+    });
     note_launch_end("tma_blur_x", s_);
   }
   // S7 Malta line sums of both channels: ac[ch] = ((0 + uhf) + hf) + mf
   {
-    dim3 block(16, 16), grid(cdiv(g_.w, GB_MALTA_TILE_W), cdiv(rows, GB_MALTA_TILE_H), 2);
-    note_launch("malta_sums", s_, 2.0 * g_.w * rows);
-    k_tma_malta_sums<<<grid, block, 0, s_>>>(fused_->map(diffs6_, 6, GB_MALTA_SW, GB_MALTA_SH, g_), ac_, pg);
+    dim3 block(16, 16), grid(cdiv(g_.w, GB_MALTA_TILE_W), cdiv(rows, GB_MALTA_TILE_H), 2 * nimg);
+    note_launch("malta_sums", s_, 2.0 * g_.w * rows * nimg);
+    with_batch<void>(nimg, [&](auto b) {
+      k_tma_malta_sums<decltype(b)::value>
+          <<<grid, block, 0, s_>>>(fused_->slots(diffs6_, 6, GB_MALTA_SW, GB_MALTA_SH, kslot, g_), ac_, pg);
+    });
     note_launch_end("malta_sums", s_);
   }
   // S8 tail + S9 on block_diff_ac[Y]: blurred noise difference, asymmetric L2 of hf[Y]
-  launch_tma_y<GB_R_NOISE, 1>(s_, fused_->map(blr_, 1, GBY_TW, GBY_TH + 2 * GB_R_NOISE, g_), 1, t_.blur[kBlurNoise], pg, ht_,
-                              kBlurNoise, EpiNoise{ps0_ + kHfY * P, ps1_ + kHfY * P, ac_ + P, asym_w0_, asym_w1_, g_.pitch},
+  launch_tma_y<GB_R_NOISE, 1>(s_, fused_->slots(blr_, 1, GBY_TW, GBY_TH + 2 * GB_R_NOISE, kslot, g_), 1, nimg,
+                              t_.blur[kBlurNoise], pg, ht_, kBlurNoise,
+                              EpiNoise{ps0_ + kHfY * P, ps1_ + kHfY * P, ac_ + P, asym_w0_, asym_w1_, g_.pitch, S},
                               "noise_fused_y");
   // y passes + S11 CombineChannels + first half of S12 -> dm_[1]
   {
     typedef MaskYCfg<GB_R_MASKX, GB_R_MASKY0, GB_R_MASKY1> C;
-    allow_smem(k_tma_mask_y<GB_R_MASKX, GB_R_MASKY0, GB_R_MASKY1>, C::kSmemBytes);
     CombineArgs ca{ps0_, ps1_, ac_, dm_ + P, t_.mask_lut, g_.pitch, P};
-    dim3 grid(cdiv(g_.w, GBY_TW), cdiv(rows, GBY_TH), 1);
-    note_launch("mask_y_combine", s_, static_cast<double>(g_.w) * rows);
-    k_tma_mask_y<GB_R_MASKX, GB_R_MASKY0, GB_R_MASKY1><<<grid, 256, C::kSmemBytes, s_>>>(
-        fused_->map(tmp_, 1, GBY_TW, C::HA, g_), fused_->map(tmp_ + 2 * P, 1, GBY_TW, C::HB, g_),
-        fused_->map(tmp_ + P, 1, GBY_TW, C::HC, g_), t_.blur[kBlurMaskX].scale_y, t_.blur[kBlurMaskY0].scale_y,
-        t_.blur[kBlurMaskY1].scale_y, pg, make_blurk<GB_R_MASKX>(ht_, kBlurMaskX), make_blurk<GB_R_MASKY0>(ht_, kBlurMaskY0),
-        make_blurk<GB_R_MASKY1>(ht_, kBlurMaskY1), ca);
+    dim3 grid(cdiv(g_.w, GBY_TW), cdiv(rows, GBY_TH), nimg);
+    note_launch("mask_y_combine", s_, static_cast<double>(g_.w) * rows * nimg);
+    with_batch<void>(nimg, [&](auto b) {
+      constexpr bool B = decltype(b)::value;
+      allow_smem(k_tma_mask_y<B, GB_R_MASKX, GB_R_MASKY0, GB_R_MASKY1>, C::kSmemBytes);
+      k_tma_mask_y<B, GB_R_MASKX, GB_R_MASKY0, GB_R_MASKY1><<<grid, 256, C::kSmemBytes, s_>>>(
+          fused_->slots(tmp_, 1, GBY_TW, C::HA, kslot, g_), fused_->slots(tmp_ + 2 * P, 1, GBY_TW, C::HB, kslot, g_),
+          fused_->slots(tmp_ + P, 1, GBY_TW, C::HC, kslot, g_), t_.blur[kBlurMaskX].scale_y, t_.blur[kBlurMaskY0].scale_y,
+          t_.blur[kBlurMaskY1].scale_y, pg, make_blurk<GB_R_MASKX>(ht_, kBlurMaskX),
+          make_blurk<GB_R_MASKY0>(ht_, kBlurMaskY0), make_blurk<GB_R_MASKY1>(ht_, kBlurMaskY1), ca);
+    });
     note_launch_end("mask_y_combine", s_);
   }
-  // S12 second half + S13: blur 1.73, mix, per-block maxima, global maximum
+  // S12 second half + S13: blur 1.73, mix, per-block maxima, global maximum (one per image)
   const bool strips = comm_ && comm_->world() > 1;
-  dev_zero(d_gmax_, sizeof(unsigned int), s_);
+  dev_zero(d_gmax_, sizeof(unsigned int) * nimg, s_);
   {
     typedef Blur2dCfg<GB_R_FINAL, 1> C;
-    EpiFinal ef{dm_, block_max_, strips ? nullptr : d_gmax_, g_.pitch, g_.bw, by_lo_, by_hi_};
-    launch_tma_2d<GB_R_FINAL, 1>(s_, fused_->map(dm_ + P, 1, C::SWI, C::HI, g_), t_.blur[kBlurFinal], pg, ht_, kBlurFinal, ef,
-                                 "final_fused");
+    EpiFinal ef{dm_, block_max_, strips ? nullptr : d_gmax_, g_.pitch, g_.bw, by_lo_, by_hi_, S, g_.nblocks};
+    launch_tma_2d<GB_R_FINAL, 1>(s_, fused_->slots(dm_ + P, 1, C::SWI, C::HI, kslot, g_), nimg, t_.blur[kBlurFinal], pg, ht_,
+                                 kBlurFinal, ef, "final_fused");
   }
 }
 #endif  // !GB200_HOSTSIM
@@ -473,7 +529,7 @@ ImageContext::ImageContext(const float* linear_rgb, int w, int h, int device)
     upload_planes(linear_rgb, lin_, 3);
     opsin(lin_, xyb_);
     separate(xyb_, ps0_);
-    fused_sup0();
+    fused_sup0(1, 0);
     stream_sync(s_);
   } catch (...) {
     release();
@@ -512,6 +568,111 @@ float ImageContext::compare_linear_device(const float* linear_rgb, float* diffma
   }
   return m;
 }
+
+ImageContext::ImageContext(int w, int h, int capacity, int device)
+    : g_(make_geom(w, h)), device_(device), comm_(nullptr) {
+  if (capacity < 1) throw std::runtime_error("butteraugli batch: the capacity must be at least 1");
+  metric_only_ = true;
+  metric_ = true;
+  prepared_ = true;
+  capacity_ = capacity;
+  try {
+    batch_init();
+  } catch (...) {
+    release();
+    throw;
+  }
+}
+
+void ImageContext::batch_init() {
+  by_lo_ = 0;
+  by_hi_ = g_.bh;
+  cr_lo_ = 0;
+  cr_hi_ = g_.h;
+  select_device(device_);
+  s_ = make_stream();
+  have_stream_ = true;
+#if !defined(GB200_HOSTSIM)
+  use_fused_ = fused_enabled();
+  if (!use_fused_) return;  // GB200_COMPARE=staged: compare_batch scores pair by pair
+  t_ = build_tables(g_.w, g_.h, s_, &owned_, &ht_);
+  malta_call_params(malta_);
+  l2_asym_weights(&asym_w0_, &asym_w1_);
+  fused_ = new Fused();
+  fused_->capacity = capacity_;
+  // One arena slot per pair with the planes that the original's analysis and the fused chain touch;
+  // the groups are at the same offsets in every slot, so that image n's group is group + n * slot.
+  kslot_ = kBatchSlotPlanes;
+  const size_t slot = static_cast<size_t>(kslot_) * g_.plane;
+  float* a = static_cast<float*>(dev_alloc(sizeof(float) * slot * capacity_));
+  owned_.push_back(a);
+  dev_zero(a, sizeof(float) * slot * capacity_, s_);
+  float** groups[] = {&lin_, &xyb_, &lf_, &mf_in_, &hf_raw_, &ps0_, &ps1_, &sup0_, &diffs6_,
+                      &noise_, &mpre_, &tmp_, &blr_, &ac_, &dm_};
+  const int nplanes[] = {3, 3, 3, 3, 2, kPsychoPlanes, kPsychoPlanes, 2, 6, 1, 2, 3, 1, 2, 2};
+  int at = 0;
+  for (size_t i = 0; i < sizeof(nplanes) / sizeof(nplanes[0]); ++i) {
+    *groups[i] = a + static_cast<size_t>(at) * g_.plane;
+    at += nplanes[i];
+  }
+  if (at != kslot_) throw std::logic_error("butteraugli batch: slot layout");
+  block_max_ = static_cast<float*>(dev_alloc(sizeof(float) * g_.nblocks * capacity_));
+  owned_.push_back(block_max_);
+  d_gmax_ = static_cast<unsigned int*>(dev_alloc(sizeof(unsigned int) * capacity_));
+  owned_.push_back(d_gmax_);
+  stream_sync(s_);
+#endif
+}
+
+void ImageContext::compare_batch(const float* rgb0, const float* rgb1, int n, float* diffmap, float* maxima, bool device,
+                                 Stream caller) {
+  if (n < 1 || n > capacity_) throw std::runtime_error("butteraugli batch: n must be in 1..capacity");
+  bind();
+#if !defined(GB200_HOSTSIM)
+  if (use_fused_) {
+    if (device) stream_wait(s_, caller);
+    fused_compare_batch(rgb0, rgb1, n, diffmap, maxima);
+    return;
+  }
+#endif
+  // the staged chain and the CPU port: one metric-only context per pair
+  const size_t img = static_cast<size_t>(3) * g_.w * g_.h, px = static_cast<size_t>(g_.w) * g_.h;
+  std::vector<float> host0;
+  for (int i = 0; i < n; ++i) {
+    const float* p0 = rgb0 + i * img;
+    if (device) {  // the pair's original goes through host memory, after the caller's work
+      host0.resize(img);
+      d2h(host0.data(), p0, img * sizeof(float), caller);
+      p0 = host0.data();
+    }
+    ImageContext ctx(p0, g_.w, g_.h, device_);
+    float* dm = diffmap != nullptr ? diffmap + i * px : nullptr;
+    if (device) {
+      maxima[i] = ctx.compare_linear_device(rgb1 + i * img, dm, caller);
+    } else {
+      maxima[i] = ctx.compare_linear(rgb1 + i * img);
+      if (dm != nullptr) ctx.download_distmap(dm);
+    }
+  }
+}
+
+#if !defined(GB200_HOSTSIM)
+void ImageContext::fused_compare_batch(const float* rgb0, const float* rgb1, int n, float* diffmap, float* maxima) {
+  const size_t row = sizeof(float) * g_.w, pitch = sizeof(float) * g_.pitch;
+  const size_t slot_rows = static_cast<size_t>(kslot_) * g_.h;  // a plane is h rows of pitch
+  // [n][3][h][w] -> the lin planes of slots 0 .. n - 1: n slices of 3h rows
+  copy_3d(lin_, pitch, slot_rows, rgb0, row, static_cast<size_t>(3) * g_.h, row, static_cast<size_t>(3) * g_.h, n, s_);
+  // PsychoImage of every original (butteraugli.cc:784) and its DiffPrecompute neighbour sums
+  fused_opsin(lin_, xyb_, n, kslot_);
+  fused_separate(xyb_, ps0_, false, n, kslot_);
+  fused_sup0(n, kslot_);
+  copy_3d(lin_, pitch, slot_rows, rgb1, row, static_cast<size_t>(3) * g_.h, row, static_cast<size_t>(3) * g_.h, n, s_);
+  fused_compare_launches(n, kslot_);
+  if (diffmap != nullptr) copy_3d(diffmap, row, g_.h, dm_, pitch, slot_rows, row, g_.h, n, s_);
+  // one transfer of the n maxima (float bits); d2h waits for it, and so for everything queued before
+  d2h(maxima, d_gmax_, sizeof(float) * n, s_);
+}
+#endif
 
 void ImageContext::download_rgb(uint8_t* rgb) {
   bind();
@@ -671,7 +832,7 @@ void ImageContext::prepare() {
   px(LinearizeRgb{d_rgb_, lin_, g_, t_.srgb_lin}, "linearize_rgb");
   opsin(lin_, xyb_);
   separate(xyb_, ps0_);
-  fused_sup0();
+  fused_sup0(1, 0);
 
   // a13: mask_xyz_ = Mask(xyb0, xyb0), only its block-corner samples are ever read.
   mask_activity(xyb_);
@@ -775,7 +936,7 @@ void ImageContext::blur(const float* in, float* out, int nplanes, int id) {
 void ImageContext::opsin(const float* lin, float* xyb) {
 #if !defined(GB200_HOSTSIM)
   if (use_fused_) {
-    fused_opsin(lin, xyb);
+    fused_opsin(lin, xyb, 1, 0);
     return;
   }
 #endif
@@ -786,7 +947,7 @@ void ImageContext::opsin(const float* lin, float* xyb) {
 void ImageContext::separate(const float* xyb, float* ps) {
 #if !defined(GB200_HOSTSIM)
   if (use_fused_) {
-    fused_separate(xyb, ps, false);
+    fused_separate(xyb, ps, false, 1, 0);
     return;
   }
 #endif

@@ -52,6 +52,18 @@ class ImageContext {
   // into lin_ (the tensor maps and the captured graph are bound to lin_).  diffmap: device memory,
   // packed [h][w], or null; it is written when the call returns.
   float compare_linear_device(const float* linear_rgb, float* diffmap, Stream caller);
+  // Metric only, batched: up to `capacity` pairs of w x h images are scored per call.  Each pair has
+  // an arena slot of kBatchSlotPlanes planes (DESIGN.md §4), and the one-time analysis of the
+  // originals and the Compare chain run as one launch per stage over all pairs.
+  ImageContext(int w, int h, int capacity, int device);
+  static constexpr int kBatchSlotPlanes = 53;
+  int capacity() const { return capacity_; }
+  // ButteraugliInterface for each of n <= capacity pairs, rgb0 / rgb1 packed [n][3][h][w]:
+  // diffmap [n][h][w] (or null) and maxima[n].  device: rgb0, rgb1 and diffmap are memory of this
+  // context's device; this context's stream first waits for the work queued so far on `caller`.
+  // Either way every output is written when the call returns.
+  void compare_batch(const float* rgb0, const float* rgb1, int n, float* diffmap, float* maxima, bool device,
+                     Stream caller);
   // ButteraugliComparator::Mask (b/butteraugli.cc:793) of the first image at every pixel, on the
   // host: mask, mask_dc [3][h][w].  Leaves the resident PsychoImage as it is.
   void mask(float* mask, float* mask_dc);
@@ -255,14 +267,20 @@ class ImageContext {
   float* sup0_ = nullptr;    // [2] DiffPrecompute neighbour sums of the original (X, Y)
   unsigned int* d_gmax_ = nullptr;  // global maximum of the distmap (float bits)
   bool use_fused_ = false;
-  void fused_opsin(const float* lin, float* xyb);
-  void fused_separate(const float* xyb, float* ps, bool with_diffs);
+  // nimg images in arena slots kslot planes apart (a single-image context passes 1, 0)
+  void fused_opsin(const float* lin, float* xyb, int nimg, int kslot);
+  void fused_separate(const float* xyb, float* ps, bool with_diffs, int nimg, int kslot);
   void fused_blur(const float* in, float* out, int nplanes, int id);
   float fused_compare_tail();
   void fused_compare_submit();
   float fused_compare_result();
-  void fused_compare_launches();
-  void fused_sup0();
+  void fused_compare_launches(int nimg, int kslot);
+  void fused_sup0(int nimg, int kslot);
+  // batched metric-only context: slots of the arena, kslot_ planes each (0: one image)
+  int capacity_ = 1;
+  int kslot_ = 0;
+  void batch_init();
+  void fused_compare_batch(const float* rgb0, const float* rgb1, int n, float* diffmap, float* maxima);
   void guarded_init(const uint8_t* rgb, const int16_t* dq_coeffs, int w, int h, bool prepare_now);
   void release();
   bool released_ = false;

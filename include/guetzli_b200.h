@@ -108,6 +108,28 @@ int gb200_butteraugli_comparator_diffmap_device(gb200_butteraugli_comparator* c,
 /* ButteraugliComparator::Mask (butteraugli.cc:793): mask and mask_dc, [3][h][w] each, host memory. */
 int gb200_butteraugli_comparator_mask(gb200_butteraugli_comparator* c, float* mask, float* mask_dc);
 void gb200_butteraugli_comparator_destroy(gb200_butteraugli_comparator* c);
+/* ---- batched butteraugli: N same-size pairs per call ----
+ * Each pair (rgb0[i], rgb1[i]) gets butteraugli::ButteraugliInterface (butteraugli.cc:1858), bit for bit
+ * what gb200_butteraugli_diffmap gives for it alone.  Up to `capacity` pairs of w x h images run through
+ * the Compare chain together, one launch per stage, each pair in its own slot of device memory
+ * (DESIGN.md §4).  Images are planar linear RGB floats in 0..255, at least 8x8.  One batch object is
+ * used by one thread at a time; separate objects may run concurrently, each has its own stream.  Every
+ * call returns once its outputs are written. */
+typedef struct gb200_butteraugli_batch gb200_butteraugli_batch;
+/* w, h at least 8 and below 65536; 1 <= capacity <= 16383; NULL on failure (gb200_last_error), with
+ * nothing left allocated */
+gb200_butteraugli_batch* gb200_butteraugli_batch_create(int w, int h, int capacity, int device);
+/* ButteraugliInterface per pair: rgb0, rgb1 [n][3][h][w] in host memory, 1 <= n <= capacity;
+ * diffmap (may be NULL) receives [n][h][w], score (may be NULL) [n], the maximum of each diffmap. */
+int gb200_butteraugli_batch_diffmap(gb200_butteraugli_batch* b, const float* rgb0, const float* rgb1, int n,
+                                    float* diffmap, double* score);
+/* The same with rgb0, rgb1 and diffmap (may be NULL) in device memory of the batch's device; stream as in
+ * gb200_butteraugli_comparator_diffmap_device.  A host pointer or memory of another device is refused,
+ * nothing runs. */
+int gb200_butteraugli_batch_diffmap_device(gb200_butteraugli_batch* b, const float* rgb0_dev, const float* rgb1_dev,
+                                           int n, float* diffmap_dev, double* score, void* stream);
+void gb200_butteraugli_batch_destroy(gb200_butteraugli_batch* b);
+
 /* butteraugli::ButteraugliAdaptiveQuantization (butteraugli.cc:1880): the Y plane of Mask(rgb, rgb),
  * [h][w] into quant.  rgb in host memory.  Fails below 16x16, where the reference returns false. */
 int gb200_butteraugli_adaptive_quantization(const float* rgb, int w, int h, int device, float* quant);

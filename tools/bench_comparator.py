@@ -6,8 +6,14 @@
   comparator_host one resident gb200_butteraugli_comparator, candidates and diffmaps in host memory
   comparator_cuda the same comparator, candidates and diffmaps as CUDA torch tensors
 
-Every call returns once its diffmap is written, so a host clock around `--n` calls is the time of
-the work.  The modes run in turn for `--rounds` rounds (the spread between rounds is part of the
+With --batch N, two more modes score N distinct pairs (a different original in each) per call:
+
+  batch_cuda      one gb200_butteraugli_batch of capacity N, pairs and diffmaps as CUDA torch tensors
+  batch_host      the same batch, pairs and diffmaps in host memory
+
+and the result gains ms per pair of the batch modes and MPix/s (scored pixels per second) of every
+mode.  Every call returns once its diffmaps are written, so a host clock around `--n` calls is the
+time of the work.  The modes run in turn for `--rounds` rounds (the spread between rounds is part of the
 result), after `--warmup` untimed calls each.  The card's name and power limit are read in the
 same run (nvidia-smi, read-only queries).  Prints one JSON line; --out also writes it to a file.
 There is no CPU mode: without a GPU the script fails."""
@@ -52,6 +58,7 @@ def main():
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--device", type=int, default=0)
+    ap.add_argument("--batch", type=int, default=0, help="pairs per call of the batch modes (0: no batch modes)")
     ap.add_argument("--out", default=None, help="also write the JSON result here")
     args = ap.parse_args()
 
@@ -80,12 +87,33 @@ def main():
         return cmp.diffmap(cands_dev[i])[1]
 
     modes = {"pairwise": pairwise, "comparator_host": comparator_host, "comparator_cuda": comparator_cuda}
+    per_call = {m: 1 for m in modes}
+    if args.batch > 0:
+        nb = args.batch
+        bpairs = [(linear(synth.gradnoise(h, w, 1000 + i)),
+                   linear(np.clip(synth.gradnoise(h, w, 1000 + i).astype(int) + synth.noise(h, w, 3000 + i) % 7 - 3,
+                                  0, 255).astype(np.uint8))) for i in range(nb)]
+        b0 = np.stack([p[0] for p in bpairs])
+        b1 = np.stack([p[1] for p in bpairs])
+        b0_dev, b1_dev = torch.from_numpy(b0).to(dev), torch.from_numpy(b1).to(dev)
+        torch.cuda.synchronize(dev)
+        batch = gb.ButteraugliBatch(h, w, nb, device=args.device)
+
+        def batch_cuda(i):
+            return batch.diffmap(b0_dev, b1_dev)[1].tolist()
+
+        def batch_host(i):
+            return batch.diffmap(b0, b1)[1].tolist()
+
+        modes.update(batch_cuda=batch_cuda, batch_host=batch_host)
+        per_call.update(batch_cuda=nb, batch_host=nb)
     scores = {}
     for name, f in modes.items():
         for i in range(args.warmup):
             f(i % args.n)
         scores[name] = [f(i) for i in range(args.n)]
-    identical = all(scores[m] == scores["pairwise"] for m in modes)
+    single = ["pairwise", "comparator_host", "comparator_cuda"]
+    identical = all(scores[m] == scores["pairwise"] for m in single)
 
     ms = {m: [] for m in modes}
     for _ in range(args.rounds):
@@ -95,13 +123,25 @@ def main():
             for i in range(args.n):
                 f(i)
             torch.cuda.synchronize(dev)
-            ms[name].append((time.perf_counter() - t0) / args.n * 1e3)
+            ms[name].append((time.perf_counter() - t0) / args.n * 1e3 / per_call[name])
     cmp.close()
 
+    def stats(v):
+        return {"median": round(statistics.median(v), 3), "min": round(min(v), 3), "max": round(max(v), 3)}
+
     result = {"size": f"{w}x{h}", "calls_per_round": args.n, "rounds": args.rounds,
-              "ms_per_image": {m: {"median": round(statistics.median(v), 3), "min": round(min(v), 3),
-                                   "max": round(max(v), 3)} for m, v in ms.items()},
+              "ms_per_image": {m: stats(ms[m]) for m in single},
               "scores_identical_across_modes": identical}
+    if args.batch > 0:
+        batch.close()
+        # every batch call scores the same pairs: host and device entry agree, and pair 0 scores as it
+        # does alone
+        alone = gb.api.butteraugli_diffmap(b0[0], b1[0], device=args.device)[1]
+        result["batch"] = args.batch
+        result["ms_per_pair"] = {m: stats(ms[m]) for m in ("batch_cuda", "batch_host")}
+        result["mpix_per_s"] = {m: round(w * h / 1e3 / statistics.median(v), 2) for m, v in ms.items()}
+        result["batch_scores_consistent"] = (all(s == scores["batch_cuda"][0] for m in ("batch_cuda", "batch_host")
+                                                 for s in scores[m]) and scores["batch_cuda"][0][0] == alone)
     result.update(gpu_info(args.device))
     line = json.dumps(result)
     print(line)
