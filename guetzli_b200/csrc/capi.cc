@@ -5,6 +5,7 @@
 #include <string.h>
 
 #include <exception>
+#include <memory>
 #include <stdexcept>
 #include <thread>
 #include <string>
@@ -29,16 +30,7 @@ Comm* thread_comm_create(ThreadGroup* g, int rank);
 #if !defined(GB200_HOSTSIM)
 void nccl_unique_id(uint8_t out[128]);
 Comm* nccl_comm_create(const uint8_t id[128], int rank, int world);
-void select_device(int device);
 void dev_trim();
-#endif
-long total_launches();
-long long h2d_bytes_total();
-long long d2h_bytes_total();
-void profiling_enable(bool on);
-std::vector<KernelStat> profiling_snapshot();
-void profiling_reset();
-#if !defined(GB200_HOSTSIM)
 int cuda_device_count();
 #endif
 }  // namespace gb200
@@ -65,13 +57,11 @@ struct gb200_image {
 };
 
 struct gb200_butteraugli_comparator {
-  gb200::ImageContext* ctx;  // metric-only context
-  int device;
+  gb200::Butteraugli* ba;
 };
 
 struct gb200_butteraugli_batch {
-  gb200::ImageContext* ctx;  // batched metric-only context
-  int device;
+  gb200::Butteraugli* ba;
 };
 
 namespace {
@@ -209,10 +199,11 @@ int gb200_butteraugli_diffmap(const float* rgb0, const float* rgb1, int w, int h
       p0 = s0.data();
       p1 = s1.data();
     }
-    gb200::ImageContext ctx(p0, ws, hs, device);
-    const float dmax = ctx.compare_linear(p1);
+    gb200::Butteraugli ba(ws, hs, device, nullptr);
+    ba.analyse_original(p0);
+    const float dmax = ba.compare_linear(p1);
     std::vector<float> dm(static_cast<size_t>(ws) * hs);
-    if (diffmap != nullptr || ws != w || hs != h) ctx.download_distmap(dm.data());
+    if (diffmap != nullptr || ws != w || hs != h) ba.download_distmap(dm.data());
     float m = 0.0f;
     if (ws != w || hs != h) {
       for (int y = 0; y < h; ++y)
@@ -238,17 +229,17 @@ gb200_butteraugli_comparator* gb200_butteraugli_comparator_create(const float* r
     // the reference class computes nothing below 8 pixels in a dimension (b/butteraugli.cc:788)
     if (w < 8 || h < 8 || w >= 65536 || h >= 65536)
       throw std::runtime_error("butteraugli comparator: the image must be at least 8x8 (and below 65536)");
-    gb200::ImageContext* ctx = new gb200::ImageContext(rgb0, w, h, device);
+    std::unique_ptr<gb200::Butteraugli> ba(new gb200::Butteraugli(w, h, device, nullptr));
+    ba->analyse_original(rgb0);
     c = new gb200_butteraugli_comparator;
-    c->ctx = ctx;
-    c->device = device;
+    c->ba = ba.release();
   });
   return c;
 }
 
 void gb200_butteraugli_comparator_destroy(gb200_butteraugli_comparator* c) {
   if (!c) return;
-  guarded([&]() { delete c->ctx; });
+  guarded([&]() { delete c->ba; });
   delete c;
 }
 
@@ -260,8 +251,8 @@ int gb200_butteraugli_comparator_diffmap(gb200_butteraugli_comparator* c, const 
     return 0;
   }
   return guarded([&]() {
-    const float m = c->ctx->compare_linear(rgb1);
-    if (diffmap) c->ctx->download_distmap(diffmap);
+    const float m = c->ba->compare_linear(rgb1);
+    if (diffmap) c->ba->download_distmap(diffmap);
     if (score) *score = m;
   });
 }
@@ -274,17 +265,17 @@ int gb200_butteraugli_comparator_diffmap_device(gb200_butteraugli_comparator* c,
     return 0;
   }
   return guarded([&]() {
-    c->ctx->bind();
+    c->ba->bind();
     const void* ptrs[2] = {rgb1_dev, diffmap_dev};
     const char* what[2] = {"rgb1", "diffmap"};
-    check_device_pointers("butteraugli comparator", c->device, ptrs, what, 2);
+    check_device_pointers("butteraugli comparator", c->ba->device(), ptrs, what, 2);
 #if defined(GB200_HOSTSIM)
     const gb200::Stream caller = 0;  // not reached: the port has no device memory
     (void)stream;
 #else
     const gb200::Stream caller = static_cast<gb200::Stream>(stream);
 #endif
-    const float m = c->ctx->compare_linear_device(rgb1_dev, diffmap_dev, caller);
+    const float m = c->ba->compare_linear_device(rgb1_dev, diffmap_dev, caller);
     if (score) *score = m;
   });
 }
@@ -298,17 +289,16 @@ gb200_butteraugli_batch* gb200_butteraugli_batch_create(int w, int h, int capaci
     // the batched Compare chain folds the image into blockIdx.z, four z per image in its widest launch
     if (capacity < 1 || capacity > 16383)
       throw std::runtime_error("butteraugli batch: the capacity must be in 1..16383");
-    gb200::ImageContext* ctx = new gb200::ImageContext(w, h, capacity, device);
+    gb200::Butteraugli* ba = new gb200::Butteraugli(w, h, capacity, device);
     b = new gb200_butteraugli_batch;
-    b->ctx = ctx;
-    b->device = device;
+    b->ba = ba;
   });
   return b;
 }
 
 void gb200_butteraugli_batch_destroy(gb200_butteraugli_batch* b) {
   if (!b) return;
-  guarded([&]() { delete b->ctx; });
+  guarded([&]() { delete b->ba; });
   delete b;
 }
 
@@ -319,25 +309,25 @@ int batch_diffmap(gb200_butteraugli_batch* b, const float* rgb0, const float* rg
     g_err = "butteraugli batch: no batch or no images";
     return 0;
   }
-  if (n < 1 || n > b->ctx->capacity()) {
+  if (n < 1 || n > b->ba->capacity()) {
     g_err = "butteraugli batch: n = " + std::to_string(n) + " pairs, the batch takes 1.." +
-            std::to_string(b->ctx->capacity());
+            std::to_string(b->ba->capacity());
     return 0;
   }
   return guarded([&]() {
-    b->ctx->bind();
+    b->ba->bind();
     gb200::Stream caller = 0;
     if (device) {
       const void* ptrs[3] = {rgb0, rgb1, diffmap};
       const char* what[3] = {"rgb0", "rgb1", "diffmap"};
-      check_device_pointers("butteraugli batch", b->device, ptrs, what, 3);
+      check_device_pointers("butteraugli batch", b->ba->device(), ptrs, what, 3);
 #if !defined(GB200_HOSTSIM)
       caller = static_cast<gb200::Stream>(stream);
 #endif
     }
     (void)stream;
     std::vector<float> m(n);
-    b->ctx->compare_batch(rgb0, rgb1, n, diffmap, m.data(), device, caller);
+    b->ba->compare_batch(rgb0, rgb1, n, diffmap, m.data(), device, caller);
     if (score)
       for (int i = 0; i < n; ++i) score[i] = m[i];
   });
@@ -360,7 +350,7 @@ int gb200_butteraugli_comparator_mask(gb200_butteraugli_comparator* c, float* ma
     g_err = "butteraugli comparator: no comparator or no output";
     return 0;
   }
-  return guarded([&]() { c->ctx->mask(mask, mask_dc); });
+  return guarded([&]() { c->ba->mask(mask, mask_dc); });
 }
 
 // butteraugli::ButteraugliAdaptiveQuantization (b/butteraugli.cc:1880)
@@ -374,8 +364,9 @@ int gb200_butteraugli_adaptive_quantization(const float* rgb, int w, int h, int 
     return 0;
   }
   return guarded([&]() {
-    gb200::ImageContext ctx(rgb, w, h, device);
-    ctx.adaptive_quantization(rgb, quant);
+    gb200::Butteraugli ba(w, h, device, nullptr);
+    ba.analyse_original(rgb);
+    ba.adaptive_quantization(rgb, quant);
   });
 }
 
