@@ -97,6 +97,12 @@ def load_library(path=None):
                                                                 C.c_void_p]
     lib.gb200_butteraugli_comparator_mask.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
     lib.gb200_butteraugli_comparator_destroy.argtypes = [C.c_void_p]
+    lib.gb200_butteraugli_comparator_create_batch.restype = C.c_void_p
+    lib.gb200_butteraugli_comparator_create_batch.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int]
+    lib.gb200_butteraugli_comparator_diffmap_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                                                               C.c_void_p]
+    lib.gb200_butteraugli_comparator_diffmap_batch_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                                                                      C.c_void_p, C.c_void_p]
     lib.gb200_butteraugli_adaptive_quantization.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]
     lib.gb200_butteraugli_batch_create.restype = C.c_void_p
     lib.gb200_butteraugli_batch_create.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int]
@@ -260,17 +266,22 @@ def _is_torch_tensor(x):
 class Comparator:
     """butteraugli::ButteraugliComparator (butteraugli.h:425) on one GPU: the original rgb0, planar
     linear RGB float32 [3][h][w] in 0..255 and at least 8x8, stays resident and is scored against
-    any number of images.  Used by one thread at a time."""
+    any number of images, up to `capacity` (1..16383) of them per diffmap() call in one pass of the
+    Compare chain.  Used by one thread at a time."""
 
-    def __init__(self, rgb0, device=0, lib=None):
+    def __init__(self, rgb0, device=0, capacity=1, lib=None):
         self.lib = lib or load_library()
         self._h = None
         a = np.ascontiguousarray(rgb0, dtype=np.float32)
         if a.ndim != 3 or a.shape[0] != 3:
             raise ValueError(f"rgb0 must be planar [3][h][w], got shape {a.shape}")
         _, self.h, self.w = a.shape
-        self.device = device
-        self._h = self.lib.gb200_butteraugli_comparator_create(a.ctypes.data, self.w, self.h, device)
+        self.device, self.capacity = device, int(capacity)
+        if self.capacity == 1:
+            self._h = self.lib.gb200_butteraugli_comparator_create(a.ctypes.data, self.w, self.h, device)
+        else:
+            self._h = self.lib.gb200_butteraugli_comparator_create_batch(a.ctypes.data, self.w, self.h,
+                                                                         self.capacity, device)
         if not self._h:
             raise RuntimeError("gb200_butteraugli_comparator_create failed: " + _err(self.lib))
 
@@ -291,7 +302,12 @@ class Comparator:
 
         A CUDA torch tensor (float32, [3][h][w]) is scored from device memory after the work queued
         on its device's current torch stream, and the diffmap comes back as a tensor on that device.
-        Anything else is read as a numpy array in host memory."""
+        Anything else is read as a numpy array in host memory.
+
+        rgb1 float32 [n][3][h][w] with 1 <= n <= capacity scores each image the same way, all in one
+        call -> (diffmaps [n][h][w], scores float64 ndarray [n])."""
+        if len(getattr(rgb1, "shape", ())) == 4:
+            return self._diffmap_batch(rgb1)
         if _is_torch_tensor(rgb1) and rgb1.is_cuda:
             return self._diffmap_device(rgb1)
         a = np.ascontiguousarray(rgb1, dtype=np.float32)
@@ -314,6 +330,32 @@ class Comparator:
         self._ck(self.lib.gb200_butteraugli_comparator_diffmap_device(self._h, t.data_ptr(), dm.data_ptr(),
                                                                       C.byref(score), stream))
         return dm, score.value
+
+    def _diffmap_batch(self, rgb1):
+        shape = tuple(rgb1.shape)
+        if shape[1:] != (3, self.h, self.w) or not 1 <= shape[0] <= self.capacity:
+            raise ValueError(f"rgb1 must have shape [n, 3, {self.h}, {self.w}] with 1 <= n <= {self.capacity}, "
+                             f"got {shape}")
+        n = shape[0]
+        score = np.empty(n, dtype=np.float64)
+        if _is_torch_tensor(rgb1) and rgb1.is_cuda:
+            import torch
+            if rgb1.dtype != torch.float32:
+                raise ValueError(f"rgb1 must be float32, got {rgb1.dtype}")
+            t = rgb1.contiguous()
+            dm = torch.empty((n, self.h, self.w), dtype=torch.float32, device=t.device)
+            stream = torch.cuda.current_stream(t.device).cuda_stream
+            self._ck(self.lib.gb200_butteraugli_comparator_diffmap_batch_device(self._h, t.data_ptr(), n, dm.data_ptr(),
+                                                                                score.ctypes.data, stream))
+            return dm, score
+        a = np.asarray(rgb1)
+        if a.dtype != np.float32:
+            raise ValueError(f"rgb1 must be float32, got {a.dtype}")
+        a = np.ascontiguousarray(a)
+        dm = np.empty((n, self.h, self.w), dtype=np.float32)
+        self._ck(self.lib.gb200_butteraugli_comparator_diffmap_batch(self._h, a.ctypes.data, n, dm.ctypes.data,
+                                                                     score.ctypes.data))
+        return dm, score
 
     def mask(self):
         """ButteraugliComparator::Mask -> (mask, mask_dc), float32 [3][h][w] each."""

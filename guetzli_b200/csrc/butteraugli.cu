@@ -49,10 +49,15 @@ void Region::upload_planes(const float* packed, float* dst, int n) const {
 
 Butteraugli::Butteraugli(int w, int h, int device, Comm* comm) : device_(device) { init(w, h, comm); }
 
-Butteraugli::Butteraugli(int w, int h, int capacity, int device) : device_(device) {
+Butteraugli::Butteraugli(int w, int h, int capacity, int device, Slots slots) : device_(device) {
   if (capacity < 1) throw std::runtime_error("butteraugli batch: the capacity must be at least 1");
   capacity_ = capacity;
-  kslot_ = kBatchSlotPlanes;
+  if (slots == Slots::kPairs) {
+    kslot_ = kBatchSlotPlanes;
+  } else if (capacity > 1) {  // capacity 1: the single-image layout
+    one_original_ = true;
+    kslot_ = kCandidateSlotPlanes;
+  }
   init(w, h, nullptr);
 }
 
@@ -85,7 +90,10 @@ void Butteraugli::init(int w, int h, Comm* comm) {
 #if !defined(GB200_HOSTSIM)
     use_fused_ = fused_enabled();
 #endif
-    if (kslot_ != 0 && !use_fused_) return;  // compare_batch scores the pairs one by one
+    // the staged chain and the CPU port have no batched launches: compare_many scores the candidates
+    // one by one on a single-image layout, compare_batch the pairs through metrics of their own
+    if (one_original_ && !use_fused_) kslot_ = 0;
+    if (kslot_ != 0 && !use_fused_) return;
     t_ = build_tables(w, h, s_, &owned_, &ht_);
     malta_call_params(malta_);
     l2_asym_weights(&asym_w0_, &asym_w1_);
@@ -110,34 +118,46 @@ float* Butteraugli::planes(size_t n) {
   return static_cast<float*>(p);
 }
 
-// The plane groups of both shapes.  They lie in one arena of capacity_ slots, each group at the
+// The plane groups of all three shapes.  They lie in one arena of `slots` slots, each group at the
 // same offset in every slot, so that slot n's copy of a group is the group plus n slots.  A batch
-// slot holds only what the analysis of an original and the fused chain touch (DESIGN.md §4).
+// slot holds only what the analysis of an original and the fused chain touch (DESIGN.md §4).  With
+// one original for all slots, the original's groups lie once after the slots, with the planes of
+// its mask activity (mask()), and a slot holds the rest.
 void Butteraugli::alloc_planes() {
   struct Group {
     float** p;
     int single, batch;  // planes in the slot of one image / of a batch
+    bool orig;          // the original's: outside the slots when they share one original
   };
   const Group groups[] = {
-      {&lin_, 3, 3},    {&xyb_, 3, 3},  {&lf_, 3, 3},  {&mf_in_, 3, 3}, {&hf_raw_, 2, 2},
-      {&ps0_, kPsychoPlanes, kPsychoPlanes},          {&ps1_, kPsychoPlanes, kPsychoPlanes},
-      {&sup0_, 2, 2},   {&diffs6_, 6, 6}, {&noise_, 2, 1}, {&mpre_, 2, 2}, {&tmp_, 3, 3},
-      {&blr_, 3, 1},    {&ac_, 2, 2},   {&dm_, 2, 2},
+      {&lin_, 3, 3, false},    {&xyb_, 3, 3, false},  {&lf_, 3, 3, false},  {&mf_in_, 3, 3, false},
+      {&hf_raw_, 2, 2, false}, {&ps0_, kPsychoPlanes, kPsychoPlanes, true}, {&ps1_, kPsychoPlanes, kPsychoPlanes, false},
+      {&sup0_, 2, 2, true},    {&diffs6_, 6, 6, false}, {&noise_, 2, 1, false}, {&mpre_, 2, 2, false},
+      {&tmp_, 3, 3, false},    {&blr_, 3, 1, false},  {&ac_, 2, 2, false},  {&dm_, 2, 2, false},
       // the staged chain's own planes and the mask activity
-      {&mf_blr_, 3, 0}, {&hf_blr_, 2, 0}, {&diffs_, 1, 0}, {&sact_, 3, 0}};
-  int slot = 0;
-  for (const Group& gr : groups) slot += kslot_ ? gr.batch : gr.single;
-  if (kslot_ != 0 && slot != kslot_) throw std::logic_error("butteraugli batch: slot layout");
-  float* a = planes(static_cast<size_t>(slot) * capacity_);
-  int at = 0;
+      {&mf_blr_, 3, 0, false}, {&hf_blr_, 2, 0, false}, {&diffs_, 1, 0, false}, {&sact_, 3, 0, true}};
+  const bool shared = one_original_ && kslot_ != 0;
+  const int slots = kslot_ ? capacity_ : 1;
+  int slot = 0, once = 0;
   for (const Group& gr : groups) {
-    const int n = kslot_ ? gr.batch : gr.single;
-    *gr.p = n ? a + static_cast<size_t>(at) * g_.plane : nullptr;
-    at += n;
+    if (shared && gr.orig) {
+      once += gr.single;
+    } else {
+      slot += kslot_ ? gr.batch : gr.single;
+    }
   }
-  block_max_ = static_cast<float*>(dev_alloc(sizeof(float) * g_.nblocks * capacity_));
+  if (kslot_ != 0 && slot != kslot_) throw std::logic_error("butteraugli batch: slot layout");
+  float* a = planes(static_cast<size_t>(slot) * slots + once);
+  int at = 0, at_once = slot * slots;
+  for (const Group& gr : groups) {
+    int& pos = shared && gr.orig ? at_once : at;
+    const int n = shared && gr.orig ? gr.single : kslot_ ? gr.batch : gr.single;
+    *gr.p = n ? a + static_cast<size_t>(pos) * g_.plane : nullptr;
+    pos += n;
+  }
+  block_max_ = static_cast<float*>(dev_alloc(sizeof(float) * g_.nblocks * slots));
   owned_.push_back(block_max_);
-  d_gmax_ = static_cast<unsigned int*>(dev_alloc(sizeof(unsigned int) * capacity_));
+  d_gmax_ = static_cast<unsigned int*>(dev_alloc(sizeof(unsigned int) * slots));
   owned_.push_back(d_gmax_);
   partial_ = static_cast<float*>(dev_alloc(sizeof(float) * 1024));
   owned_.push_back(partial_);
@@ -219,6 +239,29 @@ void Butteraugli::compare_batch(const float* rgb0, const float* rgb1, int n, flo
     } else {
       maxima[i] = pair.compare_linear(rgb1 + i * img);
       if (dm != nullptr) pair.download_distmap(dm);
+    }
+  }
+}
+
+void Butteraugli::compare_many(const float* rgb1, int n, float* diffmap, float* maxima, bool device, Stream caller) {
+  if (n < 1 || n > capacity_) throw std::runtime_error("butteraugli comparator: n must be in 1..capacity");
+  bind();
+#if !defined(GB200_HOSTSIM)
+  if (use_fused_ && kslot_ != 0) {
+    if (device) stream_wait(s_, caller);
+    fused_compare_batch(nullptr, rgb1, n, diffmap, maxima);
+    return;
+  }
+#endif
+  // capacity 1, the staged chain and the CPU port: one candidate at a time in slot 0
+  const size_t img = static_cast<size_t>(3) * g_.w * g_.h, px = static_cast<size_t>(g_.w) * g_.h;
+  for (int i = 0; i < n; ++i) {
+    float* dm = diffmap != nullptr ? diffmap + i * px : nullptr;
+    if (device) {
+      maxima[i] = compare_linear_device(rgb1 + i * img, dm, caller);
+    } else {
+      maxima[i] = compare_linear(rgb1 + i * img);
+      if (dm != nullptr) download_distmap(dm);
     }
   }
 }

@@ -1,7 +1,8 @@
 // The butteraugli metric on the device: the Compare chain (the TMA-staged fused chain, and the staged
 // chain it is checked against), the float planes it works on, and the analysis of the original.
 // One Butteraugli scores one image -- the encoder's candidate (ImageContext holds one) or a
-// stand-alone comparator's -- or a batch of same-size pairs.  It owns the stream and the tables,
+// stand-alone comparator's -- or a batch of same-size pairs, or a batch of same-size candidates
+// against one original.  It owns the stream and the tables,
 // which the encoder's kernels use as well.  See DESIGN.md §4 and §5.1.
 #pragma once
 #include <stddef.h>
@@ -114,11 +115,16 @@ class Butteraugli {
  public:
   // One image; comm: strip mode (Region).
   Butteraugli(int w, int h, int device, Comm* comm);
-  // Batched: up to `capacity` pairs of w x h images are scored per call.  Each pair has an arena
-  // slot of kBatchSlotPlanes planes (DESIGN.md §4), and the analysis of the originals and the
-  // Compare chain run as one launch per stage over all pairs.
-  Butteraugli(int w, int h, int capacity, int device);
+  // Batched, up to `capacity` images per call, one launch per stage over all of them (DESIGN.md §4).
+  //   kPairs: w x h pairs (compare_batch).  Each pair has an arena slot of kBatchSlotPlanes planes,
+  //     and the originals are analysed in the call.
+  //   kCandidates: w x h candidates against one original (compare_many), which analyse_original()
+  //     analyses once.  Its planes lie once outside the slots, and each candidate has a slot of
+  //     kCandidateSlotPlanes planes.  Capacity 1 is the single-image metric.
+  enum class Slots { kPairs, kCandidates };
+  Butteraugli(int w, int h, int capacity, int device, Slots slots = Slots::kPairs);
   static constexpr int kBatchSlotPlanes = 53;
+  static constexpr int kCandidateSlotPlanes = 41;  // a pair's slot without ps0 and sup0
   ~Butteraugli();
   Butteraugli(const Butteraugli&) = delete;
   Butteraugli& operator=(const Butteraugli&) = delete;
@@ -168,6 +174,10 @@ class Butteraugli {
   // Either way every output is written when the call returns.
   void compare_batch(const float* rgb0, const float* rgb1, int n, float* diffmap, float* maxima, bool device,
                      Stream caller);
+  // ButteraugliComparator::Diffmap against the original for each of n <= capacity candidates,
+  // rgb1 packed [n][3][h][w]; outputs, device and caller as in compare_batch.  Slots kCandidates;
+  // with capacity 1, the staged chain or the CPU port the candidates go one by one through slot 0.
+  void compare_many(const float* rgb1, int n, float* diffmap, float* maxima, bool device, Stream caller);
   // ButteraugliComparator::Mask (b/butteraugli.cc:793) of the original at every pixel, on the
   // host: mask, mask_dc [3][h][w].  Leaves the resident PsychoImage as it is.
   void mask(float* mask, float* mask_dc);
@@ -199,14 +209,16 @@ class Butteraugli {
   struct Fused;
   Fused* fused_ = nullptr;
   bool use_fused_ = false;
-  // nimg images in arena slots kslot planes apart (a single image passes 1, 0)
+  // nimg images in arena slots kslot planes apart, the original's planes kslot0 apart (kslot0 =
+  // kslot: an original per image, 0: one for all; a single image passes 1, 0, 0)
   void fused_opsin(const float* lin, float* xyb, int nimg, int kslot);
-  void fused_separate(const float* xyb, float* ps, bool with_diffs, int nimg, int kslot);
+  void fused_separate(const float* xyb, float* ps, bool with_diffs, int nimg, int kslot, int kslot0);
   void fused_blur(const float* in, float* out, int nplanes, int id);
   void fused_compare_submit();
   float fused_compare_result();
-  void fused_compare_launches(int nimg, int kslot);
+  void fused_compare_launches(int nimg, int kslot, int kslot0);
   void fused_sup0(int nimg, int kslot);
+  // n pairs, or with rgb0 null n candidates against the resident original
   void fused_compare_batch(const float* rgb0, const float* rgb1, int n, float* diffmap, float* maxima);
   bool compare_pending_ = false;
   float compare_stash_ = 0.0f;
@@ -219,6 +231,7 @@ class Butteraugli {
   // arena slots, kslot_ planes each (a single image: one slot, kslot_ = 0)
   int capacity_ = 1;
   int kslot_ = 0;
+  bool one_original_ = false;  // Slots::kCandidates with capacity > 1
   Tables t_;
   HostTables ht_;
   MaltaParams malta_[6];

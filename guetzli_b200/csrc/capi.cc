@@ -280,6 +280,68 @@ int gb200_butteraugli_comparator_diffmap_device(gb200_butteraugli_comparator* c,
   });
 }
 
+// The comparator with `capacity` candidate slots: ButteraugliComparator::ButteraugliComparator(rgb0) once
+gb200_butteraugli_comparator* gb200_butteraugli_comparator_create_batch(const float* rgb0, int w, int h, int capacity,
+                                                                        int device) {
+  gb200_butteraugli_comparator* c = nullptr;
+  guarded([&]() {
+    if (rgb0 == nullptr) throw std::runtime_error("butteraugli comparator: no image");
+    if (w < 8 || h < 8 || w >= 65536 || h >= 65536)
+      throw std::runtime_error("butteraugli comparator: the image must be at least 8x8 (and below 65536)");
+    // the batch's bound: four z per image in the widest launch of the batched Compare chain
+    if (capacity < 1 || capacity > 16383)
+      throw std::runtime_error("butteraugli comparator: the capacity must be in 1..16383");
+    std::unique_ptr<gb200::Butteraugli> ba(
+        new gb200::Butteraugli(w, h, capacity, device, gb200::Butteraugli::Slots::kCandidates));
+    ba->analyse_original(rgb0);
+    c = new gb200_butteraugli_comparator;
+    c->ba = ba.release();
+  });
+  return c;
+}
+
+namespace {
+int comparator_diffmap_batch(gb200_butteraugli_comparator* c, const float* rgb1, int n, float* diffmap, double* score,
+                             bool device, void* stream) {
+  if (c == nullptr || rgb1 == nullptr) {
+    g_err = "butteraugli comparator: no comparator or no images";
+    return 0;
+  }
+  if (n < 1 || n > c->ba->capacity()) {
+    g_err = "butteraugli comparator: n = " + std::to_string(n) + " images, the comparator takes 1.." +
+            std::to_string(c->ba->capacity());
+    return 0;
+  }
+  return guarded([&]() {
+    c->ba->bind();
+    gb200::Stream caller = 0;
+    if (device) {
+      const void* ptrs[2] = {rgb1, diffmap};
+      const char* what[2] = {"rgb1", "diffmap"};
+      check_device_pointers("butteraugli comparator", c->ba->device(), ptrs, what, 2);
+#if !defined(GB200_HOSTSIM)
+      caller = static_cast<gb200::Stream>(stream);
+#endif
+    }
+    (void)stream;
+    std::vector<float> m(n);
+    c->ba->compare_many(rgb1, n, diffmap, m.data(), device, caller);
+    if (score)
+      for (int i = 0; i < n; ++i) score[i] = m[i];
+  });
+}
+}  // namespace
+
+int gb200_butteraugli_comparator_diffmap_batch(gb200_butteraugli_comparator* c, const float* rgb1, int n,
+                                               float* diffmap, double* score) {
+  return comparator_diffmap_batch(c, rgb1, n, diffmap, score, false, nullptr);
+}
+
+int gb200_butteraugli_comparator_diffmap_batch_device(gb200_butteraugli_comparator* c, const float* rgb1_dev, int n,
+                                                      float* diffmap_dev, double* score, void* stream) {
+  return comparator_diffmap_batch(c, rgb1_dev, n, diffmap_dev, score, true, stream);
+}
+
 // ---- butteraugli::ButteraugliInterface (b/butteraugli.cc:1858) on N pairs per call ----------
 gb200_butteraugli_batch* gb200_butteraugli_batch_create(int w, int h, int capacity, int device) {
   gb200_butteraugli_batch* b = nullptr;

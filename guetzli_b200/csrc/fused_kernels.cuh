@@ -48,8 +48,10 @@ struct PlaneGeom {
   // Batched launches (kernel template argument B): image n keeps its planes in arena slot n,
   // kslot planes (kslot * plane floats) after slot 0, so every pointer moves by n * kslot * plane
   // and every TMA plane coordinate by n * kslot.  The grid's z is n * zimg + (the single-image z).
-  // Single-image instantiations (B = false) read neither field.
-  int kslot, zimg;
+  // The original's planes (ps0, sup0) move by kslot0 planes per image instead: kslot0 = kslot
+  // when every image has its own original, 0 when all images are scored against one.
+  // Single-image instantiations (B = false) read none of these fields.
+  int kslot, zimg, kslot0;
 };
 
 // image index and single-image z of a block of a batched launch; (0, blockIdx.z) when B is false
@@ -59,6 +61,9 @@ __device__ __forceinline__ int batch_image(const PlaneGeom& g) {
 }
 __device__ __forceinline__ size_t slot_offset(const PlaneGeom& g, int n) {
   return static_cast<size_t>(n) * g.kslot * g.plane;
+}
+__device__ __forceinline__ size_t slot_offset0(const PlaneGeom& g, int n) {  // the original's planes
+  return static_cast<size_t>(n) * g.kslot0 * g.plane;
 }
 
 // ---------------------------------------------------------------------------
@@ -564,7 +569,8 @@ __global__ void __launch_bounds__(256) k_tma_blur_2d(const __grid_constant__ CUt
 
 // ---------------------------------------------------------------------------
 // Epilogues.  Plane groups are addressed as base + n * slot + plane_index * g.plane + y * pitch + x,
-// where n is the image of a batched launch (0 otherwise) and slot the floats per arena slot.
+// where n is the image of a batched launch (0 otherwise) and slot the floats per arena slot; the
+// original's planes (ps0) as ps0 + n * slot0 + ..., slot0 = slot or 0 (PlaneGeom::kslot0).
 
 // Each epilogue has two halves: load() fetches the pixel's global operands through the
 // read-only path into a Pre, apply() does the arithmetic and the stores.  The kernels call
@@ -617,18 +623,19 @@ struct EpiMf {
   float* diffs;        // [6]: X uhf, hf, mf; Y uhf, hf, mf
   MaltaParams mp_x, mp_y;
   int pitch;
-  size_t plane, slot;
+  size_t plane, slot, slot0;
   struct Pre {
     float inx, iny, p0x, p0y;
   };
   static constexpr int kChunk = 8;
   __device__ __forceinline__ void load(int x, int y, int n, int, Pre& p) const {
-    const size_t o = n * slot + static_cast<size_t>(y) * pitch + x;
+    const size_t r = static_cast<size_t>(y) * pitch + x, o = n * slot + r;
     p.inx = __ldg(mf_in + o);
     p.iny = __ldg(mf_in + plane + o);
     if (ps0 != nullptr) {
-      p.p0x = __ldg(ps0 + kMfX * plane + o);
-      p.p0y = __ldg(ps0 + kMfY * plane + o);
+      const size_t o0 = n * slot0 + r;
+      p.p0x = __ldg(ps0 + kMfX * plane + o0);
+      p.p0y = __ldg(ps0 + kMfY * plane + o0);
     }
   }
   __device__ __forceinline__ void apply(int x, int y, int n, int, const float v[3], const Pre& p) const {
@@ -680,21 +687,22 @@ struct EpiHf {
   float* noise;         // [1]
   MaltaParams mp_uhf_x, mp_uhf_y, mp_hf_x, mp_hf_y;
   int pitch;
-  size_t plane, slot;
+  size_t plane, slot, slot0;
   struct Pre {
     float lfx, lfy, lfb, u0x, h0x, u0y, h0y;
   };
   static constexpr int kChunk = 4;
   __device__ __forceinline__ void load(int x, int y, int n, Pre& p) const {
-    const size_t o = n * slot + static_cast<size_t>(y) * pitch + x;
+    const size_t r = static_cast<size_t>(y) * pitch + x, o = n * slot + r;
     p.lfx = __ldg(lf_raw + o);
     p.lfy = __ldg(lf_raw + plane + o);
     p.lfb = __ldg(lf_raw + 2 * plane + o);
     if (ps0 != nullptr) {
-      p.u0x = __ldg(ps0 + kUhfX * plane + o);
-      p.h0x = __ldg(ps0 + kHfX * plane + o);
-      p.u0y = __ldg(ps0 + kUhfY * plane + o);
-      p.h0y = __ldg(ps0 + kHfY * plane + o);
+      const size_t o0 = n * slot0 + r;
+      p.u0x = __ldg(ps0 + kUhfX * plane + o0);
+      p.h0x = __ldg(ps0 + kHfX * plane + o0);
+      p.u0y = __ldg(ps0 + kUhfY * plane + o0);
+      p.h0y = __ldg(ps0 + kHfY * plane + o0);
     }
   }
   __device__ __forceinline__ void apply(int x, int y, int n, bool live, const float sharp[2], const float v[2],
@@ -753,14 +761,14 @@ struct EpiNoise {
   float* acc;        // block_diff_ac[Y], read-modify-write (each pixel by exactly one thread)
   double w_0gt1, w_0lt1;
   int pitch;
-  size_t slot;
+  size_t slot, slot0;
   struct Pre {
     float r0, r1, a;
   };
   static constexpr int kChunk = 8;
   __device__ __forceinline__ void load(int x, int y, int n, int, Pre& p) const {
-    const size_t o = n * slot + static_cast<size_t>(y) * pitch + x;
-    p.r0 = __ldg(hf0 + o);
+    const size_t r = static_cast<size_t>(y) * pitch + x, o = n * slot + r;
+    p.r0 = __ldg(hf0 + n * slot0 + r);
     p.r1 = __ldg(hf1 + o);
     p.a = acc[o];  // plain load: this launch writes the location later (same thread)
   }
@@ -896,7 +904,7 @@ __global__ void __launch_bounds__(256) k_tma_mask_y(const __grid_constant__ CUte
   uint64_t* bar = reinterpret_cast<uint64_t*>(tc + C::HC * GBY_TW);
   const int x0 = blockIdx.x * GBY_TW, yb = g.y0 + blockIdx.y * GBY_TH;
   const int n = batch_image<B>(g);
-  const size_t so = slot_offset(g, n);
+  const size_t so = slot_offset(g, n), so0 = slot_offset0(g, n);
   if (threadIdx.x == 0) {
     mbar_init(bar, 1);
     mbar_fence_init();
@@ -928,7 +936,7 @@ __global__ void __launch_bounds__(256) k_tma_mask_y(const __grid_constant__ CUte
   }
   if (x >= g.w) return;
   CombineAndSqrt comb;
-  comb.ps0 = ca.ps0 + so;
+  comb.ps0 = ca.ps0 + so0;
   comb.ps1 = ca.ps1 + so;
   comb.ac = ca.ac + so;
   comb.out = ca.out + so;
@@ -943,9 +951,9 @@ __global__ void __launch_bounds__(256) k_tma_mask_y(const __grid_constant__ CUte
     for (int i = 0; i < CH; ++i) {
       const int y = yg + o0 + i;
       if (y >= g.y_end) continue;
-      const size_t o = so + static_cast<size_t>(y) * ca.pitch + x;
-      l0x[i] = __ldg(ca.ps0 + kLfX * ca.plane + o);
-      l0b[i] = __ldg(ca.ps0 + kLfB * ca.plane + o);
+      const size_t r = static_cast<size_t>(y) * ca.pitch + x, o = so + r, o0 = so0 + r;
+      l0x[i] = __ldg(ca.ps0 + kLfX * ca.plane + o0);
+      l0b[i] = __ldg(ca.ps0 + kLfB * ca.plane + o0);
       l1x[i] = __ldg(ca.ps1 + kLfX * ca.plane + o);
       l1b[i] = __ldg(ca.ps1 + kLfB * ca.plane + o);
       acx[i] = __ldg(ca.ac + o);
@@ -1067,9 +1075,10 @@ template <bool B>
 __global__ void __launch_bounds__(256) k_mask_pre(const float* ps1, const float* sup0, float* mpre, PlaneGeom g) {
   const int x = blockIdx.x * 32 + threadIdx.x, y = g.y0 + blockIdx.y * 8 + threadIdx.y;
   if (x >= g.w || y >= g.y_end) return;
-  const size_t so = slot_offset(g, batch_image<B>(g));
+  const int n = batch_image<B>(g);
+  const size_t so = slot_offset(g, n);
   ps1 += so;
-  sup0 += so;
+  sup0 += slot_offset0(g, n);
   mpre += so;
   const int x2 = (x + 1 < g.w) ? x + 1 : (x > 0 ? x - 1 : x);
   const int y2 = (y + 1 < g.h) ? y + 1 : (y > 0 ? y - 1 : y);

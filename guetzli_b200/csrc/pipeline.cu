@@ -146,15 +146,16 @@ void launch_tma_2d(Stream s, const CUtensorMap& in_map, int nimg, const BlurTab&
 #define GB_R_FINAL 3
 
 // Launches over nimg images take the planes of arena slots 0 .. nimg - 1, kslot planes apart
-// (kslot = 0 and nimg = 1 for a single image); their tensor maps cover every slot.
+// (kslot = 0 and nimg = 1 for a single image); their tensor maps cover every slot.  The original's
+// planes are kslot0 planes apart: kslot0 = kslot when each image has its own, 0 when all share one.
 namespace {
-PlaneGeom fused_geom(const Geom& g, int y0, int y_end, int kslot) {
-  return PlaneGeom{g.w, g.h, g.pitch, g.plane, y0, y_end, kslot, 1};
+PlaneGeom fused_geom(const Geom& g, int y0, int y_end, int kslot, int kslot0) {
+  return PlaneGeom{g.w, g.h, g.pitch, g.plane, y0, y_end, kslot, 1, kslot0};
 }
 }  // namespace
 
 void Butteraugli::fused_opsin(const float* lin, float* xyb, int nimg, int kslot) {
-  const PlaneGeom pg = fused_geom(g_, r_.cr_lo, r_.cr_hi, kslot);
+  const PlaneGeom pg = fused_geom(g_, r_.cr_lo, r_.cr_hi, kslot, kslot);
   typedef Blur2dCfg<GB_R_OPSIN, 3> C;
   const CUtensorMap& m = fused_->slots(lin, 3, C::SWI, C::HI, kslot, g_);
   launch_tma_2d<GB_R_OPSIN, 3>(s_, m, nimg, t_.blur[kBlurOpsin], pg, ht_, kBlurOpsin,
@@ -162,9 +163,9 @@ void Butteraugli::fused_opsin(const float* lin, float* xyb, int nimg, int kslot)
 }
 
 // SeparateFrequencies; with_diffs: also the Malta pre-pass and the noise difference against ps0_.
-void Butteraugli::fused_separate(const float* xyb, float* ps, bool with_diffs, int nimg, int kslot) {
-  const PlaneGeom pg = fused_geom(g_, r_.cr_lo, r_.cr_hi, kslot);
-  const size_t P = g_.plane, S = kslot * P;
+void Butteraugli::fused_separate(const float* xyb, float* ps, bool with_diffs, int nimg, int kslot, int kslot0) {
+  const PlaneGeom pg = fused_geom(g_, r_.cr_lo, r_.cr_hi, kslot, kslot0);
+  const size_t P = g_.plane, S = kslot * P, S0 = kslot0 * P;
   // S2: lf = Blur(xyb, 7.47); mf_in = xyb - lf
   // (launch names are those of the former y-pass kernels, which these replace)
   launch_roll<GB_R_LF, 1>(s_, fused_->slots(xyb, 3, RollCfg<GB_R_LF, 1>::SW, GBR_CH, kslot, g_), 3, nimg, t_.blur[kBlurLf], pg, ht_,
@@ -181,6 +182,7 @@ void Butteraugli::fused_separate(const float* xyb, float* ps, bool with_diffs, i
   em.pitch = g_.pitch;
   em.plane = P;
   em.slot = S;
+  em.slot0 = S0;
   launch_roll<GB_R_MF, 3>(s_, fused_->slots(mf_in_, 3, RollCfg<GB_R_MF, 3>::SW, GBR_CH, kslot, g_), 1, nimg, t_.blur[kBlurMf], pg,
                           ht_, kBlurMf, em, "mf_fused_y");
   // S5 + S6: hf = Blur(hf_raw, 1.87) in one kernel; uhf / hf / lf "vals" (+ Malta pre-pass, noise difference)
@@ -197,6 +199,7 @@ void Butteraugli::fused_separate(const float* xyb, float* ps, bool with_diffs, i
   eh.pitch = g_.pitch;
   eh.plane = P;
   eh.slot = S;
+  eh.slot0 = S0;
   typedef Blur2dCfg<GB_R_HF, 2> C;
   launch_tma_2d<GB_R_HF, 2>(s_, fused_->slots(hf_raw_, 2, C::SWI, C::HI, kslot, g_), nimg, t_.blur[kBlurHf], pg, ht_, kBlurHf, eh,
                             "hf_fused");
@@ -205,7 +208,7 @@ void Butteraugli::fused_separate(const float* xyb, float* ps, bool with_diffs, i
 // Neighbour sums of DiffPrecompute for the original's PsychoImage (constant during the search).
 void Butteraugli::fused_sup0(int nimg, int kslot) {
   if (!use_fused_) return;
-  const PlaneGeom pg = fused_geom(g_, r_.cr_lo, r_.cr_hi, kslot);
+  const PlaneGeom pg = fused_geom(g_, r_.cr_lo, r_.cr_hi, kslot, kslot);
   const int rows = r_.cr_hi - r_.cr_lo;
   dim3 block(32, 8), grid(cdiv(g_.w, 32), cdiv(rows, 8), nimg);
   note_launch("mask_sup0", s_, static_cast<double>(g_.w) * rows * nimg);
@@ -215,7 +218,7 @@ void Butteraugli::fused_sup0(int nimg, int kslot) {
 
 // One separable blur of a plane group (tests, one-time mask of the original).
 void Butteraugli::fused_blur(const float* in, float* out, int nplanes, int id) {
-  const PlaneGeom pg = fused_geom(g_, r_.cr_lo, r_.cr_hi, 0);
+  const PlaneGeom pg = fused_geom(g_, r_.cr_lo, r_.cr_hi, 0, 0);
   const EpiStore st{out, g_.pitch, g_.plane};
 #define GB_BLUR_CASE(R)                                                                                               \
   case R:                                                                                                             \
@@ -259,7 +262,7 @@ void Butteraugli::fused_compare_submit() {
     GB_CUDA(cudaStreamBeginCapture(s_, cudaStreamCaptureModeThreadLocal));
     cudaGraph_t graph = nullptr;
     try {
-      fused_compare_launches(1, 0);
+      fused_compare_launches(1, 0, 0);
     } catch (...) {
       cudaStreamEndCapture(s_, &graph);
       if (graph) cudaGraphDestroy(graph);
@@ -275,7 +278,7 @@ void Butteraugli::fused_compare_submit() {
     GB_CUDA(cudaGraphLaunch(fused_->compare_graph, s_));
     add_launches(recorded);
   } else {
-    fused_compare_launches(1, 0);
+    fused_compare_launches(1, 0, 0);
   }
   ++fused_->compare_calls;
 }
@@ -297,12 +300,12 @@ float Butteraugli::fused_compare_result() {
 }
 
 // the stream work of one Compare after the render: no host synchronisation inside
-void Butteraugli::fused_compare_launches(int nimg, int kslot) {
-  const PlaneGeom pg = fused_geom(g_, r_.cr_lo, r_.cr_hi, kslot);
-  const size_t P = g_.plane, S = kslot * P;
+void Butteraugli::fused_compare_launches(int nimg, int kslot, int kslot0) {
+  const PlaneGeom pg = fused_geom(g_, r_.cr_lo, r_.cr_hi, kslot, kslot0);
+  const size_t P = g_.plane, S = kslot * P, S0 = kslot0 * P;
   const int rows = r_.cr_hi - r_.cr_lo;
   fused_opsin(lin_, xyb_, nimg, kslot);
-  fused_separate(xyb_, ps1_, true, nimg, kslot);
+  fused_separate(xyb_, ps1_, true, nimg, kslot, kslot0);
   // S10 mask: DiffPrecompute against the original's resident neighbour sums
   {
     dim3 block(32, 8), grid(cdiv(g_.w, 32), cdiv(rows, 8), nimg);
@@ -351,7 +354,7 @@ void Butteraugli::fused_compare_launches(int nimg, int kslot) {
   // S8 tail + S9 on block_diff_ac[Y]: blurred noise difference, asymmetric L2 of hf[Y]
   launch_tma_y<GB_R_NOISE, 1>(s_, fused_->slots(blr_, 1, GBY_TW, GBY_TH + 2 * GB_R_NOISE, kslot, g_), 1, nimg,
                               t_.blur[kBlurNoise], pg, ht_, kBlurNoise,
-                              EpiNoise{ps0_ + kHfY * P, ps1_ + kHfY * P, ac_ + P, asym_w0_, asym_w1_, g_.pitch, S},
+                              EpiNoise{ps0_ + kHfY * P, ps1_ + kHfY * P, ac_ + P, asym_w0_, asym_w1_, g_.pitch, S, S0},
                               "noise_fused_y");
   // y passes + S11 CombineChannels + first half of S12 -> dm_[1]
   {
@@ -383,14 +386,16 @@ void Butteraugli::fused_compare_launches(int nimg, int kslot) {
 void Butteraugli::fused_compare_batch(const float* rgb0, const float* rgb1, int n, float* diffmap, float* maxima) {
   const size_t row = sizeof(float) * g_.w, pitch = sizeof(float) * g_.pitch;
   const size_t slot_rows = static_cast<size_t>(kslot_) * g_.h;  // a plane is h rows of pitch
-  // [n][3][h][w] -> the lin planes of slots 0 .. n - 1: n slices of 3h rows
-  copy_3d(lin_, pitch, slot_rows, rgb0, row, static_cast<size_t>(3) * g_.h, row, static_cast<size_t>(3) * g_.h, n, s_);
-  // PsychoImage of every original (butteraugli.cc:784) and its DiffPrecompute neighbour sums
-  fused_opsin(lin_, xyb_, n, kslot_);
-  fused_separate(xyb_, ps0_, false, n, kslot_);
-  fused_sup0(n, kslot_);
+  if (rgb0 != nullptr) {
+    // [n][3][h][w] -> the lin planes of slots 0 .. n - 1: n slices of 3h rows
+    copy_3d(lin_, pitch, slot_rows, rgb0, row, static_cast<size_t>(3) * g_.h, row, static_cast<size_t>(3) * g_.h, n, s_);
+    // PsychoImage of every original (butteraugli.cc:784) and its DiffPrecompute neighbour sums
+    fused_opsin(lin_, xyb_, n, kslot_);
+    fused_separate(xyb_, ps0_, false, n, kslot_, kslot_);
+    fused_sup0(n, kslot_);
+  }
   copy_3d(lin_, pitch, slot_rows, rgb1, row, static_cast<size_t>(3) * g_.h, row, static_cast<size_t>(3) * g_.h, n, s_);
-  fused_compare_launches(n, kslot_);
+  fused_compare_launches(n, kslot_, rgb0 != nullptr ? kslot_ : 0);
   if (diffmap != nullptr) copy_3d(diffmap, row, g_.h, dm_, pitch, slot_rows, row, g_.h, n, s_);
   // one transfer of the n maxima (float bits); d2h waits for it, and so for everything queued before
   d2h(maxima, d_gmax_, sizeof(float) * n, s_);
@@ -444,7 +449,7 @@ void Butteraugli::opsin(const float* lin, float* xyb) {
 
 void Butteraugli::separate(const float* xyb, float* ps) {
 #if !defined(GB200_HOSTSIM)
-  if (use_fused_) return fused_separate(xyb, ps, false, 1, 0);
+  if (use_fused_) return fused_separate(xyb, ps, false, 1, 0, 0);
 #endif
   blur(xyb, lf_, 3, kBlurLf);
   r_.px(SubPlanes{xyb, lf_, mf_in_, g_}, "sub_planes", 3);

@@ -108,6 +108,24 @@ int gb200_butteraugli_comparator_diffmap_device(gb200_butteraugli_comparator* c,
 /* ButteraugliComparator::Mask (butteraugli.cc:793): mask and mask_dc, [3][h][w] each, host memory. */
 int gb200_butteraugli_comparator_mask(gb200_butteraugli_comparator* c, float* mask, float* mask_dc);
 void gb200_butteraugli_comparator_destroy(gb200_butteraugli_comparator* c);
+/* A comparator that scores up to `capacity` images per call against its original, all of them in one
+ * pass of the Compare chain, one launch per stage; the original is analysed once, here (DESIGN.md §4).
+ * w, h as in gb200_butteraugli_comparator_create; 1 <= capacity <= 16383.  Capacity 1 is the comparator
+ * gb200_butteraugli_comparator_create makes.  The other comparator calls work on it unchanged.  NULL on
+ * failure (gb200_last_error), with nothing left allocated. */
+gb200_butteraugli_comparator* gb200_butteraugli_comparator_create_batch(const float* rgb0, int w, int h, int capacity,
+                                                                        int device);
+/* ButteraugliComparator::Diffmap (butteraugli.cc:799) and ButteraugliScoreFromDiffmap (butteraugli.cc:1623)
+ * for each image: rgb1 [n][3][h][w] in host memory, 1 <= n <= capacity; diffmap (may be NULL) receives
+ * [n][h][w], score (may be NULL) [n], the maximum of each diffmap.  Each image gets the bits that
+ * gb200_butteraugli_comparator_diffmap gives for it.  The reference class has no batched call. */
+int gb200_butteraugli_comparator_diffmap_batch(gb200_butteraugli_comparator* c, const float* rgb1, int n,
+                                               float* diffmap, double* score);
+/* The same with rgb1 and diffmap (may be NULL) in device memory of the comparator's device; stream as in
+ * gb200_butteraugli_comparator_diffmap_device.  A host pointer or memory of another device is refused,
+ * nothing runs. */
+int gb200_butteraugli_comparator_diffmap_batch_device(gb200_butteraugli_comparator* c, const float* rgb1_dev, int n,
+                                                      float* diffmap_dev, double* score, void* stream);
 /* ---- batched butteraugli: N same-size pairs per call ----
  * Each pair (rgb0[i], rgb1[i]) gets butteraugli::ButteraugliInterface (butteraugli.cc:1858), bit for bit
  * what gb200_butteraugli_diffmap gives for it alone.  Up to `capacity` pairs of w x h images run through

@@ -11,8 +11,13 @@ With --batch N, two more modes score N distinct pairs (a different original in e
   batch_cuda      one gb200_butteraugli_batch of capacity N, pairs and diffmaps as CUDA torch tensors
   batch_host      the same batch, pairs and diffmaps in host memory
 
-and the result gains ms per pair of the batch modes and MPix/s (scored pixels per second) of every
-mode.  Every call returns once its diffmaps are written, so a host clock around `--n` calls is the
+and two more score N distinct candidates against the one original per call:
+
+  comparator_batch_cuda  one comparator of capacity N, candidates and diffmaps as CUDA torch tensors
+  comparator_batch_host  the same comparator, candidates and diffmaps in host memory
+
+and the result gains ms per pair or candidate of the batched modes and MPix/s (scored pixels per
+second) of every mode.  Every call returns once its diffmaps are written, so a host clock around `--n` calls is the
 time of the work.  The modes run in turn for `--rounds` rounds (the spread between rounds is part of the
 result), after `--warmup` untimed calls each.  The card's name and power limit are read in the
 same run (nvidia-smi, read-only queries).  Prints one JSON line; --out also writes it to a file.
@@ -98,6 +103,17 @@ def main():
         b0_dev, b1_dev = torch.from_numpy(b0).to(dev), torch.from_numpy(b1).to(dev)
         torch.cuda.synchronize(dev)
         batch = gb.ButteraugliBatch(h, w, nb, device=args.device)
+        c1 = np.stack([linear(np.clip(base + synth.noise(h, w, 5000 + k) % 7 - 3, 0, 255).astype(np.uint8))
+                       for k in range(nb)])
+        c1_dev = torch.from_numpy(c1).to(dev)
+        torch.cuda.synchronize(dev)
+        cmpb = gb.Comparator(orig, device=args.device, capacity=nb)
+
+        def comparator_batch_cuda(i):
+            return cmpb.diffmap(c1_dev)[1].tolist()
+
+        def comparator_batch_host(i):
+            return cmpb.diffmap(c1)[1].tolist()
 
         def batch_cuda(i):
             return batch.diffmap(b0_dev, b1_dev)[1].tolist()
@@ -105,8 +121,9 @@ def main():
         def batch_host(i):
             return batch.diffmap(b0, b1)[1].tolist()
 
-        modes.update(batch_cuda=batch_cuda, batch_host=batch_host)
-        per_call.update(batch_cuda=nb, batch_host=nb)
+        modes.update(batch_cuda=batch_cuda, batch_host=batch_host, comparator_batch_cuda=comparator_batch_cuda,
+                     comparator_batch_host=comparator_batch_host)
+        per_call.update(batch_cuda=nb, batch_host=nb, comparator_batch_cuda=nb, comparator_batch_host=nb)
     scores = {}
     for name, f in modes.items():
         for i in range(args.warmup):
@@ -124,6 +141,10 @@ def main():
                 f(i)
             torch.cuda.synchronize(dev)
             ms[name].append((time.perf_counter() - t0) / args.n * 1e3 / per_call[name])
+    if args.batch > 0:
+        # the last candidate of the batched comparator scores as it does alone
+        cand_alone = cmp.diffmap(c1[-1])[1]
+        cmpb.close()
     cmp.close()
 
     def stats(v):
@@ -139,9 +160,13 @@ def main():
         alone = gb.api.butteraugli_diffmap(b0[0], b1[0], device=args.device)[1]
         result["batch"] = args.batch
         result["ms_per_pair"] = {m: stats(ms[m]) for m in ("batch_cuda", "batch_host")}
+        result["ms_per_candidate"] = {m: stats(ms[m]) for m in ("comparator_batch_cuda", "comparator_batch_host")}
         result["mpix_per_s"] = {m: round(w * h / 1e3 / statistics.median(v), 2) for m, v in ms.items()}
         result["batch_scores_consistent"] = (all(s == scores["batch_cuda"][0] for m in ("batch_cuda", "batch_host")
                                                  for s in scores[m]) and scores["batch_cuda"][0][0] == alone)
+        cb = ("comparator_batch_cuda", "comparator_batch_host")
+        result["comparator_batch_scores_consistent"] = (
+            all(s == scores[cb[0]][0] for m in cb for s in scores[m]) and scores[cb[0]][0][-1] == cand_alone)
     result.update(gpu_info(args.device))
     line = json.dumps(result)
     print(line)
