@@ -242,8 +242,10 @@ def read_jpeg(jpeg_in, lib=None):
 
 
 def butteraugli_diffmap(rgb0, rgb1, device=0, lib=None):
-    """butteraugli::ButteraugliInterface: rgb0, rgb1 planar linear RGB float32 [3][h][w] (0..255).
-    -> (diffmap [h][w] float32, score)."""
+    """butteraugli::ButteraugliInterface: rgb0, rgb1 planar linear RGB float32 [3][h][w], nominally in
+    0..255 -> (diffmap [h][w] float32, score).  Values outside 0..255 (ringing below 0, highlights above 255) are scored as the reference scores
+    them, bit for bit; this is tested from -300 to 4500.  NaN and infinities must not be passed: the
+    reference's result is undefined for them."""
     lib = lib or load_library()
     a = np.ascontiguousarray(rgb0, dtype=np.float32)
     b = np.ascontiguousarray(rgb1, dtype=np.float32)
@@ -265,9 +267,11 @@ def _is_torch_tensor(x):
 
 class Comparator:
     """butteraugli::ButteraugliComparator (butteraugli.h:425) on one GPU: the original rgb0, planar
-    linear RGB float32 [3][h][w] in 0..255 and at least 8x8, stays resident and is scored against
-    any number of images, up to `capacity` (1..16383) of them per diffmap() call in one pass of the
-    Compare chain.  Used by one thread at a time."""
+    linear RGB float32 [3][h][w], nominally in 0..255 and at least 8x8, stays resident and is scored
+    against any number of images, up to `capacity` (1..16383) of them per diffmap() call in one pass of
+    the Compare chain.  Used by one thread at a time.  Values outside 0..255 (ringing below 0, highlights above 255) are scored as the reference scores
+    them, bit for bit; this is tested from -300 to 4500.  NaN and infinities must not be passed: the
+    reference's result is undefined for them."""
 
     def __init__(self, rgb0, device=0, capacity=1, lib=None):
         self.lib = lib or load_library()
@@ -368,8 +372,10 @@ class Comparator:
 class ButteraugliBatch:
     """butteraugli::ButteraugliInterface on up to `capacity` same-size pairs per call, on one GPU: each
     pair (rgb0[i], rgb1[i]) is scored as gb.butteraugli_diffmap scores it alone, bit for bit, with the
-    pairs going through the Compare chain together.  Images are planar linear RGB float32 in 0..255,
-    at least 8x8.  Used by one thread at a time."""
+    pairs going through the Compare chain together.  Images are planar linear RGB float32, nominally in
+    0..255, at least 8x8.  Used by one thread at a time.  Values outside 0..255 (ringing below 0, highlights above 255) are scored as the reference scores
+    them, bit for bit; this is tested from -300 to 4500.  NaN and infinities must not be passed: the
+    reference's result is undefined for them."""
 
     def __init__(self, h, w, capacity, device=0, lib=None):
         self.lib = lib or load_library()
@@ -438,8 +444,11 @@ class ButteraugliBatch:
 
 
 def adaptive_quantization(rgb, device=0, lib=None):
-    """butteraugli::ButteraugliAdaptiveQuantization: rgb planar linear RGB float32 [3][h][w] (0..255)
-    -> quant [h][w] float32.  Raises ValueError below 16x16, where the reference returns false."""
+    """butteraugli::ButteraugliAdaptiveQuantization: rgb planar linear RGB float32 [3][h][w], nominally
+    in 0..255 -> quant [h][w] float32.  Raises ValueError below 16x16, where the reference returns
+    false.  Values outside 0..255 (ringing below 0, highlights above 255) are scored as the reference scores
+    them, bit for bit; this is tested from -300 to 4500.  NaN and infinities must not be passed: the
+    reference's result is undefined for them."""
     lib = lib or load_library()
     a = np.ascontiguousarray(rgb, dtype=np.float32)
     if a.ndim != 3 or a.shape[0] != 3:

@@ -80,14 +80,18 @@ int gb200_process_jpeg(const gb200_params* params, const uint8_t* jpeg_in, size_
 
 /* butteraugli::ButteraugliInterface(rgb0, rgb1, diffmap, diffvalue)
  * (third_party/butteraugli/butteraugli/butteraugli.cc:1858; the stand-alone `butteraugli`
- * tool, butteraugli_main.cc:362): both images as planar linear RGB floats [3][h][w] in
- * 0..255; diffmap (may be NULL) receives w*h floats, *score their maximum. */
+ * tool, butteraugli_main.cc:362): both images as planar linear RGB floats [3][h][w], nominally in
+ * 0..255; diffmap (may be NULL) receives w*h floats, *score their maximum.  Values outside 0..255
+ * (ringing below 0, highlights above 255) are scored as the reference scores them, bit for bit; this
+ * is tested from -300 to 4500.  NaN and infinities must not be passed: the reference's result is
+ * undefined for them.  The same holds for every butteraugli entry below. */
 int gb200_butteraugli_diffmap(const float* rgb0, const float* rgb1, int w, int h, int device, float* diffmap,
                               double* score);
 
 /* ---- butteraugli::ButteraugliComparator (third_party/butteraugli/butteraugli/butteraugli.h:425) ----
  * One original kept resident on one GPU (its PsychoImage, the neighbour sums of its mask) and scored
- * against any number of images.  Images are planar linear RGB floats [3][h][w] in 0..255, the
+ * against any number of images.  Images are planar linear RGB floats [3][h][w], nominally in 0..255
+ * (values outside it as for gb200_butteraugli_diffmap), the
  * original at least 8x8 (the reference class computes nothing below that; gb200_butteraugli_diffmap
  * pads small images).  One comparator is used by one thread at a time; separate comparators may run
  * concurrently, each has its own stream.  Every call returns once its outputs are written. */
@@ -130,7 +134,8 @@ int gb200_butteraugli_comparator_diffmap_batch_device(gb200_butteraugli_comparat
  * Each pair (rgb0[i], rgb1[i]) gets butteraugli::ButteraugliInterface (butteraugli.cc:1858), bit for bit
  * what gb200_butteraugli_diffmap gives for it alone.  Up to `capacity` pairs of w x h images run through
  * the Compare chain together, one launch per stage, each pair in its own slot of device memory
- * (DESIGN.md §4).  Images are planar linear RGB floats in 0..255, at least 8x8.  One batch object is
+ * (DESIGN.md §4).  Images are planar linear RGB floats, nominally in 0..255 (values outside it as for
+ * gb200_butteraugli_diffmap), at least 8x8.  One batch object is
  * used by one thread at a time; separate objects may run concurrently, each has its own stream.  Every
  * call returns once its outputs are written. */
 typedef struct gb200_butteraugli_batch gb200_butteraugli_batch;

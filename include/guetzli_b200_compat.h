@@ -129,8 +129,10 @@ inline bool Process(const Params& params, ProcessStats* stats, const std::string
 namespace guetzli_b200 {
 
 // butteraugli::ButteraugliComparator (third_party/butteraugli/butteraugli/butteraugli.h:425) with
-// the original resident on one GPU.  Images are three planes of linear RGB (0..255), each w*h floats
-// row by row, as ButteraugliAdaptiveQuantization takes them; outputs are laid out the same way.
+// the original resident on one GPU.  Images are three planes of linear RGB (nominally 0..255; values
+// outside it are scored as the reference scores them, tested from -300 to 4500; no NaN or infinity),
+// each w*h floats row by row, as ButteraugliAdaptiveQuantization takes them; outputs are laid out the
+// same way.
 // The methods return false on failure (gb200_last_error), where the reference's return nothing.
 // One comparator is used by one thread at a time.
 class ButteraugliComparator {
