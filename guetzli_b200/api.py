@@ -111,6 +111,18 @@ def load_library(path=None):
     lib.gb200_butteraugli_batch_diffmap_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
                                                            C.c_void_p, C.c_void_p]
     lib.gb200_butteraugli_batch_destroy.argtypes = [C.c_void_p]
+    lib.gb200_butteraugli_diffmap_srgb.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
+                                                   C.c_void_p, P(C.c_double)]
+    lib.gb200_butteraugli_batch_diffmap_srgb.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                                         C.c_void_p, C.c_void_p]
+    lib.gb200_butteraugli_batch_diffmap_srgb_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                                                C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.gb200_butteraugli_comparator_create_srgb.restype = C.c_void_p
+    lib.gb200_butteraugli_comparator_create_srgb.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]
+    lib.gb200_butteraugli_comparator_diffmap_srgb.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                                                              C.c_void_p]
+    lib.gb200_butteraugli_comparator_diffmap_srgb_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                                                                     C.c_void_p, C.c_void_p]
     _libs[path] = lib
     return lib
 
@@ -265,6 +277,52 @@ def _is_torch_tensor(x):
     return type(x).__module__.split(".")[0] == "torch"
 
 
+def _srgb_images(name, x, ranks, cuda_ok=True):
+    """Checks an 8-bit image argument: a uint8 numpy array, or a CUDA torch tensor where cuda_ok, whose
+    rank is in `ranks` and whose last axis holds 3 (RGB) or 4 (RGBA) channels -> (x, is_cuda), contiguous."""
+    cuda = _is_torch_tensor(x) and x.is_cuda
+    if cuda and not cuda_ok:
+        raise ValueError(f"{name} must be in host memory (a numpy array), got a CUDA tensor")
+    if cuda:
+        import torch
+        if x.dtype != torch.uint8:
+            raise ValueError(f"{name} must be uint8, got {x.dtype}")
+        x = x.contiguous()
+    else:
+        if _is_torch_tensor(x):
+            x = x.numpy()
+        x = np.asarray(x)
+        if x.dtype != np.uint8:
+            raise ValueError(f"{name} must be uint8, got {x.dtype}")
+        x = np.ascontiguousarray(x)
+    if x.ndim not in ranks:
+        raise ValueError(f"{name} must have {' or '.join(str(r) for r in ranks)} axes ([n][h][w][C] or [h][w][C]), "
+                         f"got shape {tuple(x.shape)}")
+    if x.shape[-1] not in (3, 4):
+        raise ValueError(f"{name} must have 3 (RGB) or 4 (RGBA) channels in its last axis, got shape {tuple(x.shape)}")
+    return x, cuda
+
+
+def butteraugli_srgb(img0, img1, device=0, lib=None):
+    """The stand-alone `butteraugli` tool's comparison of two 8-bit sRGB images: img0, img1 uint8
+    [h][w][C] in host memory, C = 3 (RGB) or 4 (RGBA), any size from 1x1 -> (diffmap [h][w] float32,
+    score).  Each image is converted to linear RGB with the tool's table; RGBA is laid over black and
+    over white in sRGB space, and the larger score wins with its diffmap (black on a tie).  The result
+    is butteraugli_diffmap's on the converted planes, bit for bit."""
+    lib = lib or load_library()
+    a, _ = _srgb_images("img0", img0, (3,), cuda_ok=False)
+    b, _ = _srgb_images("img1", img1, (3,), cuda_ok=False)
+    if a.shape != b.shape:
+        raise ValueError(f"img0 and img1 differ in shape: {a.shape} and {b.shape}")
+    h, w, ch = a.shape
+    dm = np.empty((h, w), dtype=np.float32)
+    score = C.c_double()
+    if not lib.gb200_butteraugli_diffmap_srgb(a.ctypes.data, b.ctypes.data, w, h, ch, device, dm.ctypes.data,
+                                              C.byref(score)):
+        raise RuntimeError(_err(lib))
+    return dm, score.value
+
+
 class Comparator:
     """butteraugli::ButteraugliComparator (butteraugli.h:425) on one GPU: the original rgb0, planar
     linear RGB float32 [3][h][w], nominally in 0..255 and at least 8x8, stays resident and is scored
@@ -276,6 +334,7 @@ class Comparator:
     def __init__(self, rgb0, device=0, capacity=1, lib=None):
         self.lib = lib or load_library()
         self._h = None
+        self.channels = 0  # made from float planes
         a = np.ascontiguousarray(rgb0, dtype=np.float32)
         if a.ndim != 3 or a.shape[0] != 3:
             raise ValueError(f"rgb0 must be planar [3][h][w], got shape {a.shape}")
@@ -288,6 +347,24 @@ class Comparator:
                                                                          self.capacity, device)
         if not self._h:
             raise RuntimeError("gb200_butteraugli_comparator_create failed: " + _err(self.lib))
+
+    @classmethod
+    def from_srgb(cls, img0, capacity=1, device=0, lib=None):
+        """A comparator whose original is an 8-bit sRGB image, uint8 [h][w][C] in host memory with C = 3
+        (RGB) or 4 (RGBA), at least 8x8, scored as butteraugli_srgb scores it.  With C = 4 the original
+        is kept twice, laid over black and over white.  diffmap() then takes uint8 [h][w][C] or
+        [n][h][w][C] with the same C, numpy or CUDA tensors, and nothing else; mask() refuses RGBA."""
+        self = cls.__new__(cls)
+        self.lib = lib or load_library()
+        self._h = None
+        a, _ = _srgb_images("img0", img0, (3,), cuda_ok=False)
+        self.h, self.w, self.channels = a.shape
+        self.device, self.capacity = device, int(capacity)
+        self._h = self.lib.gb200_butteraugli_comparator_create_srgb(a.ctypes.data, self.w, self.h, self.channels,
+                                                                    self.capacity, device)
+        if not self._h:
+            raise RuntimeError("gb200_butteraugli_comparator_create_srgb failed: " + _err(self.lib))
+        return self
 
     def close(self):
         if self._h:
@@ -309,7 +386,11 @@ class Comparator:
         Anything else is read as a numpy array in host memory.
 
         rgb1 float32 [n][3][h][w] with 1 <= n <= capacity scores each image the same way, all in one
-        call -> (diffmaps [n][h][w], scores float64 ndarray [n])."""
+        call -> (diffmaps [n][h][w], scores float64 ndarray [n]).
+
+        On a comparator made by from_srgb, rgb1 is uint8 [h][w][C] or [n][h][w][C] instead."""
+        if self.channels:
+            return self._diffmap_srgb(rgb1)
         if len(getattr(rgb1, "shape", ())) == 4:
             return self._diffmap_batch(rgb1)
         if _is_torch_tensor(rgb1) and rgb1.is_cuda:
@@ -360,6 +441,27 @@ class Comparator:
         self._ck(self.lib.gb200_butteraugli_comparator_diffmap_batch(self._h, a.ctypes.data, n, dm.ctypes.data,
                                                                      score.ctypes.data))
         return dm, score
+
+    def _diffmap_srgb(self, img1):
+        x, cuda = _srgb_images("img1", img1, (3, 4))
+        single = x.ndim == 3
+        shape = tuple(x.shape[1:] if not single else x.shape)
+        n = 1 if single else x.shape[0]
+        if shape != (self.h, self.w, self.channels) or not 1 <= n <= self.capacity:
+            raise ValueError(f"img1 must have shape [{self.h}, {self.w}, {self.channels}] or [n, {self.h}, {self.w}, "
+                             f"{self.channels}] with 1 <= n <= {self.capacity}, got {tuple(x.shape)}")
+        score = np.empty(n, dtype=np.float64)
+        if cuda:
+            import torch
+            dm = torch.empty((n, self.h, self.w), dtype=torch.float32, device=x.device)
+            stream = torch.cuda.current_stream(x.device).cuda_stream
+            self._ck(self.lib.gb200_butteraugli_comparator_diffmap_srgb_device(self._h, x.data_ptr(), n, dm.data_ptr(),
+                                                                               score.ctypes.data, stream))
+        else:
+            dm = np.empty((n, self.h, self.w), dtype=np.float32)
+            self._ck(self.lib.gb200_butteraugli_comparator_diffmap_srgb(self._h, x.ctypes.data, n, dm.ctypes.data,
+                                                                        score.ctypes.data))
+        return (dm[0], float(score[0])) if single else (dm, score)
 
     def mask(self):
         """ButteraugliComparator::Mask -> (mask, mask_dc), float32 [3][h][w] each."""
@@ -439,6 +541,38 @@ class ButteraugliBatch:
         stream = torch.cuda.current_stream(t0.device).cuda_stream
         if not self.lib.gb200_butteraugli_batch_diffmap_device(self._h, t0.data_ptr(), t1.data_ptr(), n, dm.data_ptr(),
                                                                score.ctypes.data, stream):
+            raise RuntimeError(_err(self.lib))
+        return dm, score
+
+    def diffmap_srgb(self, img0, img1):
+        """The same for 8-bit sRGB pairs, each scored as butteraugli_srgb scores it: img0, img1 uint8
+        [n][h][w][C], C = 3 (RGB) or 4 (RGBA) -> (diffmaps [n][h][w], scores float64 [n]).  Host arrays
+        are uploaded once as bytes; CUDA tensors are read in place after the work queued on their device's
+        current torch stream, and the diffmaps come back as a tensor on that device."""
+        a, cuda0 = _srgb_images("img0", img0, (4,))
+        b, cuda1 = _srgb_images("img1", img1, (4,))
+        if cuda0 != cuda1:
+            raise ValueError("img0 and img1 must both be CUDA tensors or both host arrays")
+        if tuple(a.shape) != tuple(b.shape):
+            raise ValueError(f"img0 and img1 differ in shape: {tuple(a.shape)} and {tuple(b.shape)}")
+        n, h, w, ch = a.shape
+        if (h, w) != (self.h, self.w) or not 1 <= n <= self.capacity:
+            raise ValueError(f"img0 and img1 must have shape [n, {self.h}, {self.w}, C] with 1 <= n <= "
+                             f"{self.capacity}, got {tuple(a.shape)}")
+        score = np.empty(n, dtype=np.float64)
+        if cuda0:
+            import torch
+            if a.device != b.device:
+                raise ValueError(f"img0 and img1 are on different devices: {a.device} and {b.device}")
+            dm = torch.empty((n, h, w), dtype=torch.float32, device=a.device)
+            stream = torch.cuda.current_stream(a.device).cuda_stream
+            ok = self.lib.gb200_butteraugli_batch_diffmap_srgb_device(self._h, a.data_ptr(), b.data_ptr(), n, ch,
+                                                                      dm.data_ptr(), score.ctypes.data, stream)
+        else:
+            dm = np.empty((n, h, w), dtype=np.float32)
+            ok = self.lib.gb200_butteraugli_batch_diffmap_srgb(self._h, a.ctypes.data, b.ctypes.data, n, ch,
+                                                               dm.ctypes.data, score.ctypes.data)
+        if not ok:
             raise RuntimeError(_err(self.lib))
         return dm, score
 

@@ -2,7 +2,8 @@
 //   butteraugli image1.png image2.png [heatmap.ppm]
 // Interface, messages, score format and heat map of
 // third_party/butteraugli/butteraugli/butteraugli_main.cc:362-455; the distance map
-// comes from gb200_butteraugli_diffmap (ButteraugliInterface, butteraugli.cc:1858).
+// comes from gb200_butteraugli_diffmap_srgb (the tool's sRGB conversion and alpha rule in front of
+// ButteraugliInterface, butteraugli.cc:1858).
 // PNG input only: the reference decodes JPEG with libjpeg, whose IDCT this repo does
 // not reproduce, so JPEG arguments are refused instead of scored differently.
 #include <math.h>
@@ -58,35 +59,6 @@ Picture ReadImageOrDie(const char* name) {
   return p;
 }
 
-// butteraugli_main.cc:137 / :239: sRGB byte -> linear 0..255; transparent pixels are laid
-// over `background` in sRGB space first.
-void ToLinear(const Picture& p, int background, std::vector<float>* planes) {
-  static double table[256];
-  static bool ready = false;
-  if (!ready) {
-    for (int i = 0; i < 256; ++i) {
-      const double srgb = i / 255.0;
-      table[i] = 255.0 * (srgb <= 0.04045 ? srgb / 12.92 : pow((srgb + 0.055) / 1.055, 2.4));
-    }
-    ready = true;
-  }
-  const size_t n = static_cast<size_t>(p.w) * p.h;
-  planes->resize(3 * n);
-  for (int c = 0; c < 3; ++c)
-    for (size_t i = 0; i < n; ++i) {
-      int v = p.rgba[4 * i + c];
-      if (p.has_alpha) {
-        const int a = p.rgba[4 * i + 3];
-        if (a == 0) {
-          v = background;
-        } else if (a != 255) {
-          v = (v * a + background * (255 - a) + 127) / 255;
-        }
-      }
-      (*planes)[c * n + i] = static_cast<float>(table[v]);
-    }
-}
-
 // butteraugli.cc:1902 / :1923
 double FuzzyClass(double score) {
   const double width_up = 6.07887388532, width_down = 5.50793514384, m0 = 2.0, scaler = 0.840253347958;
@@ -124,12 +96,27 @@ void ScoreToRgb(double score, double good, double bad, uint8_t rgb[3]) {
   }
 }
 
-bool Compare(const Picture& a, const Picture& b, int background, int device, std::vector<float>* map, double* value) {
-  std::vector<float> l0, l1;
-  ToLinear(a, background, &l0);
-  ToLinear(b, background, &l1);
+// The tool's comparison (butteraugli_main.cc:239-281, :390-419): with alpha over black and over white,
+// the larger distance and its map win.
+bool Compare(const Picture& a, const Picture& b, int device, std::vector<float>* map, double* value) {
+  const int channels = a.has_alpha ? 4 : 3;
+  std::vector<uint8_t> rgb0, rgb1;
+  const uint8_t* p0 = a.rgba.data();
+  const uint8_t* p1 = b.rgba.data();
+  if (channels == 3) {  // the reader gives RGBA
+    const size_t n = static_cast<size_t>(a.w) * a.h;
+    rgb0.resize(3 * n);
+    rgb1.resize(3 * n);
+    for (size_t i = 0; i < n; ++i)
+      for (int c = 0; c < 3; ++c) {
+        rgb0[3 * i + c] = a.rgba[4 * i + c];
+        rgb1[3 * i + c] = b.rgba[4 * i + c];
+      }
+    p0 = rgb0.data();
+    p1 = rgb1.data();
+  }
   map->resize(static_cast<size_t>(a.w) * a.h);
-  if (!gb200_butteraugli_diffmap(l0.data(), l1.data(), a.w, a.h, device, map->data(), value)) {
+  if (!gb200_butteraugli_diffmap_srgb(p0, p1, a.w, a.h, channels, device, map->data(), value)) {
     fprintf(stderr, "Butteraugli comparison failed\n");
     if (*gb200_last_error()) fprintf(stderr, "%s\n", gb200_last_error());
     return false;
@@ -157,23 +144,14 @@ int main(int argc, char** argv) {
   }
   int device = 0;
   if (const char* e = getenv("GUETZLI_B200_DEVICE")) device = atoi(e);
-  std::vector<float> map, map_white;
+  std::vector<float> map;
   double value = 0;
-  if (!Compare(a, b, 0, device, &map, &value)) return 1;
-  const std::vector<float>* best = &map;
-  if (a.has_alpha) {  // also over a white background; the worse of the two counts
-    double value_white = 0;
-    if (!Compare(a, b, 255, device, &map_white, &value_white)) return 1;
-    if (value_white > value) {
-      value = value_white;
-      best = &map_white;
-    }
-  }
+  if (!Compare(a, b, device, &map, &value)) return 1;
   printf("%lf\n", value);
   if (argc == 4) {
     const double good = FuzzyInverse(1.5), bad = FuzzyInverse(0.5);
-    std::vector<uint8_t> rgb(3 * best->size());
-    for (size_t i = 0; i < best->size(); ++i) ScoreToRgb((*best)[i], good, bad, &rgb[3 * i]);
+    std::vector<uint8_t> rgb(3 * map.size());
+    for (size_t i = 0; i < map.size(); ++i) ScoreToRgb(map[i], good, bad, &rgb[3 * i]);
     FILE* f = fopen(argv[3], "wb");
     if (f == NULL) {
       fprintf(stderr, "Cannot open %s\n", argv[3]);

@@ -266,6 +266,129 @@ void Butteraugli::compare_many(const float* rgb1, int n, float* diffmap, float* 
   }
 }
 
+// ---- 8-bit sRGB input (butteraugli.h) ----
+namespace {
+// The converted planes are handed to the float entries as device memory.  The CPU port has no device
+// memory (its dev_alloc is host memory, and its device entries refuse), so there they go in as host
+// memory.
+#if defined(GB200_HOSTSIM)
+constexpr bool kScratchOnDevice = false;
+#else
+constexpr bool kScratchOnDevice = true;
+#endif
+
+void check_channels(int channels) {
+  if (channels != 3 && channels != 4)
+    throw std::runtime_error("butteraugli: channels = " + std::to_string(channels) +
+                             ", 8-bit images must have 3 (RGB) or 4 (RGBA)");
+}
+}  // namespace
+
+void Butteraugli::srgb_alloc(int per_slot) {
+  if (srgb_lin_ != nullptr) return;
+  // the pair batch builds no tables of its own where its pairs go through metrics of their own; the
+  // conversion needs only the sRGB table
+  if (t_.srgb_lin == nullptr) t_.srgb_lin = upload_srgb_lin(s_, &owned_, nullptr);
+  const size_t px = static_cast<size_t>(g_.w) * g_.h, imgs = static_cast<size_t>(per_slot) * capacity_;
+  srgb_u8_ = static_cast<uint8_t*>(dev_alloc(4 * px * imgs));
+  owned_.push_back(srgb_u8_);
+  srgb_lin_ = static_cast<float*>(dev_alloc(sizeof(float) * 3 * px * imgs));
+  owned_.push_back(srgb_lin_);
+  for (float*& dm : srgb_dm_) {
+    dm = static_cast<float*>(dev_alloc(sizeof(float) * px * capacity_));
+    owned_.push_back(dm);
+  }
+}
+
+template <class Score>
+void Butteraugli::srgb_backgrounds(int n, int channels, int only, float* diffmap, float* maxima, bool device,
+                                   const Score& score) {
+  const size_t px = static_cast<size_t>(g_.w) * g_.h;
+  const bool both = channels == 4 && only < 0;
+  float* dm = diffmap == nullptr ? nullptr : device ? diffmap : srgb_dm_[0];
+  score(only < 0 ? 0 : only, dm, maxima);
+  if (both) {
+    std::vector<float> white(n);
+    score(255, dm != nullptr ? srgb_dm_[1] : nullptr, white.data());
+    for (int i = 0; i < n; ++i) {
+      if (!(white[i] > maxima[i])) continue;  // a tie keeps black (butteraugli_main.cc:414)
+      maxima[i] = white[i];
+      if (dm != nullptr) d2d(dm + i * px, srgb_dm_[1] + i * px, sizeof(float) * px, s_);
+    }
+  }
+  if (dm != nullptr && !device) {
+    d2h(diffmap, dm, sizeof(float) * px * n, s_);
+  } else if (both) {
+    stream_sync(s_);  // the white diffmaps copied into the caller's memory
+  }
+}
+
+void Butteraugli::analyse_original_srgb(const uint8_t* img0, int channels, int background) {
+  check_channels(channels);
+  bind();
+  const size_t bytes = static_cast<size_t>(g_.w) * g_.h * channels;
+  uint8_t* u8 = static_cast<uint8_t*>(dev_alloc(bytes));
+  try {
+    h2d(u8, img0, bytes, s_);
+    srgb_to_linear(u8, 1, channels, background, lin_, g_.pitch);
+    analyse_original();
+    stream_sync(s_);
+  } catch (...) {
+    dev_free(u8);
+    throw;
+  }
+  dev_free(u8);
+}
+
+void Butteraugli::compare_batch_srgb(const uint8_t* img0, const uint8_t* img1, int n, int channels, float* diffmap,
+                                     float* maxima, bool device, Stream caller, int background) {
+  if (n < 1 || n > capacity_) throw std::runtime_error("butteraugli batch: n must be in 1..capacity");
+  check_channels(channels);
+  if (background != -1 && background != 0 && background != 255)
+    throw std::logic_error("butteraugli batch: the background must be 0 or 255");
+  bind();
+  srgb_alloc(2);
+  const size_t bytes = static_cast<size_t>(g_.w) * g_.h * channels * n;
+  const size_t half = static_cast<size_t>(g_.w) * g_.h * capacity_;  // images of one side
+  const uint8_t* in0 = img0;
+  const uint8_t* in1 = img1;
+  if (device) {
+    stream_wait(s_, caller);
+  } else {  // one upload of each side
+    h2d(srgb_u8_, img0, bytes, s_);
+    h2d(srgb_u8_ + 4 * half, img1, bytes, s_);
+    in0 = srgb_u8_;
+    in1 = srgb_u8_ + 4 * half;
+  }
+  float* lin0 = srgb_lin_;
+  float* lin1 = srgb_lin_ + 3 * half;
+  srgb_backgrounds(n, channels, background, diffmap, maxima, device, [&](int bg, float* dm, float* m) {
+    srgb_to_linear(in0, n, channels, bg, lin0, g_.w);
+    srgb_to_linear(in1, n, channels, bg, lin1, g_.w);
+    compare_batch(lin0, lin1, n, dm, m, kScratchOnDevice, s_);
+  });
+}
+
+void Butteraugli::compare_many_srgb(const uint8_t* img1, int n, int channels, Butteraugli* white, float* diffmap,
+                                    float* maxima, bool device, Stream caller) {
+  if (n < 1 || n > capacity_) throw std::runtime_error("butteraugli comparator: n must be in 1..capacity");
+  check_channels(channels);
+  if (channels == 4 && white == nullptr) throw std::logic_error("butteraugli comparator: RGBA needs the original over white");
+  bind();
+  srgb_alloc(1);
+  const uint8_t* in = img1;
+  if (device) {
+    stream_wait(s_, caller);
+  } else {
+    h2d(srgb_u8_, img1, static_cast<size_t>(g_.w) * g_.h * channels * n, s_);
+    in = srgb_u8_;
+  }
+  srgb_backgrounds(n, channels, -1, diffmap, maxima, device, [&](int background, float* dm, float* m) {
+    srgb_to_linear(in, n, channels, background, srgb_lin_, g_.w);
+    (background == 0 ? this : white)->compare_many(srgb_lin_, n, dm, m, kScratchOnDevice, s_);
+  });
+}
+
 void Butteraugli::adaptive_quantization(const float* linear_rgb, float* quant) {
   bind();
   r_.upload_planes(linear_rgb, lin_, 3);

@@ -178,6 +178,25 @@ class Butteraugli {
   // rgb1 packed [n][3][h][w]; outputs, device and caller as in compare_batch.  Slots kCandidates;
   // with capacity 1, the staged chain or the CPU port the candidates go one by one through slot 0.
   void compare_many(const float* rgb1, int n, float* diffmap, float* maxima, bool device, Stream caller);
+
+  // 8-bit sRGB input, as the stand-alone `butteraugli` tool reads it (b/butteraugli_main.cc:239-281,
+  // :390-419): images interleaved [n][h][w][channels], channels 3 (RGB) or 4 (RGBA).  They are
+  // converted to linear planes on the device (SrgbToLinear) and scored by the float entries above from
+  // device memory (DESIGN.md §4).  RGBA is laid over black and scored, then over white and scored; where
+  // white scores strictly higher, its score and its diffmap replace black's.
+  //
+  // The original of a comparator, in host memory, laid over `background` (0 or 255), into lin and
+  // analysed there (analyse_original).
+  void analyse_original_srgb(const uint8_t* img0, int channels, int background);
+  // compare_batch on 8-bit pairs; outputs, device and caller as there.  background 0 or 255: the pairs
+  // laid over that background only, with no choice between backgrounds (gb200_butteraugli_diffmap_srgb
+  // makes the choice itself, on padded images after it has cropped them).
+  void compare_batch_srgb(const uint8_t* img0, const uint8_t* img1, int n, int channels, float* diffmap,
+                          float* maxima, bool device, Stream caller, int background = -1);
+  // compare_many on 8-bit candidates against the original analyse_original_srgb() laid over black;
+  // for channels 4, `white` is the metric of the same shape whose original it laid over white.
+  void compare_many_srgb(const uint8_t* img1, int n, int channels, Butteraugli* white, float* diffmap,
+                         float* maxima, bool device, Stream caller);
   // ButteraugliComparator::Mask (b/butteraugli.cc:793) of the original at every pixel, on the
   // host: mask, mask_dc [3][h][w].  Leaves the resident PsychoImage as it is.
   void mask(float* mask, float* mask_dc);
@@ -204,6 +223,16 @@ class Butteraugli {
   void mask_activity(const float* xy);
   // Mask(xy, xy) at every pixel -> mask_ (mask [3], then mask_dc [3], allocated on first use)
   void mask_planes(const float* xy);
+  // n 8-bit images (memory of this device) over `background` -> dst [n][3][h][pitch]
+  void srgb_to_linear(const uint8_t* src, int n, int channels, int background, float* dst, int pitch);
+  // the 8-bit entries' buffers, for `per_slot` images in each of the capacity slots (first use)
+  void srgb_alloc(int per_slot);
+  // n images laid over black by score(background, diffmap, maxima), for RGBA over white as well, and
+  // the winner of each into diffmap / maxima (outputs as in compare_batch); only >= 0: that background
+  // alone
+  template <class Score>
+  void srgb_backgrounds(int n, int channels, int only, float* diffmap, float* maxima, bool device,
+                        const Score& score);
 
   // TMA-staged fused Compare chain (fused_kernels.cuh; CUDA build only)
   struct Fused;
@@ -232,7 +261,7 @@ class Butteraugli {
   int capacity_ = 1;
   int kslot_ = 0;
   bool one_original_ = false;  // Slots::kCandidates with capacity > 1
-  Tables t_;
+  Tables t_ = Tables();  // null until built: the pair batch's staged chain builds none
   HostTables ht_;
   MaltaParams malta_[6];
   double asym_w0_, asym_w1_;
@@ -262,6 +291,11 @@ class Butteraugli {
   float* block_max_ = nullptr;      // [capacity][nblocks]
   unsigned int* d_gmax_ = nullptr;  // [capacity] global maximum of the distmap (float bits)
   float* partial_ = nullptr;        // [1024]
+
+  // the 8-bit entries' buffers (srgb_alloc), per_slot images in each slot, packed
+  uint8_t* srgb_u8_ = nullptr;                 // [per_slot][capacity][h][w][4] host input, uploaded
+  float* srgb_lin_ = nullptr;                  // [per_slot][capacity][3][h][w] converted planes
+  float* srgb_dm_[2] = {nullptr, nullptr};     // [capacity][h][w] diffmaps: host output; over white
 };
 
 #if defined(__CUDACC__) && !defined(GB200_HOSTSIM)

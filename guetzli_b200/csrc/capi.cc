@@ -58,6 +58,10 @@ struct gb200_image {
 
 struct gb200_butteraugli_comparator {
   gb200::Butteraugli* ba;
+  // made from 8-bit images: their channels (3 or 4), and for RGBA the original laid over white (ba
+  // holds it laid over black); 0 and null when made from float planes
+  int channels = 0;
+  gb200::Butteraugli* white = nullptr;
 };
 
 struct gb200_butteraugli_batch {
@@ -65,6 +69,14 @@ struct gb200_butteraugli_batch {
 };
 
 namespace {
+// A comparator made from float planes takes float images, one made from 8-bit images 8-bit images.
+bool comparator_takes(const gb200_butteraugli_comparator* c, bool srgb) {
+  if ((c->channels != 0) == srgb) return true;
+  g_err = srgb ? "butteraugli comparator: made from float planes, it takes float images, not 8-bit ones"
+               : "butteraugli comparator: made from 8-bit images, it takes 8-bit images, not float planes";
+  return false;
+}
+
 // device pointers of a *_device entry: memory of `device`, else a message naming the argument
 void check_device_pointers(const char* who, int device, const void* const* ptrs, const char* const* what, int n) {
   for (int i = 0; i < n; ++i) {
@@ -239,7 +251,10 @@ gb200_butteraugli_comparator* gb200_butteraugli_comparator_create(const float* r
 
 void gb200_butteraugli_comparator_destroy(gb200_butteraugli_comparator* c) {
   if (!c) return;
-  guarded([&]() { delete c->ba; });
+  guarded([&]() {
+    delete c->ba;
+    delete c->white;
+  });
   delete c;
 }
 
@@ -250,6 +265,7 @@ int gb200_butteraugli_comparator_diffmap(gb200_butteraugli_comparator* c, const 
     g_err = "butteraugli comparator: no comparator or no image";
     return 0;
   }
+  if (!comparator_takes(c, false)) return 0;
   return guarded([&]() {
     const float m = c->ba->compare_linear(rgb1);
     if (diffmap) c->ba->download_distmap(diffmap);
@@ -264,6 +280,7 @@ int gb200_butteraugli_comparator_diffmap_device(gb200_butteraugli_comparator* c,
     g_err = "butteraugli comparator: no comparator or no image";
     return 0;
   }
+  if (!comparator_takes(c, false)) return 0;
   return guarded([&]() {
     c->ba->bind();
     const void* ptrs[2] = {rgb1_dev, diffmap_dev};
@@ -307,6 +324,7 @@ int comparator_diffmap_batch(gb200_butteraugli_comparator* c, const float* rgb1,
     g_err = "butteraugli comparator: no comparator or no images";
     return 0;
   }
+  if (!comparator_takes(c, false)) return 0;
   if (n < 1 || n > c->ba->capacity()) {
     g_err = "butteraugli comparator: n = " + std::to_string(n) + " images, the comparator takes 1.." +
             std::to_string(c->ba->capacity());
@@ -406,10 +424,189 @@ int gb200_butteraugli_batch_diffmap_device(gb200_butteraugli_batch* b, const flo
   return batch_diffmap(b, rgb0_dev, rgb1_dev, n, diffmap_dev, score, true, stream);
 }
 
+// ---- 8-bit sRGB input: the stand-alone tool's conversion and alpha rule (butteraugli_main.cc:239-281,
+// :390-419) in front of the float entries above ----
+namespace {
+bool channels_ok(const char* who, int channels) {
+  if (channels == 3 || channels == 4) return true;
+  g_err = std::string(who) + ": channels = " + std::to_string(channels) + ", 8-bit images must have 3 (RGB) or 4 (RGBA)";
+  return false;
+}
+}  // namespace
+
+int gb200_butteraugli_diffmap_srgb(const uint8_t* img0, const uint8_t* img1, int w, int h, int channels, int device,
+                                   float* diffmap, double* score) {
+  if (img0 == nullptr || img1 == nullptr || w < 1 || h < 1) {
+    g_err = "butteraugli: no image";
+    return 0;
+  }
+  if (!channels_ok("butteraugli", channels)) return 0;
+  return guarded([&]() {
+    // below 8 pixels in a dimension, edge-replicated to 8 as gb200_butteraugli_diffmap pads its planes;
+    // the conversion is per pixel, so replicating bytes first gives the same planes
+    const int kMin = 8;
+    const int xb = w < kMin ? (kMin - w) / 2 : 0, yb = h < kMin ? (kMin - h) / 2 : 0;
+    const int ws = std::max(w, kMin), hs = std::max(h, kMin);
+    const size_t C = channels;
+    std::vector<uint8_t> s0, s1;
+    const uint8_t* p0 = img0;
+    const uint8_t* p1 = img1;
+    if (ws != w || hs != h) {
+      s0.resize(C * ws * hs);
+      s1.resize(s0.size());
+      for (int y = 0; y < hs; ++y)
+        for (int x = 0; x < ws; ++x) {
+          const int x2 = std::min(w - 1, std::max(0, x - xb)), y2 = std::min(h - 1, std::max(0, y - yb));
+          const size_t d = (static_cast<size_t>(y) * ws + x) * C, s = (static_cast<size_t>(y2) * w + x2) * C;
+          memcpy(&s0[d], img0 + s, C);
+          memcpy(&s1[d], img1 + s, C);
+        }
+      p0 = s0.data();
+      p1 = s1.data();
+    }
+    gb200::Butteraugli ba(ws, hs, 1, device);  // a pair batch of one
+    std::vector<float> dm(static_cast<size_t>(ws) * hs);
+    // Each background is scored as ButteraugliInterface scores it, padded and then cropped, and the
+    // tool chooses on those cropped scores (butteraugli_main.cc:390-419).  Padding can hold the maximum
+    // of a padded diffmap, so the choice cannot be made on the padded maxima.
+    float best = 0.0f;
+    for (int k = 0; k < (channels == 4 ? 2 : 1); ++k) {
+      float m = 0.0f;
+      ba.compare_batch_srgb(p0, p1, 1, channels, dm.data(), &m, false, 0, k == 0 ? 0 : 255);
+      if (ws != w || hs != h) {
+        m = 0.0f;
+        for (int y = 0; y < h; ++y)
+          for (int x = 0; x < w; ++x) m = std::max(m, dm[static_cast<size_t>(y + yb) * ws + x + xb]);
+      }
+      if (k == 1 && !(m > best)) continue;  // a tie keeps black (butteraugli_main.cc:414)
+      best = m;
+      if (diffmap)
+        for (int y = 0; y < h; ++y)
+          memcpy(diffmap + static_cast<size_t>(y) * w, &dm[static_cast<size_t>(y + yb) * ws + xb], sizeof(float) * w);
+    }
+    if (score) *score = best;
+  });
+}
+
+namespace {
+int batch_diffmap_srgb(gb200_butteraugli_batch* b, const uint8_t* img0, const uint8_t* img1, int n, int channels,
+                       float* diffmap, double* score, bool device, void* stream) {
+  if (b == nullptr || img0 == nullptr || img1 == nullptr) {
+    g_err = "butteraugli batch: no batch or no images";
+    return 0;
+  }
+  if (n < 1 || n > b->ba->capacity()) {
+    g_err = "butteraugli batch: n = " + std::to_string(n) + " pairs, the batch takes 1.." +
+            std::to_string(b->ba->capacity());
+    return 0;
+  }
+  if (!channels_ok("butteraugli batch", channels)) return 0;
+  return guarded([&]() {
+    b->ba->bind();
+    gb200::Stream caller = 0;
+    if (device) {
+      const void* ptrs[3] = {img0, img1, diffmap};
+      const char* what[3] = {"img0", "img1", "diffmap"};
+      check_device_pointers("butteraugli batch", b->ba->device(), ptrs, what, 3);
+#if !defined(GB200_HOSTSIM)
+      caller = static_cast<gb200::Stream>(stream);
+#endif
+    }
+    (void)stream;
+    std::vector<float> m(n);
+    b->ba->compare_batch_srgb(img0, img1, n, channels, diffmap, m.data(), device, caller);
+    if (score)
+      for (int i = 0; i < n; ++i) score[i] = m[i];
+  });
+}
+
+int comparator_diffmap_srgb(gb200_butteraugli_comparator* c, const uint8_t* img1, int n, float* diffmap, double* score,
+                            bool device, void* stream) {
+  if (c == nullptr || img1 == nullptr) {
+    g_err = "butteraugli comparator: no comparator or no images";
+    return 0;
+  }
+  if (!comparator_takes(c, true)) return 0;
+  if (n < 1 || n > c->ba->capacity()) {
+    g_err = "butteraugli comparator: n = " + std::to_string(n) + " images, the comparator takes 1.." +
+            std::to_string(c->ba->capacity());
+    return 0;
+  }
+  return guarded([&]() {
+    c->ba->bind();
+    gb200::Stream caller = 0;
+    if (device) {
+      const void* ptrs[2] = {img1, diffmap};
+      const char* what[2] = {"img1", "diffmap"};
+      check_device_pointers("butteraugli comparator", c->ba->device(), ptrs, what, 2);
+#if !defined(GB200_HOSTSIM)
+      caller = static_cast<gb200::Stream>(stream);
+#endif
+    }
+    (void)stream;
+    std::vector<float> m(n);
+    c->ba->compare_many_srgb(img1, n, c->channels, c->white, diffmap, m.data(), device, caller);
+    if (score)
+      for (int i = 0; i < n; ++i) score[i] = m[i];
+  });
+}
+}  // namespace
+
+int gb200_butteraugli_batch_diffmap_srgb(gb200_butteraugli_batch* b, const uint8_t* img0, const uint8_t* img1, int n,
+                                         int channels, float* diffmap, double* score) {
+  return batch_diffmap_srgb(b, img0, img1, n, channels, diffmap, score, false, nullptr);
+}
+
+int gb200_butteraugli_batch_diffmap_srgb_device(gb200_butteraugli_batch* b, const uint8_t* img0_dev,
+                                                const uint8_t* img1_dev, int n, int channels, float* diffmap_dev,
+                                                double* score, void* stream) {
+  return batch_diffmap_srgb(b, img0_dev, img1_dev, n, channels, diffmap_dev, score, true, stream);
+}
+
+gb200_butteraugli_comparator* gb200_butteraugli_comparator_create_srgb(const uint8_t* img0, int w, int h, int channels,
+                                                                       int capacity, int device) {
+  gb200_butteraugli_comparator* c = nullptr;
+  if (!channels_ok("butteraugli comparator", channels)) return nullptr;
+  guarded([&]() {
+    if (img0 == nullptr) throw std::runtime_error("butteraugli comparator: no image");
+    if (w < 8 || h < 8 || w >= 65536 || h >= 65536)
+      throw std::runtime_error("butteraugli comparator: the image must be at least 8x8 (and below 65536)");
+    if (capacity < 1 || capacity > 16383)
+      throw std::runtime_error("butteraugli comparator: the capacity must be in 1..16383");
+    const gb200::Butteraugli::Slots kind = gb200::Butteraugli::Slots::kCandidates;
+    std::unique_ptr<gb200::Butteraugli> black(new gb200::Butteraugli(w, h, capacity, device, kind));
+    black->analyse_original_srgb(img0, channels, 0);
+    std::unique_ptr<gb200::Butteraugli> white;
+    if (channels == 4) {  // a second resident original, laid over white
+      white.reset(new gb200::Butteraugli(w, h, capacity, device, kind));
+      white->analyse_original_srgb(img0, channels, 255);
+    }
+    c = new gb200_butteraugli_comparator;
+    c->ba = black.release();
+    c->white = white.release();
+    c->channels = channels;
+  });
+  return c;
+}
+
+int gb200_butteraugli_comparator_diffmap_srgb(gb200_butteraugli_comparator* c, const uint8_t* img1, int n,
+                                              float* diffmap, double* score) {
+  return comparator_diffmap_srgb(c, img1, n, diffmap, score, false, nullptr);
+}
+
+int gb200_butteraugli_comparator_diffmap_srgb_device(gb200_butteraugli_comparator* c, const uint8_t* img1_dev, int n,
+                                                     float* diffmap_dev, double* score, void* stream) {
+  return comparator_diffmap_srgb(c, img1_dev, n, diffmap_dev, score, true, stream);
+}
+
 // ButteraugliComparator::Mask (b/butteraugli.cc:793)
 int gb200_butteraugli_comparator_mask(gb200_butteraugli_comparator* c, float* mask, float* mask_dc) {
   if (c == nullptr || mask == nullptr || mask_dc == nullptr) {
     g_err = "butteraugli comparator: no comparator or no output";
+    return 0;
+  }
+  if (c->channels == 4) {
+    g_err = "butteraugli comparator: an RGBA comparator has two originals (over black and over white), no one mask";
     return 0;
   }
   return guarded([&]() { c->ba->mask(mask, mask_dc); });

@@ -73,6 +73,35 @@ struct LinearizeRgb {
   }
 };
 
+// The stand-alone `butteraugli` tool's input (FromSrgbToLinear, b/butteraugli_main.cc:239-281): u8 sRGB
+// images interleaved [n][h][w][C] -> linear planes [n][3][h][pitch].  C = 4: the pixel is laid over
+// `background` in sRGB space first, in integers: alpha 255 keeps it, alpha 0 gives the background,
+// any other alpha (v a + background (255 - a) + 127) / 255.  lut: Tables::srgb_lin, which equals the
+// tool's table once both are rounded to float.  Launched over w x n*h.
+struct SrgbToLinear {
+  const uint8_t* src;
+  int C, background;
+  float* dst;
+  int w, h, pitch;
+  const float* lut;
+  GB_HD void operator()(int x, int yy) const {
+    const int i = yy / h, y = yy - i * h;
+    const uint8_t* p = src + (static_cast<size_t>(yy) * w + x) * C;
+    const int a = C == 4 ? p[3] : 255;
+    const size_t plane = static_cast<size_t>(h) * pitch;
+    float* o = dst + 3 * plane * i + static_cast<size_t>(y) * pitch + x;
+    for (int c = 0; c < 3; ++c) {
+      int v = p[c];
+      if (a == 0) {
+        v = background;
+      } else if (a != 255) {
+        v = (v * a + background * (255 - a) + 127) / 255;
+      }
+      o[c * plane] = lut[v];
+    }
+  }
+};
+
 // a8: ApplyGlobalQuantization on top of CopyFromJpegData with unit quant
 // (g/output_image.cc:211-243): cand = Quantize(orig, q[c][k]).
 struct QuantizeCoeffs {

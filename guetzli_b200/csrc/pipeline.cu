@@ -428,6 +428,17 @@ void Butteraugli::mask(float* mask, float* mask_dc) {
   r_.download_planes(mask_ + 3 * g_.plane, mask_dc, 3);
 }
 
+void Butteraugli::srgb_to_linear(const uint8_t* src, int n, int channels, int background, float* dst, int pitch) {
+  // a launch covers at most 65535 * 8 rows (launch_2d's grid y), so large batches go in parts
+  const int per = std::max(1, 65535 * 8 / g_.h);
+  const size_t in = static_cast<size_t>(g_.w) * g_.h * channels, out = static_cast<size_t>(3) * g_.h * pitch;
+  for (int i = 0; i < n; i += per) {
+    const int k = std::min(per, n - i);
+    launch_2d(s_, SrgbToLinear{src + i * in, channels, background, dst + i * out, g_.w, g_.h, pitch, t_.srgb_lin},
+              g_.w, k * g_.h, "srgb_to_linear");
+  }
+}
+
 void Butteraugli::blur(const float* in, float* out, int nplanes, int id) {
 #if defined(GB200_HOSTSIM)
   r_.px(BlurX{in, tmp_, t_.blur[id], g_}, "blur_x", nplanes);

@@ -119,11 +119,9 @@ float border_scale(const std::vector<float>& taps, float weight_no_border, float
 
 }  // namespace
 
-Tables build_tables(int w, int h, Stream s, std::vector<void*>* owned, HostTables* host) {
-  Tables t;
+const float* upload_srgb_lin(Stream s, std::vector<void*>* owned, HostTables* host) {
   HostTables local;
   HostTables& ht = host ? *host : local;
-
   // sRGB -> linear, gamma_correct.cc:23-33
   ht.srgb_lin_d.resize(256);
   ht.srgb_lin.resize(256);
@@ -132,7 +130,15 @@ Tables build_tables(int w, int h, Stream s, std::vector<void*>* owned, HostTable
     ht.srgb_lin_d[i] = v;
     ht.srgb_lin[i] = static_cast<float>(v);
   }
-  t.srgb_lin = upload(ht.srgb_lin, s, owned);
+  return upload(ht.srgb_lin, s, owned);
+}
+
+Tables build_tables(int w, int h, Stream s, std::vector<void*>* owned, HostTables* host) {
+  Tables t;
+  HostTables local;
+  HostTables& ht = host ? *host : local;
+
+  t.srgb_lin = upload_srgb_lin(s, owned, &ht);
 
   // YCbCr -> RGB, the libjpeg 16.16 fixed-point tables (color_transform.h:22-140)
   ht.cr_r.resize(256); ht.cb_b.resize(256); ht.cr_g.resize(256); ht.cb_g.resize(256);

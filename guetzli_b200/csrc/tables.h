@@ -80,6 +80,8 @@ std::vector<float> make_blur_taps(float sigma);
 // Builds all tables for a w x h image and uploads them. Returns the device
 // allocations in *owned so the caller can free them.
 Tables build_tables(int w, int h, Stream s, std::vector<void*>* owned, HostTables* host);
+// The sRGB table alone (Tables::srgb_lin), uploaded the same way.
+const float* upload_srgb_lin(Stream s, std::vector<void*>* owned, HostTables* host);
 
 const int* zigzag_to_natural();  // [64] JPEG zig-zag scan position -> natural index
 const int* natural_to_zigzag();  // [64] inverse

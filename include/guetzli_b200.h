@@ -153,6 +153,45 @@ int gb200_butteraugli_batch_diffmap_device(gb200_butteraugli_batch* b, const flo
                                            int n, float* diffmap_dev, double* score, void* stream);
 void gb200_butteraugli_batch_destroy(gb200_butteraugli_batch* b);
 
+/* ---- 8-bit sRGB images, scored as the stand-alone `butteraugli` tool scores them ----
+ * Images are interleaved uint8 [h][w][channels] (or [n][h][w][channels]), channels 3 (RGB) or 4 (RGBA),
+ * both images of a pair with the same channels.  Each is converted on the device as the tool converts
+ * it (FromSrgbToLinear, butteraugli_main.cc:239-281): sRGB bytes to linear 0..255 through the tool's
+ * table, and with alpha laid over a background in sRGB space first, in integers:
+ * (v a + bg (255 - a) + 127) / 255, alpha 255 keeping the pixel and 0 giving the background.  RGB is
+ * scored once.  RGBA is scored over black and over white (butteraugli_main.cc:390-419): the larger score
+ * and its diffmap are the result, black on a tie.  The float entries above then score the converted
+ * planes, so each result is bit for bit theirs on those planes.  Other channel counts are refused.
+ *
+ * The tool's whole comparison of one pair in host memory, any size from 1x1 (padded below 8 pixels as
+ * gb200_butteraugli_diffmap pads, each background cropped back before the two are compared, as the tool
+ * compares them); diffmap (may be NULL) receives [h][w], *score its maximum. */
+int gb200_butteraugli_diffmap_srgb(const uint8_t* img0, const uint8_t* img1, int w, int h, int channels, int device,
+                                   float* diffmap, double* score);
+/* gb200_butteraugli_batch_diffmap on 8-bit pairs: img0, img1 [n][h][w][channels] in host memory, uploaded
+ * once whatever the channels. */
+int gb200_butteraugli_batch_diffmap_srgb(gb200_butteraugli_batch* b, const uint8_t* img0, const uint8_t* img1, int n,
+                                         int channels, float* diffmap, double* score);
+/* The same with img0, img1 and diffmap (may be NULL) in device memory of the batch's device, read in
+ * place; stream as in gb200_butteraugli_comparator_diffmap_device. */
+int gb200_butteraugli_batch_diffmap_srgb_device(gb200_butteraugli_batch* b, const uint8_t* img0_dev,
+                                                const uint8_t* img1_dev, int n, int channels, float* diffmap_dev,
+                                                double* score, void* stream);
+/* A comparator (gb200_butteraugli_comparator_create_batch) whose original img0 [h][w][channels] is given
+ * in host memory, at least 8x8; 1 <= capacity <= 16383.  With channels 4 it keeps two resident
+ * originals, over black and over white.  It takes 8-bit candidates with its own channels only (the
+ * entries below); the float entries refuse it, and gb200_butteraugli_comparator_mask refuses an RGBA one. */
+gb200_butteraugli_comparator* gb200_butteraugli_comparator_create_srgb(const uint8_t* img0, int w, int h, int channels,
+                                                                       int capacity, int device);
+/* img1 [n][h][w][channels] in host memory, 1 <= n <= capacity; diffmap (may be NULL) [n][h][w], score
+ * (may be NULL) [n].  A comparator made from float planes refuses it. */
+int gb200_butteraugli_comparator_diffmap_srgb(gb200_butteraugli_comparator* c, const uint8_t* img1, int n,
+                                              float* diffmap, double* score);
+/* The same with img1 and diffmap (may be NULL) in device memory of the comparator's device, read in
+ * place; stream as in gb200_butteraugli_comparator_diffmap_device. */
+int gb200_butteraugli_comparator_diffmap_srgb_device(gb200_butteraugli_comparator* c, const uint8_t* img1_dev, int n,
+                                                     float* diffmap_dev, double* score, void* stream);
+
 /* butteraugli::ButteraugliAdaptiveQuantization (butteraugli.cc:1880): the Y plane of Mask(rgb, rgb),
  * [h][w] into quant.  rgb in host memory.  Fails below 16x16, where the reference returns false. */
 int gb200_butteraugli_adaptive_quantization(const float* rgb, int w, int h, int device, float* quant);

@@ -16,8 +16,15 @@ and two more score N distinct candidates against the one original per call:
   comparator_batch_cuda  one comparator of capacity N, candidates and diffmaps as CUDA torch tensors
   comparator_batch_host  the same comparator, candidates and diffmaps in host memory
 
-and the result gains ms per pair or candidate of the batched modes and MPix/s (scored pixels per
-second) of every mode.  Every call returns once its diffmaps are written, so a host clock around `--n` calls is the
+and four more take the same images as 8-bit sRGB (RGB, 3 bytes per pixel), converted on the device:
+
+  batch_srgb_cuda, batch_srgb_host                       ButteraugliBatch.diffmap_srgb
+  comparator_batch_srgb_cuda, comparator_batch_srgb_host  a comparator made by Comparator.from_srgb
+
+Their scores must equal their float twins' (scores_srgb_equal_float).  The result gains ms per pair or
+candidate of the batched modes, MPix/s (scored pixels per second) of every mode, and the device memory
+the batch and the batched comparators (RGB, and RGBA with its two originals) hold after creation and after
+their first 8-bit call (MiB, from torch.cuda.mem_get_info after gb200_trim_memory).  Every call returns once its diffmaps are written, so a host clock around `--n` calls is the
 time of the work.  The modes run in turn for `--rounds` rounds (the spread between rounds is part of the
 result), after `--warmup` untimed calls each.  The card's name and power limit are read in the
 same run (nvidia-smi, read-only queries).  Prints one JSON line; --out also writes it to a file.
@@ -93,21 +100,62 @@ def main():
 
     modes = {"pairwise": pairwise, "comparator_host": comparator_host, "comparator_cuda": comparator_cuda}
     per_call = {m: 1 for m in modes}
+    memory = {}
     if args.batch > 0:
         nb = args.batch
-        bpairs = [(linear(synth.gradnoise(h, w, 1000 + i)),
-                   linear(np.clip(synth.gradnoise(h, w, 1000 + i).astype(int) + synth.noise(h, w, 3000 + i) % 7 - 3,
-                                  0, 255).astype(np.uint8))) for i in range(nb)]
-        b0 = np.stack([p[0] for p in bpairs])
-        b1 = np.stack([p[1] for p in bpairs])
+        u0 = np.stack([synth.gradnoise(h, w, 1000 + i) for i in range(nb)])
+        u1 = np.stack([np.clip(synth.gradnoise(h, w, 1000 + i).astype(int) + synth.noise(h, w, 3000 + i) % 7 - 3,
+                               0, 255).astype(np.uint8) for i in range(nb)])
+        b0 = np.stack([linear(x) for x in u0])
+        b1 = np.stack([linear(x) for x in u1])
         b0_dev, b1_dev = torch.from_numpy(b0).to(dev), torch.from_numpy(b1).to(dev)
+        u0_dev, u1_dev = torch.from_numpy(u0).to(dev), torch.from_numpy(u1).to(dev)
+        uc = np.stack([np.clip(base + synth.noise(h, w, 5000 + k) % 7 - 3, 0, 255).astype(np.uint8) for k in range(nb)])
+        c1 = np.stack([linear(x) for x in uc])
+        c1_dev, uc_dev = torch.from_numpy(c1).to(dev), torch.from_numpy(uc).to(dev)
         torch.cuda.synchronize(dev)
+
+        def free_mib():
+            lib.gb200_trim_memory()
+            torch.cuda.synchronize(dev)
+            return torch.cuda.mem_get_info(dev)[0] / 2**20
+
+        f0 = free_mib()
         batch = gb.ButteraugliBatch(h, w, nb, device=args.device)
-        c1 = np.stack([linear(np.clip(base + synth.noise(h, w, 5000 + k) % 7 - 3, 0, 255).astype(np.uint8))
-                       for k in range(nb)])
-        c1_dev = torch.from_numpy(c1).to(dev)
-        torch.cuda.synchronize(dev)
+        f1 = free_mib()
+        batch.diffmap_srgb(u0, u1)
+        f2 = free_mib()
         cmpb = gb.Comparator(orig, device=args.device, capacity=nb)
+        f3 = free_mib()
+        cmps = gb.Comparator.from_srgb(base.astype(np.uint8), device=args.device, capacity=nb)
+        f4 = free_mib()
+        cmps.diffmap(uc)
+        f5 = free_mib()
+        # an RGBA comparator (two resident originals), measured and freed again before the timed modes
+        alpha = (synth.noise(h, w, 77)[..., :1] | 1).astype(np.uint8)
+        cmpa = gb.Comparator.from_srgb(np.concatenate([base.astype(np.uint8), alpha], axis=2), device=args.device,
+                                       capacity=nb)
+        f6 = free_mib()
+        cmpa.diffmap(np.concatenate([uc, np.broadcast_to(alpha, uc.shape[:3] + (1,))], axis=3))
+        f7 = free_mib()
+        cmpa.close()
+        memory = {"batch_mib": round(f0 - f1, 1), "batch_srgb_buffers_mib": round(f1 - f2, 1),
+                  "comparator_batch_mib": round(f2 - f3, 1), "comparator_batch_srgb_mib": round(f3 - f4, 1),
+                  "comparator_batch_srgb_buffers_mib": round(f4 - f5, 1),
+                  "comparator_batch_srgba_mib": round(f5 - f6, 1),
+                  "comparator_batch_srgba_buffers_mib": round(f6 - f7, 1)}
+
+        def batch_srgb_cuda(i):
+            return batch.diffmap_srgb(u0_dev, u1_dev)[1].tolist()
+
+        def batch_srgb_host(i):
+            return batch.diffmap_srgb(u0, u1)[1].tolist()
+
+        def comparator_batch_srgb_cuda(i):
+            return cmps.diffmap(uc_dev)[1].tolist()
+
+        def comparator_batch_srgb_host(i):
+            return cmps.diffmap(uc)[1].tolist()
 
         def comparator_batch_cuda(i):
             return cmpb.diffmap(c1_dev)[1].tolist()
@@ -121,9 +169,12 @@ def main():
         def batch_host(i):
             return batch.diffmap(b0, b1)[1].tolist()
 
-        modes.update(batch_cuda=batch_cuda, batch_host=batch_host, comparator_batch_cuda=comparator_batch_cuda,
-                     comparator_batch_host=comparator_batch_host)
-        per_call.update(batch_cuda=nb, batch_host=nb, comparator_batch_cuda=nb, comparator_batch_host=nb)
+        # each 8-bit mode right after its float twin
+        modes.update(batch_cuda=batch_cuda, batch_srgb_cuda=batch_srgb_cuda, batch_host=batch_host,
+                     batch_srgb_host=batch_srgb_host, comparator_batch_cuda=comparator_batch_cuda,
+                     comparator_batch_srgb_cuda=comparator_batch_srgb_cuda, comparator_batch_host=comparator_batch_host,
+                     comparator_batch_srgb_host=comparator_batch_srgb_host)
+        per_call.update({m: nb for m in modes if "batch" in m})
     scores = {}
     for name, f in modes.items():
         for i in range(args.warmup):
@@ -145,6 +196,7 @@ def main():
         # the last candidate of the batched comparator scores as it does alone
         cand_alone = cmp.diffmap(c1[-1])[1]
         cmpb.close()
+        cmps.close()
     cmp.close()
 
     def stats(v):
@@ -159,14 +211,17 @@ def main():
         # does alone
         alone = gb.api.butteraugli_diffmap(b0[0], b1[0], device=args.device)[1]
         result["batch"] = args.batch
-        result["ms_per_pair"] = {m: stats(ms[m]) for m in ("batch_cuda", "batch_host")}
-        result["ms_per_candidate"] = {m: stats(ms[m]) for m in ("comparator_batch_cuda", "comparator_batch_host")}
+        result["ms_per_pair"] = {m: stats(ms[m]) for m in ms if m.startswith("batch")}
+        result["ms_per_candidate"] = {m: stats(ms[m]) for m in ms if m.startswith("comparator_batch")}
         result["mpix_per_s"] = {m: round(w * h / 1e3 / statistics.median(v), 2) for m, v in ms.items()}
         result["batch_scores_consistent"] = (all(s == scores["batch_cuda"][0] for m in ("batch_cuda", "batch_host")
                                                  for s in scores[m]) and scores["batch_cuda"][0][0] == alone)
         cb = ("comparator_batch_cuda", "comparator_batch_host")
         result["comparator_batch_scores_consistent"] = (
             all(s == scores[cb[0]][0] for m in cb for s in scores[m]) and scores[cb[0]][0][-1] == cand_alone)
+        # the 8-bit modes score the converted planes of the float modes' images
+        result["scores_srgb_equal_float"] = all(scores[m] == scores[m.replace("_srgb", "")] for m in ms if "_srgb" in m)
+        result["device_memory"] = memory
     result.update(gpu_info(args.device))
     line = json.dumps(result)
     print(line)
