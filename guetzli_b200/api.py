@@ -110,6 +110,11 @@ def load_library(path=None):
                                                     C.c_void_p]
     lib.gb200_butteraugli_batch_diffmap_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
                                                            C.c_void_p, C.c_void_p]
+    lib.gb200_butteraugli_batch_diffmap_sizes.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                          C.c_int, C.c_void_p, C.c_void_p]
+    lib.gb200_butteraugli_batch_diffmap_sizes_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                                 C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                                                 C.c_void_p]
     lib.gb200_butteraugli_batch_destroy.argtypes = [C.c_void_p]
     lib.gb200_butteraugli_diffmap_srgb.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                                    C.c_void_p, P(C.c_double)]
@@ -541,6 +546,76 @@ class ButteraugliBatch:
         stream = torch.cuda.current_stream(t0.device).cuda_stream
         if not self.lib.gb200_butteraugli_batch_diffmap_device(self._h, t0.data_ptr(), t1.data_ptr(), n, dm.data_ptr(),
                                                                score.ctypes.data, stream):
+            raise RuntimeError(_err(self.lib))
+        return dm, score
+
+    def diffmap_sizes(self, rgb0s, rgb1s):
+        """Pairs of different sizes in one call: rgb0s, rgb1s equal-length sequences (1 <= n <= capacity) of
+        float32 [3][h_i][w_i] with 8 <= h_i <= h and 8 <= w_i <= w, pair i the same shape on both sides ->
+        (list of n diffmaps [h_i][w_i], scores float64 [n]), each pair bit for bit butteraugli_diffmap's.
+
+        The items are all numpy arrays (host memory) or all CUDA tensors, scored after the work queued on
+        the batch device's current torch stream; the diffmaps come back the same kind, CUDA tensors on the
+        batch's device.  As in diffmap(), a tensor on another device is refused by the C entry (RuntimeError,
+        naming the argument and its device); malformed arguments raise ValueError."""
+        rgb0s, rgb1s = list(rgb0s), list(rgb1s)
+        n = len(rgb0s)
+        if len(rgb1s) != n:
+            raise ValueError(f"rgb0s and rgb1s differ in length: {n} and {len(rgb1s)}")
+        if not 1 <= n <= self.capacity:
+            raise ValueError(f"the batch takes 1..{self.capacity} pairs, got {n}")
+        items = rgb0s + rgb1s
+        cuda = _is_torch_tensor(items[0]) and items[0].is_cuda
+        if cuda:
+            import torch
+            dev = torch.device("cuda", self.device)
+        ptrs, shapes = [], []
+        for k, x in enumerate(items):  # one pass: a call may hold hundreds of small pairs
+            name = ("rgb0s", "rgb1s")[k // n]
+            if isinstance(x, np.ndarray):
+                if cuda:
+                    raise ValueError("the images must all be CUDA tensors or all host arrays")
+                if x.dtype != np.float32:
+                    raise ValueError(f"{name}[{k % n}] must be float32, got {x.dtype}")
+                contiguous = x.flags.c_contiguous
+                ptrs.append(x.ctypes.data)
+            elif _is_torch_tensor(x) and x.is_cuda:
+                if not cuda:
+                    raise ValueError("the images must all be CUDA tensors or all host arrays")
+                if x.dtype != torch.float32:
+                    raise ValueError(f"{name}[{k % n}] must be float32, got {x.dtype}")
+                contiguous = x.is_contiguous()
+                ptrs.append(x.data_ptr())
+            else:
+                raise ValueError(f"{name}[{k % n}] must be a numpy array or a CUDA tensor, got {type(x).__name__}")
+            shape = tuple(x.shape)
+            if len(shape) != 3 or shape[0] != 3:
+                raise ValueError(f"{name}[{k % n}] must be planar [3][h][w], got shape {shape}")
+            if not contiguous:
+                raise ValueError(f"{name}[{k % n}] must be contiguous")
+            shapes.append(shape)
+        for i in range(n):
+            if shapes[i] != shapes[n + i]:
+                raise ValueError(f"pair {i} differs in shape: {shapes[i]} and {shapes[n + i]}")
+            _, h, w = shapes[i]
+            if not (8 <= h <= self.h and 8 <= w <= self.w):
+                raise ValueError(f"pair {i} is {h}x{w}; the batch takes 8x8 up to {self.h}x{self.w}")
+        ws = np.array([s[2] for s in shapes[:n]], dtype=np.int32)
+        hs = np.array([s[1] for s in shapes[:n]], dtype=np.int32)
+        P = C.c_void_p * n
+        p0, p1 = P(*ptrs[:n]), P(*ptrs[n:])
+        score = np.empty(n, dtype=np.float64)
+        if cuda:
+            dm = [torch.empty(s[1:], dtype=torch.float32, device=dev) for s in shapes[:n]]
+            stream = torch.cuda.current_stream(dev).cuda_stream
+            ok = self.lib.gb200_butteraugli_batch_diffmap_sizes_device(
+                self._h, ws.ctypes.data, hs.ctypes.data, p0, p1, n, P(*[t.data_ptr() for t in dm]), score.ctypes.data,
+                stream)
+        else:
+            dm = [np.empty(s[1:], dtype=np.float32) for s in shapes[:n]]
+            ok = self.lib.gb200_butteraugli_batch_diffmap_sizes(self._h, ws.ctypes.data, hs.ctypes.data, p0, p1, n,
+                                                                P(*[d.ctypes.data for d in dm]), score.ctypes.data)
+        if not ok:
             raise RuntimeError(_err(self.lib))
         return dm, score
 

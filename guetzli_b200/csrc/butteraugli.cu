@@ -13,6 +13,7 @@ namespace gb200 {
 
 #if defined(GB200_HOSTSIM)
 void Butteraugli::fused_sup0(int, int) {}
+void Butteraugli::mixed_release() {}
 #endif
 
 void Region::gather_blocks(void* dev_buf, size_t elem_bytes_per_block) const {
@@ -174,6 +175,7 @@ void Butteraugli::release() {
   }
   for (size_t i = 0; i < owned_.size(); ++i) dev_free(owned_[i]);
   owned_.clear();
+  mixed_release();
 #if !defined(GB200_HOSTSIM)
   delete fused_;
   fused_ = nullptr;
@@ -238,6 +240,41 @@ void Butteraugli::compare_batch(const float* rgb0, const float* rgb1, int n, flo
       maxima[i] = pair.compare_linear_device(rgb1 + i * img, dm, caller);
     } else {
       maxima[i] = pair.compare_linear(rgb1 + i * img);
+      if (dm != nullptr) pair.download_distmap(dm);
+    }
+  }
+}
+
+void Butteraugli::compare_batch_sizes(const int* w, const int* h, const float* const* rgb0, const float* const* rgb1,
+                                      int n, float* const* diffmap, float* maxima, bool device, Stream caller) {
+  if (n < 1 || n > capacity_) throw std::runtime_error("butteraugli batch: n must be in 1..capacity");
+  for (int i = 0; i < n; ++i)
+    if (w[i] < 8 || h[i] < 8 || w[i] > g_.w || h[i] > g_.h) throw std::runtime_error("butteraugli batch: pair size");
+  bind();
+#if !defined(GB200_HOSTSIM)
+  if (use_fused_) {
+    if (device) stream_wait(s_, caller);
+    fused_compare_sizes(w, h, rgb0, rgb1, n, diffmap, maxima, device);
+    return;
+  }
+#endif
+  // the staged chain and the CPU port: one single-image metric per pair, of the pair's size
+  for (int i = 0; i < n; ++i) {
+    const size_t img = static_cast<size_t>(3) * w[i] * h[i];
+    const float* p0 = rgb0[i];
+    std::vector<float> host0;
+    if (device) {  // the pair's original goes through host memory, after the caller's work
+      host0.resize(img);
+      d2h(host0.data(), p0, img * sizeof(float), caller);
+      p0 = host0.data();
+    }
+    Butteraugli pair(w[i], h[i], device_, nullptr);
+    pair.analyse_original(p0);
+    float* dm = diffmap != nullptr ? diffmap[i] : nullptr;
+    if (device) {
+      maxima[i] = pair.compare_linear_device(rgb1[i], dm, caller);
+    } else {
+      maxima[i] = pair.compare_linear(rgb1[i]);
       if (dm != nullptr) pair.download_distmap(dm);
     }
   }

@@ -22,6 +22,9 @@
 
 namespace gb200 {
 
+struct MixPass;  // one pass of a mixed-size call over the fused chain (pipeline.cu)
+struct MapReq;   // the tensor map argument of a fused launch (pipeline.cu)
+
 struct KernelStat {
   std::string name;
   long launches;
@@ -178,6 +181,13 @@ class Butteraugli {
   // rgb1 packed [n][3][h][w]; outputs, device and caller as in compare_batch.  Slots kCandidates;
   // with capacity 1, the staged chain or the CPU port the candidates go one by one through slot 0.
   void compare_many(const float* rgb1, int n, float* diffmap, float* maxima, bool device, Stream caller);
+  // compare_batch on n <= capacity pairs of different sizes: pair i is w[i] x h[i], each at least 8x8 and
+  // at most this batch's size, rgb0[i] / rgb1[i] packed [3][h[i]][w[i]], diffmap[i] [h[i]][w[i]] (diffmap
+  // itself may be null).  Outputs, device and caller as in compare_batch.  The fused chain scores all pairs
+  // in one pass of launches over (image, tile) work items, with tensor maps of each distinct size; the
+  // staged chain and the CPU port score each pair through a metric of its own size.
+  void compare_batch_sizes(const int* w, const int* h, const float* const* rgb0, const float* const* rgb1, int n,
+                           float* const* diffmap, float* maxima, bool device, Stream caller);
 
   // 8-bit sRGB input, as the stand-alone `butteraugli` tool reads it (b/butteraugli_main.cc:239-281,
   // :390-419): images interleaved [n][h][w][channels], channels 3 (RGB) or 4 (RGBA).  They are
@@ -249,6 +259,15 @@ class Butteraugli {
   void fused_sup0(int nimg, int kslot);
   // n pairs, or with rgb0 null n candidates against the resident original
   void fused_compare_batch(const float* rgb0, const float* rgb1, int n, float* diffmap, float* maxima);
+  // compare_batch_sizes on the fused chain; its buffers and tables (allocated on the first call, kept)
+  void fused_compare_sizes(const int* w, const int* h, const float* const* rgb0, const float* const* rgb1, int n,
+                           float* const* diffmap, float* maxima, bool device);
+  struct Mixed;
+  Mixed* mixed_ = nullptr;
+  MixPass* mix_ = nullptr;  // set while the launches of a mixed pass are queued
+  void mixed_release();
+  // the tensor map argument of a launch over plane group `base` (the batch's, or a mixed pass's per size)
+  MapReq maps(const float* base, int nplanes, int box_w, int box_h, int kslot);
   bool compare_pending_ = false;
   float compare_stash_ = 0.0f;
 
@@ -301,7 +320,7 @@ class Butteraugli {
 #if defined(__CUDACC__) && !defined(GB200_HOSTSIM)
 // Tensor maps of the plane groups and the Compare chain captured as a CUDA graph.
 struct Butteraugli::Fused {
-  typedef std::tuple<const float*, int, int, int> Key;  // base, planes, box w, box h
+  typedef std::tuple<const float*, int, int, int, int, int> Key;  // base, planes, box w, box h, w, h
   std::map<Key, CUtensorMap> maps;
   // the Compare chain as a CUDA graph: same kernels, same arguments every call (all buffers
   // live as long as the metric), one driver call instead of sixteen
@@ -311,12 +330,27 @@ struct Butteraugli::Fused {
   ~Fused() {
     if (compare_graph) cudaGraphExecDestroy(compare_graph);
   }
-  const CUtensorMap& map(const float* base, int nplanes, int box_w, int box_h, const Geom& g) {
-    const Key key(base, nplanes, box_w, box_h);
+  // the group's planes as a w x h image (w, h 0: the metric's size)
+  const CUtensorMap& map(const float* base, int nplanes, int box_w, int box_h, const Geom& g, int w = 0, int h = 0) {
+    if (w == 0) {
+      w = g.w;
+      h = g.h;
+    }
+    const Key key(base, nplanes, box_w, box_h, w, h);
     std::map<Key, CUtensorMap>::iterator it = maps.find(key);
     if (it == maps.end())
-      it = maps.insert(std::make_pair(key, make_plane_map(base, g.w, g.h, g.pitch, g.plane, nplanes, box_w, box_h))).first;
+      it = maps.insert(std::make_pair(key, make_plane_map(base, w, h, g.pitch, g.plane, nplanes, box_w, box_h))).first;
     return it->second;
+  }
+  // drops the maps of other sizes than the metric's (those of mixed-size calls)
+  void drop_other_sizes(const Geom& g) {
+    for (std::map<Key, CUtensorMap>::iterator it = maps.begin(); it != maps.end();) {
+      if (std::get<4>(it->first) != g.w || std::get<5>(it->first) != g.h) {
+        it = maps.erase(it);
+      } else {
+        ++it;
+      }
+    }
   }
   // a group of nplanes planes in each of the `capacity` arena slots of a batch, kslot planes apart
   // (kslot = 0: the group alone)

@@ -424,6 +424,68 @@ int gb200_butteraugli_batch_diffmap_device(gb200_butteraugli_batch* b, const flo
   return batch_diffmap(b, rgb0_dev, rgb1_dev, n, diffmap_dev, score, true, stream);
 }
 
+namespace {
+// pairs of different sizes: every argument is checked before anything is queued
+int batch_diffmap_sizes(gb200_butteraugli_batch* b, const int* w, const int* h, const float* const* rgb0,
+                        const float* const* rgb1, int n, float* const* diffmap, double* score, bool device,
+                        void* stream) {
+  if (b == nullptr || w == nullptr || h == nullptr || rgb0 == nullptr || rgb1 == nullptr) {
+    g_err = "butteraugli batch: no batch, no sizes or no images";
+    return 0;
+  }
+  if (n < 1 || n > b->ba->capacity()) {
+    g_err = "butteraugli batch: n = " + std::to_string(n) + " pairs, the batch takes 1.." +
+            std::to_string(b->ba->capacity());
+    return 0;
+  }
+  const int bw = b->ba->region().g.w, bh = b->ba->region().g.h;
+  for (int i = 0; i < n; ++i) {
+    if (w[i] < 8 || h[i] < 8 || w[i] > bw || h[i] > bh) {
+      g_err = "butteraugli batch: pair " + std::to_string(i) + " is " + std::to_string(w[i]) + "x" +
+              std::to_string(h[i]) + ", the batch takes 8x8 up to " + std::to_string(bw) + "x" + std::to_string(bh);
+      return 0;
+    }
+    if (rgb0[i] == nullptr || rgb1[i] == nullptr || (diffmap != nullptr && diffmap[i] == nullptr)) {
+      g_err = "butteraugli batch: pair " + std::to_string(i) + " has a null image or diffmap pointer";
+      return 0;
+    }
+  }
+  return guarded([&]() {
+    b->ba->bind();
+    gb200::Stream caller = 0;
+    if (device) {
+      for (int i = 0; i < n; ++i) {
+        const void* ptrs[3] = {rgb0[i], rgb1[i], diffmap != nullptr ? diffmap[i] : nullptr};
+        const std::string k = "[" + std::to_string(i) + "]";
+        const std::string names[3] = {"rgb0" + k, "rgb1" + k, "diffmap" + k};
+        const char* what[3] = {names[0].c_str(), names[1].c_str(), names[2].c_str()};
+        check_device_pointers("butteraugli batch", b->ba->device(), ptrs, what, 3);
+      }
+#if !defined(GB200_HOSTSIM)
+      caller = static_cast<gb200::Stream>(stream);
+#endif
+    }
+    (void)stream;
+    std::vector<float> m(n);
+    b->ba->compare_batch_sizes(w, h, rgb0, rgb1, n, diffmap, m.data(), device, caller);
+    if (score)
+      for (int i = 0; i < n; ++i) score[i] = m[i];
+  });
+}
+}  // namespace
+
+int gb200_butteraugli_batch_diffmap_sizes(gb200_butteraugli_batch* b, const int* w, const int* h,
+                                          const float* const* rgb0, const float* const* rgb1, int n,
+                                          float* const* diffmap, double* score) {
+  return batch_diffmap_sizes(b, w, h, rgb0, rgb1, n, diffmap, score, false, nullptr);
+}
+
+int gb200_butteraugli_batch_diffmap_sizes_device(gb200_butteraugli_batch* b, const int* w, const int* h,
+                                                 const float* const* rgb0_dev, const float* const* rgb1_dev, int n,
+                                                 float* const* diffmap_dev, double* score, void* stream) {
+  return batch_diffmap_sizes(b, w, h, rgb0_dev, rgb1_dev, n, diffmap_dev, score, true, stream);
+}
+
 // ---- 8-bit sRGB input: the stand-alone tool's conversion and alpha rule (butteraugli_main.cc:239-281,
 // :390-419) in front of the float entries above ----
 namespace {

@@ -41,6 +41,24 @@ struct BlurK {
   float raw[2 * R + 1];  // raw taps: border rule
 };
 
+// Mixed-size launches (kernel template argument B = 2): the images of a pass have sizes of their own,
+// each at most the batch's, in arena slots n0 .. n0 + m - 1 at the batch's pitch and plane size.
+// The grid is one-dimensional over (image, tile) work items: image j owns items
+// [tile0[j], tile0[j + 1]), its tiles in x-major, then y, then single-image z order.
+#define GB_MIX_SHAPES 16  // distinct sizes per pass: tensor maps of each in the kernel parameters
+struct MixImage {
+  int w, h;
+  int shape;   // index of its tensor maps in the pass's map sets
+  int sx, sy;  // offsets of its border scales (x, y) in the pass's scale table of a blur
+  int seg;     // rows of a rolling-blur segment (launch_roll's rule for h rows)
+  int pad[2];  // 32 bytes
+};
+struct MixGeom {
+  const MixImage* img;  // [m]
+  const int* tile0;     // [m + 1] first work item of each image, for the launch's tile shape
+  int m, n0;
+};
+
 struct PlaneGeom {
   int w, h, pitch;
   size_t plane;   // floats per plane
@@ -50,15 +68,82 @@ struct PlaneGeom {
   // and every TMA plane coordinate by n * kslot.  The grid's z is n * zimg + (the single-image z).
   // The original's planes (ps0, sup0) move by kslot0 planes per image instead: kslot0 = kslot
   // when every image has its own original, 0 when all images are scored against one.
-  // Single-image instantiations (B = false) read none of these fields.
+  // Single-image instantiations (B = 0) read none of these fields.
   int kslot, zimg, kslot0;
 };
+// the geometry argument of a mixed launch: the batch's, and the pass's images
+struct PlaneGeomMix : PlaneGeom {
+  MixGeom mix;
+};
+template <int B>
+struct GeomArg {
+  typedef PlaneGeom type;
+};
+template <>
+struct GeomArg<2> {
+  typedef PlaneGeomMix type;
+};
 
-// image index and single-image z of a block of a batched launch; (0, blockIdx.z) when B is false
-template <bool B>
+// image index and single-image z of a block of a batched launch; (0, blockIdx.z) when B is 0
+template <int B>
 __device__ __forceinline__ int batch_image(const PlaneGeom& g) {
   return B ? static_cast<int>(blockIdx.z) / g.zimg : 0;
 }
+
+// A block's work item: arena slot, tile column, tile row, single-image z.
+struct Item {
+  int n;
+  unsigned x, y, z;  // unsigned as blockIdx, so that B < 2 computes what it computed before
+};
+// the j with t0[j] <= v < t0[j + 1], for a non-decreasing t0[0 .. m] with t0[0] <= v < t0[m]
+__device__ __forceinline__ int mix_find(const int* t0, int m, int v) {
+  int lo = 0, hi = m;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (__ldg(t0 + mid) <= v) {
+      lo = mid;
+    } else {
+      hi = mid;
+    }
+  }
+  return lo;
+}
+// Mixed launch: the item of this block, with g's w, h and rows made the image's; th = 0 takes the
+// image's rolling-blur segment as the tile height.
+__device__ __forceinline__ MixImage mix_item(PlaneGeomMix& g, int tw, int th, Item& it) {
+  const int lin = blockIdx.x;
+  const int* t0 = g.mix.tile0;
+  const int lo = mix_find(t0, g.mix.m, lin);
+  const MixImage im = g.mix.img[lo];
+  const int tx = (im.w + tw - 1) / tw, tyh = th ? th : im.seg, ty = (im.h + tyh - 1) / tyh;
+  int local = lin - __ldg(t0 + lo);
+  it.n = g.mix.n0 + lo;
+  it.x = local % tx;
+  local /= tx;
+  it.y = local % ty;
+  it.z = local / ty;
+  g.w = im.w;
+  g.h = im.h;
+  g.y0 = 0;
+  g.y_end = im.h;
+  return im;
+}
+
+// Tensor maps of a launch: one (B < 2), or one per distinct size of a mixed pass, with that size's
+// true dims so that the TMA unit zero-fills at each image's own border.
+struct MixMaps {
+  CUtensorMap m[GB_MIX_SHAPES];
+};
+template <int B>
+struct MapArg {
+  typedef CUtensorMap type;
+};
+template <>
+struct MapArg<2> {
+  typedef MixMaps type;
+};
+__device__ __forceinline__ const CUtensorMap* map_of(const CUtensorMap& m, int) { return &m; }
+__device__ __forceinline__ const CUtensorMap* map_of(const MixMaps& m, int shape) { return &m.m[shape]; }
 __device__ __forceinline__ size_t slot_offset(const PlaneGeom& g, int n) {
   return static_cast<size_t>(n) * g.kslot * g.plane;
 }
@@ -124,9 +209,10 @@ struct BlurXCfg {
 // body of the x pass for one tile; `tile` holds GBX_TH * BlurXCfg<R>::SW floats, `bar` one mbarrier
 template <int R>
 __device__ __forceinline__ void blur_x_tile(float* tile, uint64_t* bar, const CUtensorMap* in_map, float* out,
-                                            const float* scale_x, const PlaneGeom& g, const BlurK<R>& k, int pl) {
+                                            const float* scale_x, const PlaneGeom& g, const BlurK<R>& k, int pl,
+                                            int bx, int by) {
   constexpr int SW = BlurXCfg<R>::SW, RP = XTile<R>::RP;
-  const int x0 = blockIdx.x * GBX_TW, yb = g.y0 + blockIdx.y * GBX_TH;
+  const int x0 = bx * GBX_TW, yb = g.y0 + by * GBX_TH;
   if (threadIdx.x == 0) {
     mbar_init(bar, 1);
     mbar_fence_init();
@@ -178,23 +264,34 @@ struct BlurX4Args {
   BlurK<R3> k3;
 };
 
-template <bool B, int R0, int R1, int R2, int R3>
-__global__ void __launch_bounds__(128) k_tma_blur_x4(const __grid_constant__ CUtensorMap m0,
-                                                     const __grid_constant__ CUtensorMap m1,
-                                                     const __grid_constant__ CUtensorMap m2,
-                                                     const __grid_constant__ CUtensorMap m3, PlaneGeom g,
+template <int B, int R0, int R1, int R2, int R3>
+__global__ void __launch_bounds__(128) k_tma_blur_x4(const __grid_constant__ typename MapArg<B>::type m0,
+                                                     const __grid_constant__ typename MapArg<B>::type m1,
+                                                     const __grid_constant__ typename MapArg<B>::type m2,
+                                                     const __grid_constant__ typename MapArg<B>::type m3,
+                                                     typename GeomArg<B>::type g,
                                                      const __grid_constant__ BlurX4Args<R0, R1, R2, R3> a) {
   constexpr int RMAX = R0 > R1 ? (R0 > R2 ? (R0 > R3 ? R0 : R3) : (R2 > R3 ? R2 : R3))
                                : (R1 > R2 ? (R1 > R3 ? R1 : R3) : (R2 > R3 ? R2 : R3));
   __shared__ __align__(128) float tile[GBX_TH * BlurXCfg<RMAX>::SW];
   __shared__ __align__(8) uint64_t bar;
+  Item it;
+  int shape = 0, sx = 0;
+  if constexpr (B == 2) {
+    const MixImage im = mix_item(g, GBX_TW, GBX_TH, it);
+    shape = im.shape;
+    sx = im.sx;
+  } else {
+    it = Item{B ? static_cast<int>(blockIdx.z) >> 2 : 0, blockIdx.x, blockIdx.y,
+              B ? blockIdx.z & 3 : blockIdx.z};
+  }
   // the image's first plane: blur_x_tile takes it as the TMA plane and as the output plane
-  const int n = B ? static_cast<int>(blockIdx.z) >> 2 : 0, pl = n * g.kslot;
-  switch (B ? blockIdx.z & 3 : blockIdx.z) {  // uniform per CTA
-    case 0: blur_x_tile<R0>(tile, &bar, &m0, a.out[0], a.scale_x[0], g, a.k0, pl); break;
-    case 1: blur_x_tile<R1>(tile, &bar, &m1, a.out[1], a.scale_x[1], g, a.k1, pl); break;
-    case 2: blur_x_tile<R2>(tile, &bar, &m2, a.out[2], a.scale_x[2], g, a.k2, pl); break;
-    default: blur_x_tile<R3>(tile, &bar, &m3, a.out[3], a.scale_x[3], g, a.k3, pl); break;
+  const int pl = it.n * g.kslot;
+  switch (it.z) {  // uniform per CTA
+    case 0: blur_x_tile<R0>(tile, &bar, map_of(m0, shape), a.out[0], a.scale_x[0] + sx, g, a.k0, pl, it.x, it.y); break;
+    case 1: blur_x_tile<R1>(tile, &bar, map_of(m1, shape), a.out[1], a.scale_x[1] + sx, g, a.k1, pl, it.x, it.y); break;
+    case 2: blur_x_tile<R2>(tile, &bar, map_of(m2, shape), a.out[2], a.scale_x[2] + sx, g, a.k2, pl, it.x, it.y); break;
+    default: blur_x_tile<R3>(tile, &bar, map_of(m3, shape), a.out[3], a.scale_x[3] + sx, g, a.k3, pl, it.x, it.y); break;
   }
 }
 
@@ -207,15 +304,25 @@ __global__ void __launch_bounds__(128) k_tma_blur_x4(const __grid_constant__ CUt
 #define GBY_TH 32
 #define GBY_G 16
 
-template <bool B, int R, int NP, class Epi>
-__global__ void __launch_bounds__(256, NP == 1 ? 3 : 2) k_tma_blur_y(const __grid_constant__ CUtensorMap in_map, const float* scale_y,
-                                                    PlaneGeom g, BlurK<R> k, Epi epi) {
+template <int B, int R, int NP, class Epi>
+__global__ void __launch_bounds__(256, NP == 1 ? 3 : 2) k_tma_blur_y(const __grid_constant__ typename MapArg<B>::type in_map, const float* scale_y,
+                                                    typename GeomArg<B>::type g, BlurK<R> k, Epi epi) {
   constexpr int HI = GBY_TH + 2 * R;
   extern __shared__ __align__(128) float dyn_smem[];
   float* tile = dyn_smem;                                                     // [NP][HI][TW]
   uint64_t* bar = reinterpret_cast<uint64_t*>(dyn_smem + NP * HI * GBY_TW);  // 8-byte aligned: sizes are multiples of 128 B
-  const int n = batch_image<B>(g);
-  const int x0 = blockIdx.x * GBY_TW, yb = g.y0 + blockIdx.y * GBY_TH, pz = blockIdx.z - n * g.zimg;
+  Item it;
+  int shape = 0;
+  if constexpr (B == 2) {
+    const MixImage im = mix_item(g, GBY_TW, GBY_TH, it);
+    shape = im.shape;
+    scale_y += im.sy;
+  } else {
+    const int n = batch_image<B>(g);
+    it = Item{n, blockIdx.x, blockIdx.y, blockIdx.z - n * g.zimg};
+  }
+  const int n = it.n, pz = it.z;
+  const int x0 = it.x * GBY_TW, yb = g.y0 + it.y * GBY_TH;
   if (threadIdx.x == 0) {
     mbar_init(bar, 1);
     mbar_fence_init();
@@ -225,7 +332,7 @@ __global__ void __launch_bounds__(256, NP == 1 ? 3 : 2) k_tma_blur_y(const __gri
     mbar_expect_tx(bar, NP * HI * GBY_TW * 4);
 #pragma unroll
     for (int p = 0; p < NP; ++p)
-      tma_load_box(tile + p * HI * GBY_TW, &in_map, bar, x0, yb - R, n * g.kslot + (NP == 1 ? pz : p));
+      tma_load_box(tile + p * HI * GBY_TW, map_of(in_map, shape), bar, x0, yb - R, n * g.kslot + (NP == 1 ? pz : p));
   }
   const int c = threadIdx.x & (GBY_TW - 1), grp = threadIdx.x >> 7;
   const int x = x0 + c, yg = yb + GBY_G * grp;
@@ -373,19 +480,33 @@ __device__ __forceinline__ void roll_y(const float* s, const BlurK<R>& k, const 
 // NP planes blurred by the same thread and handed to the epilogue as v[NP] per pixel
 // (NP == 1: blockIdx.z picks the plane).  grid (ceil(w / TW), ceil(rows / seg), NP == 1 ? planes : 1),
 // times the images of a batched launch.
-template <bool B, int R, int NP, class Epi>
-__global__ void __launch_bounds__(128) k_roll_blur(const __grid_constant__ CUtensorMap in_map, const float* scale_x,
-                                                   const float* scale_y, PlaneGeom g, int seg, BlurK<R> k, Epi epi) {
+template <int B, int R, int NP, class Epi>
+__global__ void __launch_bounds__(128) k_roll_blur(const __grid_constant__ typename MapArg<B>::type in_map_arg,
+                                                   const float* scale_x, const float* scale_y, typename GeomArg<B>::type g, int seg,
+                                                   BlurK<R> k, Epi epi) {
   typedef RollCfg<R, NP> C;
   constexpr int D = C::D, RP = XTile<R>::RP, NS = C::NS, NPOS = C::RING / GBR_CH;
   extern __shared__ __align__(128) float dyn_smem[];
   float* stage = dyn_smem;                        // [NS][NP][CH][SW]
   float* ring = dyn_smem + NS * C::kStageFloats;  // [NP][RBUF][TW]
   uint64_t* bar = reinterpret_cast<uint64_t*>(ring + C::kRingFloats);
-  const int n = batch_image<B>(g), pl0 = n * g.kslot;  // image, its first TMA plane
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, pz = blockIdx.z - n * g.zimg;
-  const int x0 = blockIdx.x * GBR_TW, x = x0 + lane;
-  const int ys = g.y0 + blockIdx.y * seg;
+  Item it;
+  int shape = 0;
+  if constexpr (B == 2) {
+    const MixImage im = mix_item(g, GBR_TW, 0, it);
+    shape = im.shape;
+    seg = im.seg;
+    scale_x += im.sx;
+    scale_y += im.sy;
+  } else {
+    const int n = batch_image<B>(g);
+    it = Item{n, blockIdx.x, blockIdx.y, blockIdx.z - n * g.zimg};
+  }
+  const CUtensorMap& in_map = *map_of(in_map_arg, shape);
+  const int n = it.n, pl0 = n * g.kslot;  // image, its first TMA plane
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, pz = it.z;
+  const int x0 = it.x * GBR_TW, x = x0 + lane;
+  const int ys = g.y0 + it.y * seg;
   const int ye = min(ys + seg, g.y_end);
   const int nsteps = (ye - ys + GBR_CH - 1) / GBR_CH, nchunks = nsteps + D;
   const int yin = ys - R;  // first input row of chunk 0
@@ -474,17 +595,28 @@ struct Blur2dCfg {
   static_assert(NP == 1 || (HI * SWI * 4) % 128 == 0, "TMA destinations must be 128-byte aligned");
 };
 
-template <bool B, int R, int NP, class Epi>
-__global__ void __launch_bounds__(256) k_tma_blur_2d(const __grid_constant__ CUtensorMap in_map, const float* scale_x,
-                                                     const float* scale_y, PlaneGeom g, BlurK<R> k, Epi epi) {
+template <int B, int R, int NP, class Epi>
+__global__ void __launch_bounds__(256) k_tma_blur_2d(const __grid_constant__ typename MapArg<B>::type in_map,
+                                                     const float* scale_x, const float* scale_y, typename GeomArg<B>::type g,
+                                                     BlurK<R> k, Epi epi) {
   typedef Blur2dCfg<R, NP> C;
   constexpr int SWI = C::SWI, HI = C::HI, RP = XTile<R>::RP;
   extern __shared__ __align__(128) float dyn_smem[];
   float* in = dyn_smem;                 // [NP][HI][SWI]
   float* tmp = dyn_smem + C::kInFloats;  // [NP][HI][TW]
   uint64_t* bar = reinterpret_cast<uint64_t*>(dyn_smem + C::kInFloats + C::kTmpFloats);
-  const int x0 = blockIdx.x * GB2_TW, yb = g.y0 + blockIdx.y * GB2_TH;
-  const int tid = threadIdx.x, n = batch_image<B>(g);
+  Item it;
+  int shape = 0;
+  if constexpr (B == 2) {
+    const MixImage im = mix_item(g, GB2_TW, GB2_TH, it);
+    shape = im.shape;
+    scale_x += im.sx;
+    scale_y += im.sy;
+  } else {
+    it = Item{batch_image<B>(g), blockIdx.x, blockIdx.y, 0};
+  }
+  const int x0 = it.x * GB2_TW, yb = g.y0 + it.y * GB2_TH;
+  const int tid = threadIdx.x, n = it.n;
   if (tid == 0) {
     mbar_init(bar, 1);
     mbar_fence_init();
@@ -493,7 +625,8 @@ __global__ void __launch_bounds__(256) k_tma_blur_2d(const __grid_constant__ CUt
   if (tid == 0) {
     mbar_expect_tx(bar, C::kInFloats * 4);
 #pragma unroll
-    for (int p = 0; p < NP; ++p) tma_load_box(in + p * HI * SWI, &in_map, bar, x0 - RP, yb - R, n * g.kslot + p);
+    for (int p = 0; p < NP; ++p)
+      tma_load_box(in + p * HI * SWI, map_of(in_map, shape), bar, x0 - RP, yb - R, n * g.kslot + p);
   }
   const bool edge_x = (x0 < R) || (x0 + GB2_TW + R > g.w);
   const bool edge_y = (yb < R) || (yb + GB2_TH + R > g.h);
@@ -890,20 +1023,31 @@ struct CombineArgs {
 };
 
 // grid (ceil(w / TW), ceil(rows / TH), 1), or (..., images) batched.
-template <bool B, int RA, int RB, int RC>
-__global__ void __launch_bounds__(256) k_tma_mask_y(const __grid_constant__ CUtensorMap map_a,
-                                                    const __grid_constant__ CUtensorMap map_b,
-                                                    const __grid_constant__ CUtensorMap map_c, const float* sya,
-                                                    const float* syb, const float* syc, PlaneGeom g, BlurK<RA> ka,
-                                                    BlurK<RB> kb, BlurK<RC> kc, CombineArgs ca) {
+template <int B, int RA, int RB, int RC>
+__global__ void __launch_bounds__(256) k_tma_mask_y(const __grid_constant__ typename MapArg<B>::type map_a,
+                                                    const __grid_constant__ typename MapArg<B>::type map_b,
+                                                    const __grid_constant__ typename MapArg<B>::type map_c,
+                                                    const float* sya, const float* syb, const float* syc, typename GeomArg<B>::type g,
+                                                    BlurK<RA> ka, BlurK<RB> kb, BlurK<RC> kc, CombineArgs ca) {
   typedef MaskYCfg<RA, RB, RC> C;
   extern __shared__ __align__(128) float dyn_smem[];
   float* ta = dyn_smem;
   float* tb = ta + C::HA * GBY_TW;
   float* tc = tb + C::HB * GBY_TW;
   uint64_t* bar = reinterpret_cast<uint64_t*>(tc + C::HC * GBY_TW);
-  const int x0 = blockIdx.x * GBY_TW, yb = g.y0 + blockIdx.y * GBY_TH;
-  const int n = batch_image<B>(g);
+  Item it;
+  int shape = 0;
+  if constexpr (B == 2) {
+    const MixImage im = mix_item(g, GBY_TW, GBY_TH, it);
+    shape = im.shape;
+    sya += im.sy;
+    syb += im.sy;
+    syc += im.sy;
+  } else {
+    it = Item{batch_image<B>(g), blockIdx.x, blockIdx.y, 0};
+  }
+  const int x0 = it.x * GBY_TW, yb = g.y0 + it.y * GBY_TH;
+  const int n = it.n;
   const size_t so = slot_offset(g, n), so0 = slot_offset0(g, n);
   if (threadIdx.x == 0) {
     mbar_init(bar, 1);
@@ -912,9 +1056,9 @@ __global__ void __launch_bounds__(256) k_tma_mask_y(const __grid_constant__ CUte
   __syncthreads();
   if (threadIdx.x == 0) {
     mbar_expect_tx(bar, (C::HA + C::HB + C::HC) * GBY_TW * 4);
-    tma_load_box(ta, &map_a, bar, x0, yb - RA, n * g.kslot);
-    tma_load_box(tb, &map_b, bar, x0, yb - RB, n * g.kslot);
-    tma_load_box(tc, &map_c, bar, x0, yb - RC, n * g.kslot);
+    tma_load_box(ta, map_of(map_a, shape), bar, x0, yb - RA, n * g.kslot);
+    tma_load_box(tb, map_of(map_b, shape), bar, x0, yb - RB, n * g.kslot);
+    tma_load_box(tc, map_of(map_c, shape), bar, x0, yb - RC, n * g.kslot);
   }
   const int c = threadIdx.x & (GBY_TW - 1), grp = threadIdx.x >> 7;
   const int x = x0 + c, yg = yb + GBY_G * grp;
@@ -976,16 +1120,25 @@ __global__ void __launch_bounds__(256) k_tma_mask_y(const __grid_constant__ CUte
 // fill outside the image is PaddedMaltaUnit's padding.  Line sums as in k_malta_sums
 // (tiled_kernels.cuh): a thread evaluates 2 x 4 pixels from a 9 x 12 register window.
 // grid (ceil(w / 64), ceil(rows / 32), 2 channels), times the images of a batched launch; 256 threads.
-template <bool B>
-__global__ void __launch_bounds__(256, 2) k_tma_malta_sums(const __grid_constant__ CUtensorMap diffs_map, float* acc,
-                                                           PlaneGeom g) {
+template <int B>
+__global__ void __launch_bounds__(256, 2) k_tma_malta_sums(const __grid_constant__ typename MapArg<B>::type diffs_map_arg,
+                                                           float* acc, typename GeomArg<B>::type g) {
   __shared__ __align__(128) float tile[2][GB_MALTA_SH * GB_MALTA_SW];
   __shared__ __align__(8) uint64_t bar[2];
   const int tx = threadIdx.x, ty = threadIdx.y;  // 16 x 16
   const int tid = ty * 16 + tx;
-  const int n = B ? static_cast<int>(blockIdx.z) >> 1 : 0;
-  const int x0 = blockIdx.x * GB_MALTA_TILE_W, y0 = g.y0 + blockIdx.y * GB_MALTA_TILE_H;
-  const int ch = B ? blockIdx.z & 1 : blockIdx.z, pl = n * g.kslot + 3 * ch;  // first plane of the channel's bands
+  Item it;
+  int shape = 0;
+  if constexpr (B == 2) {
+    shape = mix_item(g, GB_MALTA_TILE_W, GB_MALTA_TILE_H, it).shape;
+  } else {
+    it = Item{B ? static_cast<int>(blockIdx.z) >> 1 : 0, blockIdx.x, blockIdx.y,
+              B ? blockIdx.z & 1 : blockIdx.z};
+  }
+  const CUtensorMap& diffs_map = *map_of(diffs_map_arg, shape);
+  const int n = it.n;
+  const int x0 = it.x * GB_MALTA_TILE_W, y0 = g.y0 + it.y * GB_MALTA_TILE_H;
+  const int ch = it.z, pl = n * g.kslot + 3 * ch;  // first plane of the channel's bands
   constexpr uint32_t kBytes = GB_MALTA_SH * GB_MALTA_SW * 4;
   if (tid == 0) {
     mbar_init(&bar[0], 1);
@@ -1049,11 +1202,28 @@ __device__ __forceinline__ float mask_combo_y(float uhf, float hf) {
 // sup = |v - v_right| + |v - v_down| (float magnitudes, float sum, widened by the consumer),
 // neighbours mirrored at the last column / row; one plane per channel: sup[0] = X, sup[1] = Y.
 // grid (ceil(w / 32), ceil(rows / 8), 1), or (..., images) batched; 32 x 8 threads.
-template <bool B>
-__global__ void __launch_bounds__(256) k_mask_sup(const float* ps, float* sup, PlaneGeom g) {
-  const int x = blockIdx.x * 32 + threadIdx.x, y = g.y0 + blockIdx.y * 8 + threadIdx.y;
+// 32 x 8 tiles of k_mask_sup / k_mask_pre; B < 2 leaves the image to image_of (after the kernel's early exit)
+template <int B>
+__device__ __forceinline__ Item px_item(typename GeomArg<B>::type& g) {
+  Item it;
+  if constexpr (B == 2) {
+    mix_item(g, 32, 8, it);
+  } else {
+    it = Item{0, blockIdx.x, blockIdx.y, 0};
+  }
+  return it;
+}
+template <int B>
+__device__ __forceinline__ int image_of(const Item& it, const typename GeomArg<B>::type& g) {
+  return B == 2 ? it.n : batch_image<B>(g);
+}
+
+template <int B>
+__global__ void __launch_bounds__(256) k_mask_sup(const float* ps, float* sup, typename GeomArg<B>::type g) {
+  const Item it = px_item<B>(g);
+  const int x = it.x * 32 + threadIdx.x, y = g.y0 + it.y * 8 + threadIdx.y;
   if (x >= g.w || y >= g.y_end) return;
-  const size_t so = slot_offset(g, batch_image<B>(g));
+  const size_t so = slot_offset(g, image_of<B>(it, g));
   ps += so;
   sup += so;
   const int x2 = (x + 1 < g.w) ? x + 1 : (x > 0 ? x - 1 : x);
@@ -1071,11 +1241,12 @@ __global__ void __launch_bounds__(256) k_mask_sup(const float* ps, float* sup, P
 }
 
 // mpre[c] = min(cutoff, mul0 * min(sup0_c, sup1_c)) for c = X, Y.  Grid as k_mask_sup.
-template <bool B>
-__global__ void __launch_bounds__(256) k_mask_pre(const float* ps1, const float* sup0, float* mpre, PlaneGeom g) {
-  const int x = blockIdx.x * 32 + threadIdx.x, y = g.y0 + blockIdx.y * 8 + threadIdx.y;
+template <int B>
+__global__ void __launch_bounds__(256) k_mask_pre(const float* ps1, const float* sup0, float* mpre, typename GeomArg<B>::type g) {
+  const Item it = px_item<B>(g);
+  const int x = it.x * 32 + threadIdx.x, y = g.y0 + it.y * 8 + threadIdx.y;
   if (x >= g.w || y >= g.y_end) return;
-  const int n = batch_image<B>(g);
+  const int n = image_of<B>(it, g);
   const size_t so = slot_offset(g, n);
   ps1 += so;
   sup0 += slot_offset0(g, n);
@@ -1105,6 +1276,29 @@ __global__ void __launch_bounds__(256) k_mask_pre(const float* ps1, const float*
     float v = static_cast<float>(mul0 * hd_min(s0, sup1));
     if (v >= cutoff) v = static_cast<float>(cutoff);
     mpre[g.plane + o] = v;
+  }
+}
+
+// ---------------------------------------------------------------------------
+// Mixed-size calls: rows between the caller's packed images and the arena, all images of a pass in
+// one launch.  Image j has rows [row0[j], row0[j + 1]) of w floats at ext[j] (3h of its RGB planes,
+// or h of its diffmap); row r of it is row r % h of plane r / h of arena slot n0 + j.  A warp per
+// row, 8 rows per block.
+template <bool TO_ARENA>
+__global__ void __launch_bounds__(256) k_mix_rows(float* const* ext, const int* row0, float* arena, PlaneGeomMix g) {
+  const int row = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (row >= __ldg(row0 + g.mix.m)) return;
+  const int j = mix_find(row0, g.mix.m, row);
+  const int w = g.mix.img[j].w, h = g.mix.img[j].h;
+  const int r = row - __ldg(row0 + j), c = r / h, y = r - c * h;
+  float* a = arena + slot_offset(g, g.mix.n0 + j) + c * g.plane + static_cast<size_t>(y) * g.pitch;
+  float* e = ext[j] + static_cast<size_t>(r) * w;
+  for (int x = lane; x < w; x += 32) {
+    if (TO_ARENA) {
+      a[x] = e[x];
+    } else {
+      e[x] = a[x];
+    }
   }
 }
 

@@ -17,6 +17,8 @@
 #include "jpeg_dev.h"
 #include "walk_dev.h"
 #if !defined(GB200_HOSTSIM)
+#include <deque>
+#include <map>
 #include <mutex>
 #include <set>
 #include <type_traits>
@@ -59,75 +61,154 @@ void allow_smem(K kernel, size_t bytes) {
 }
 
 inline int cdiv(int a, int b) { return (a + b - 1) / b; }
+// rows of a rolling-blur segment for `rows` rows: whole steps, about GBR_SEG rows
+inline int roll_seg(int rows) {
+  const int nseg = cdiv(rows, GBR_SEG);
+  return cdiv(cdiv(rows, nseg), GBR_CH) * GBR_CH;
+}
 
-// f(std::true_type()) for a launch over several images (the kernels' batched instantiation, which
-// takes the image from blockIdx.z), f(std::false_type()) for one image.  EpiStore (stand-alone
-// blurs) has no batched form.
+}  // namespace
+
+// One pass of a mixed-size call (Butteraugli::fused_compare_sizes): its images, slots n0 .. n0 + m - 1,
+// have at most GB_MIX_SHAPES distinct sizes.  Device tables: the images, and per tile shape of the
+// chain's launches the first work item of each image.
+enum MixKind { kMix2d, kMixRollLf, kMixRollMf, kMixPx, kMixX4, kMixMalta, kMixY, kMixKinds };
+struct MixPass {
+  int n0 = 0, m = 0;
+  std::vector<std::pair<int, int> > shapes;  // (w, h) of map set index s
+  const MixImage* img = nullptr;
+  const int* tile0 = nullptr;  // [kMixKinds][m + 1]
+  int total[kMixKinds];        // work items per tile shape
+  BlurTab tab[kNumBlurs];      // border scales of the pass's sizes (MixImage::sx, sy index them)
+  const int* rows_rgb = nullptr;  // [m + 1] 3h rows per image
+  const int* rows_dm = nullptr;   // [m + 1] h rows per image
+  float* const* ext0 = nullptr;   // [m] rgb0 of each image (device memory)
+  float* const* ext1 = nullptr;
+  float* const* extdm = nullptr;  // [m] diffmap of each image, or null
+  int rows_rgb_total = 0, rows_dm_total = 0;
+  std::deque<MixMaps> mapsets;  // the map sets of the launches queued so far (stable addresses)
+  MixGeom geom(int kind) const { return MixGeom{img, tile0 + kind * (m + 1), m, n0}; }
+};
+
+struct MapReq {
+  const CUtensorMap* one;
+  const MixMaps* mix;  // a mixed pass's: one map per size
+  template <int B>
+  const typename MapArg<B>::type& get() const {
+    if constexpr (B == 2) {
+      return *mix;
+    } else {
+      return *one;
+    }
+  }
+};
+
+MapReq Butteraugli::maps(const float* base, int nplanes, int box_w, int box_h, int kslot) {
+  MapReq r{&fused_->slots(base, nplanes, box_w, box_h, kslot, g_), nullptr};
+  if (mix_ != nullptr) {
+    mix_->mapsets.emplace_back();
+    MixMaps& set = mix_->mapsets.back();
+    const int planes = (fused_->capacity - 1) * kslot + nplanes;
+    for (size_t i = 0; i < mix_->shapes.size(); ++i)
+      set.m[i] = fused_->map(base, planes, box_w, box_h, g_, mix_->shapes[i].first, mix_->shapes[i].second);
+    r.mix = &set;
+  }
+  return r;
+}
+
+namespace {
+// f(integral_constant<int, 1>) for a launch over several images (the kernels' batched instantiation,
+// which takes the image from blockIdx.z), f(<2>) for a mixed pass (images and tiles from the pass's
+// work items), f(<0>) for one image.  EpiStore (stand-alone blurs) has no batched form.
 template <class Epi, class F>
-void with_batch(int nimg, const F& f) {
+void with_batch(int nimg, const MixPass* mix, const F& f) {
   if constexpr (!std::is_same<Epi, EpiStore>::value) {
+    if (mix != nullptr) {
+      f(std::integral_constant<int, 2>());
+      return;
+    }
     if (nimg > 1) {
-      f(std::true_type());
+      f(std::integral_constant<int, 1>());
       return;
     }
   }
-  if (nimg != 1) throw std::runtime_error("with_batch: no batched form of this launch");
-  f(std::false_type());
+  if (nimg != 1 || mix != nullptr) throw std::runtime_error("with_batch: no batched form of this launch");
+  f(std::integral_constant<int, 0>());
 }
+
+// the grid of a launch: `grid`, or a mixed pass's work items of tile shape `kind`
+dim3 grid_of(dim3 grid, const MixPass* mix, int kind) { return mix == nullptr ? grid : dim3(mix->total[kind]); }
+// the geometry argument of a launch of instantiation B: pg, and for a mixed pass its work items of `kind`
+template <int B>
+typename GeomArg<B>::type geom_arg(const PlaneGeom& pg, const MixPass* mix, int kind) {
+  if constexpr (B == 2) {
+    PlaneGeomMix g;
+    static_cast<PlaneGeom&>(g) = pg;
+    g.mix = mix->geom(kind);
+    return g;
+  } else {
+    return pg;
+  }
+}
+const BlurTab& tab_of(const Tables& t, const MixPass* mix, int id) { return mix ? mix->tab[id] : t.blur[id]; }
 
 // Rolling-window blur of a plane group with epilogue (k_roll_blur); `in_map` has boxes of
 // RollCfg<R, NP>::SW x GBR_CH.  The launch's rows are cut into segments of whole steps of
 // about GBR_SEG rows.  nimg images: arena slots 0 .. nimg - 1 (PlaneGeom::kslot).
 template <int R, int NP, class Epi>
-void launch_roll(Stream s, const CUtensorMap& in_map, int planes_z, int nimg, const BlurTab& tab, PlaneGeom pg,
-                 const HostTables& ht, int id, const Epi& epi, const char* name) {
+void launch_roll(Stream s, const MapReq& in_map, int planes_z, int nimg, const BlurTab& tab, PlaneGeom pg,
+                 const HostTables& ht, int id, const Epi& epi, const char* name, const MixPass* mix = nullptr,
+                 int kind = 0) {
   const int rows = pg.y_end - pg.y0;
   if (rows <= 0) return;
   typedef RollCfg<R, NP> C;
-  const int nseg = cdiv(rows, GBR_SEG);
-  const int seg = cdiv(cdiv(rows, nseg), GBR_CH) * GBR_CH;
+  const int seg = roll_seg(rows);
   pg.zimg = planes_z;
-  dim3 grid(cdiv(pg.w, GBR_TW), cdiv(rows, seg), planes_z * nimg);
+  const dim3 grid = grid_of(dim3(cdiv(pg.w, GBR_TW), cdiv(rows, seg), planes_z * nimg), mix, kind);
   note_launch(name, s, static_cast<double>(pg.w) * rows * (NP == 1 ? planes_z : NP) * nimg);
-  with_batch<Epi>(nimg, [&](auto b) {
-    constexpr bool B = decltype(b)::value;
+  with_batch<Epi>(nimg, mix, [&](auto b) {
+    constexpr int B = decltype(b)::value;
     allow_smem(k_roll_blur<B, R, NP, Epi>, C::kSmemBytes);
-    k_roll_blur<B, R, NP, Epi><<<grid, 128, C::kSmemBytes, s>>>(in_map, tab.scale_x, tab.scale_y, pg, seg,
+    k_roll_blur<B, R, NP, Epi><<<grid, 128, C::kSmemBytes, s>>>(in_map.get<B>(), tab.scale_x, tab.scale_y,
+                                                                geom_arg<B>(pg, mix, kind), seg,
                                                                 make_blurk<R>(ht, id), epi);
   });
   note_launch_end(name, s);
 }
 
 template <int R, int NP, class Epi>
-void launch_tma_y(Stream s, const CUtensorMap& in_map, int planes_z, int nimg, const BlurTab& tab, PlaneGeom pg,
-                  const HostTables& ht, int id, const Epi& epi, const char* name) {
+void launch_tma_y(Stream s, const MapReq& in_map, int planes_z, int nimg, const BlurTab& tab, PlaneGeom pg,
+                  const HostTables& ht, int id, const Epi& epi, const char* name, const MixPass* mix = nullptr,
+                  int kind = 0) {
   const int rows = pg.y_end - pg.y0;
   if (rows <= 0) return;
   const size_t smem = static_cast<size_t>(NP) * (GBY_TH + 2 * R) * GBY_TW * sizeof(float) + 16;
   pg.zimg = planes_z;
-  dim3 grid(cdiv(pg.w, GBY_TW), cdiv(rows, GBY_TH), planes_z * nimg);
+  const dim3 grid = grid_of(dim3(cdiv(pg.w, GBY_TW), cdiv(rows, GBY_TH), planes_z * nimg), mix, kind);
   note_launch(name, s, static_cast<double>(pg.w) * rows * (NP == 1 ? planes_z : NP) * nimg);
-  with_batch<Epi>(nimg, [&](auto b) {
-    constexpr bool B = decltype(b)::value;
+  with_batch<Epi>(nimg, mix, [&](auto b) {
+    constexpr int B = decltype(b)::value;
     allow_smem(k_tma_blur_y<B, R, NP, Epi>, smem);
-    k_tma_blur_y<B, R, NP, Epi><<<grid, 256, smem, s>>>(in_map, tab.scale_y, pg, make_blurk<R>(ht, id), epi);
+    k_tma_blur_y<B, R, NP, Epi><<<grid, 256, smem, s>>>(in_map.get<B>(), tab.scale_y, geom_arg<B>(pg, mix, kind),
+                                                        make_blurk<R>(ht, id), epi);
   });
   note_launch_end(name, s);
 }
 
 template <int R, int NP, class Epi>
-void launch_tma_2d(Stream s, const CUtensorMap& in_map, int nimg, const BlurTab& tab, PlaneGeom pg,
-                   const HostTables& ht, int id, const Epi& epi, const char* name) {
+void launch_tma_2d(Stream s, const MapReq& in_map, int nimg, const BlurTab& tab, PlaneGeom pg,
+                   const HostTables& ht, int id, const Epi& epi, const char* name, const MixPass* mix = nullptr) {
   const int rows = pg.y_end - pg.y0;
   if (rows <= 0) return;
   typedef Blur2dCfg<R, NP> C;
   pg.zimg = 1;
-  dim3 grid(cdiv(pg.w, GB2_TW), cdiv(rows, GB2_TH), nimg);
+  const dim3 grid = grid_of(dim3(cdiv(pg.w, GB2_TW), cdiv(rows, GB2_TH), nimg), mix, kMix2d);
   note_launch(name, s, static_cast<double>(pg.w) * rows * nimg);
-  with_batch<Epi>(nimg, [&](auto b) {
-    constexpr bool B = decltype(b)::value;
+  with_batch<Epi>(nimg, mix, [&](auto b) {
+    constexpr int B = decltype(b)::value;
     allow_smem(k_tma_blur_2d<B, R, NP, Epi>, C::kSmemBytes);
-    k_tma_blur_2d<B, R, NP, Epi><<<grid, 256, C::kSmemBytes, s>>>(in_map, tab.scale_x, tab.scale_y, pg,
+    k_tma_blur_2d<B, R, NP, Epi><<<grid, 256, C::kSmemBytes, s>>>(in_map.get<B>(), tab.scale_x, tab.scale_y,
+                                                                  geom_arg<B>(pg, mix, kMix2d),
                                                                   make_blurk<R>(ht, id), epi);
   });
   note_launch_end(name, s);
@@ -157,9 +238,8 @@ PlaneGeom fused_geom(const Geom& g, int y0, int y_end, int kslot, int kslot0) {
 void Butteraugli::fused_opsin(const float* lin, float* xyb, int nimg, int kslot) {
   const PlaneGeom pg = fused_geom(g_, r_.cr_lo, r_.cr_hi, kslot, kslot);
   typedef Blur2dCfg<GB_R_OPSIN, 3> C;
-  const CUtensorMap& m = fused_->slots(lin, 3, C::SWI, C::HI, kslot, g_);
-  launch_tma_2d<GB_R_OPSIN, 3>(s_, m, nimg, t_.blur[kBlurOpsin], pg, ht_, kBlurOpsin,
-                               EpiOpsin{xyb, g_.pitch, g_.plane, kslot * g_.plane}, "opsin_fused");
+  launch_tma_2d<GB_R_OPSIN, 3>(s_, maps(lin, 3, C::SWI, C::HI, kslot), nimg, tab_of(t_, mix_, kBlurOpsin), pg, ht_,
+                               kBlurOpsin, EpiOpsin{xyb, g_.pitch, g_.plane, kslot * g_.plane}, "opsin_fused", mix_);
 }
 
 // SeparateFrequencies; with_diffs: also the Malta pre-pass and the noise difference against ps0_.
@@ -168,8 +248,8 @@ void Butteraugli::fused_separate(const float* xyb, float* ps, bool with_diffs, i
   const size_t P = g_.plane, S = kslot * P, S0 = kslot0 * P;
   // S2: lf = Blur(xyb, 7.47); mf_in = xyb - lf
   // (launch names are those of the former y-pass kernels, which these replace)
-  launch_roll<GB_R_LF, 1>(s_, fused_->slots(xyb, 3, RollCfg<GB_R_LF, 1>::SW, GBR_CH, kslot, g_), 3, nimg, t_.blur[kBlurLf], pg, ht_,
-                          kBlurLf, EpiLf{xyb, lf_, mf_in_, g_.pitch, P, S}, "lf_fused_y");
+  launch_roll<GB_R_LF, 1>(s_, maps(xyb, 3, RollCfg<GB_R_LF, 1>::SW, GBR_CH, kslot), 3, nimg, tab_of(t_, mix_, kBlurLf), pg,
+                          ht_, kBlurLf, EpiLf{xyb, lf_, mf_in_, g_.pitch, P, S}, "lf_fused_y", mix_, kMixRollLf);
   // S3 + S4: mf = Blur(mf_in, 3.73); split, range tweaks, SuppressXByY (+ Malta pre-pass of the mf bands)
   EpiMf em;
   em.mf_in = mf_in_;
@@ -183,8 +263,8 @@ void Butteraugli::fused_separate(const float* xyb, float* ps, bool with_diffs, i
   em.plane = P;
   em.slot = S;
   em.slot0 = S0;
-  launch_roll<GB_R_MF, 3>(s_, fused_->slots(mf_in_, 3, RollCfg<GB_R_MF, 3>::SW, GBR_CH, kslot, g_), 1, nimg, t_.blur[kBlurMf], pg,
-                          ht_, kBlurMf, em, "mf_fused_y");
+  launch_roll<GB_R_MF, 3>(s_, maps(mf_in_, 3, RollCfg<GB_R_MF, 3>::SW, GBR_CH, kslot), 1, nimg, tab_of(t_, mix_, kBlurMf),
+                          pg, ht_, kBlurMf, em, "mf_fused_y", mix_, kMixRollMf);
   // S5 + S6: hf = Blur(hf_raw, 1.87) in one kernel; uhf / hf / lf "vals" (+ Malta pre-pass, noise difference)
   EpiHf eh;
   eh.lf_raw = lf_;
@@ -201,8 +281,8 @@ void Butteraugli::fused_separate(const float* xyb, float* ps, bool with_diffs, i
   eh.slot = S;
   eh.slot0 = S0;
   typedef Blur2dCfg<GB_R_HF, 2> C;
-  launch_tma_2d<GB_R_HF, 2>(s_, fused_->slots(hf_raw_, 2, C::SWI, C::HI, kslot, g_), nimg, t_.blur[kBlurHf], pg, ht_, kBlurHf, eh,
-                            "hf_fused");
+  launch_tma_2d<GB_R_HF, 2>(s_, maps(hf_raw_, 2, C::SWI, C::HI, kslot), nimg, tab_of(t_, mix_, kBlurHf), pg, ht_, kBlurHf,
+                            eh, "hf_fused", mix_);
 }
 
 // Neighbour sums of DiffPrecompute for the original's PsychoImage (constant during the search).
@@ -210,9 +290,12 @@ void Butteraugli::fused_sup0(int nimg, int kslot) {
   if (!use_fused_) return;
   const PlaneGeom pg = fused_geom(g_, r_.cr_lo, r_.cr_hi, kslot, kslot);
   const int rows = r_.cr_hi - r_.cr_lo;
-  dim3 block(32, 8), grid(cdiv(g_.w, 32), cdiv(rows, 8), nimg);
+  dim3 block(32, 8), grid = grid_of(dim3(cdiv(g_.w, 32), cdiv(rows, 8), nimg), mix_, kMixPx);
   note_launch("mask_sup0", s_, static_cast<double>(g_.w) * rows * nimg);
-  with_batch<void>(nimg, [&](auto b) { k_mask_sup<decltype(b)::value><<<grid, block, 0, s_>>>(ps0_, sup0_, pg); });
+  with_batch<void>(nimg, mix_, [&](auto b) {
+    constexpr int B = decltype(b)::value;
+    k_mask_sup<B><<<grid, block, 0, s_>>>(ps0_, sup0_, geom_arg<B>(pg, mix_, kMixPx));
+  });
   note_launch_end("mask_sup0", s_);
 }
 
@@ -222,8 +305,8 @@ void Butteraugli::fused_blur(const float* in, float* out, int nplanes, int id) {
   const EpiStore st{out, g_.pitch, g_.plane};
 #define GB_BLUR_CASE(R)                                                                                               \
   case R:                                                                                                             \
-    launch_roll<R, 1>(s_, fused_->map(in, nplanes, RollCfg<R, 1>::SW, GBR_CH, g_), nplanes, 1, t_.blur[id], pg, ht_, id, \
-                      st, "tma_blur_y");                                                                              \
+    launch_roll<R, 1>(s_, MapReq{&fused_->map(in, nplanes, RollCfg<R, 1>::SW, GBR_CH, g_), nullptr}, nplanes, 1,      \
+                      t_.blur[id], pg, ht_, id, st, "tma_blur_y");                                                    \
     break;
   switch (t_.blur[id].r) {
     GB_BLUR_CASE(2)
@@ -308,9 +391,12 @@ void Butteraugli::fused_compare_launches(int nimg, int kslot, int kslot0) {
   fused_separate(xyb_, ps1_, true, nimg, kslot, kslot0);
   // S10 mask: DiffPrecompute against the original's resident neighbour sums
   {
-    dim3 block(32, 8), grid(cdiv(g_.w, 32), cdiv(rows, 8), nimg);
+    dim3 block(32, 8), grid = grid_of(dim3(cdiv(g_.w, 32), cdiv(rows, 8), nimg), mix_, kMixPx);
     note_launch("mask_pre", s_, static_cast<double>(g_.w) * rows * nimg);
-    with_batch<void>(nimg, [&](auto b) { k_mask_pre<decltype(b)::value><<<grid, block, 0, s_>>>(ps1_, sup0_, mpre_, pg); });
+    with_batch<void>(nimg, mix_, [&](auto b) {
+      constexpr int B = decltype(b)::value;
+      k_mask_pre<B><<<grid, block, 0, s_>>>(ps1_, sup0_, mpre_, geom_arg<B>(pg, mix_, kMixPx));
+    });
     note_launch_end("mask_pre", s_);
   }
   // x passes of the noise blur (S8) and of the three mask blurs in one launch:
@@ -322,64 +408,72 @@ void Butteraugli::fused_compare_launches(int nimg, int kslot, int kslot0) {
     xa.out[1] = tmp_;
     xa.out[2] = tmp_ + P;
     xa.out[3] = tmp_ + 2 * P;
-    xa.scale_x[0] = t_.blur[kBlurNoise].scale_x;
-    xa.scale_x[1] = t_.blur[kBlurMaskX].scale_x;
-    xa.scale_x[2] = t_.blur[kBlurMaskY1].scale_x;
-    xa.scale_x[3] = t_.blur[kBlurMaskY0].scale_x;
+    xa.scale_x[0] = tab_of(t_, mix_, kBlurNoise).scale_x;
+    xa.scale_x[1] = tab_of(t_, mix_, kBlurMaskX).scale_x;
+    xa.scale_x[2] = tab_of(t_, mix_, kBlurMaskY1).scale_x;
+    xa.scale_x[3] = tab_of(t_, mix_, kBlurMaskY0).scale_x;
     xa.k0 = make_blurk<GB_R_NOISE>(ht_, kBlurNoise);
     xa.k1 = make_blurk<GB_R_MASKX>(ht_, kBlurMaskX);
     xa.k2 = make_blurk<GB_R_MASKY1>(ht_, kBlurMaskY1);
     xa.k3 = make_blurk<GB_R_MASKY0>(ht_, kBlurMaskY0);
-    dim3 grid(cdiv(g_.w, GBX_TW), cdiv(rows, GBX_TH), 4 * nimg);
+    const dim3 grid = grid_of(dim3(cdiv(g_.w, GBX_TW), cdiv(rows, GBX_TH), 4 * nimg), mix_, kMixX4);
     note_launch("tma_blur_x", s_, 4.0 * g_.w * rows * nimg);
-    with_batch<void>(nimg, [&](auto b) {
-      k_tma_blur_x4<decltype(b)::value, GB_R_NOISE, GB_R_MASKX, GB_R_MASKY1, GB_R_MASKY0><<<grid, 128, 0, s_>>>(
-          fused_->slots(noise_, 1, BlurXCfg<GB_R_NOISE>::SW, GBX_TH, kslot, g_),
-          fused_->slots(mpre_, 1, BlurXCfg<GB_R_MASKX>::SW, GBX_TH, kslot, g_),
-          fused_->slots(mpre_ + P, 1, BlurXCfg<GB_R_MASKY1>::SW, GBX_TH, kslot, g_),
-          fused_->slots(mpre_ + P, 1, BlurXCfg<GB_R_MASKY0>::SW, GBX_TH, kslot, g_), pg, xa);
+    const MapReq m0 = maps(noise_, 1, BlurXCfg<GB_R_NOISE>::SW, GBX_TH, kslot);
+    const MapReq m1 = maps(mpre_, 1, BlurXCfg<GB_R_MASKX>::SW, GBX_TH, kslot);
+    const MapReq m2 = maps(mpre_ + P, 1, BlurXCfg<GB_R_MASKY1>::SW, GBX_TH, kslot);
+    const MapReq m3 = maps(mpre_ + P, 1, BlurXCfg<GB_R_MASKY0>::SW, GBX_TH, kslot);
+    with_batch<void>(nimg, mix_, [&](auto b) {
+      constexpr int B = decltype(b)::value;
+      k_tma_blur_x4<B, GB_R_NOISE, GB_R_MASKX, GB_R_MASKY1, GB_R_MASKY0>
+          <<<grid, 128, 0, s_>>>(m0.get<B>(), m1.get<B>(), m2.get<B>(), m3.get<B>(), geom_arg<B>(pg, mix_, kMixX4), xa);
     });
     note_launch_end("tma_blur_x", s_);
   }
   // S7 Malta line sums of both channels: ac[ch] = ((0 + uhf) + hf) + mf
   {
-    dim3 block(16, 16), grid(cdiv(g_.w, GB_MALTA_TILE_W), cdiv(rows, GB_MALTA_TILE_H), 2 * nimg);
+    dim3 block(16, 16);
+    const dim3 grid = grid_of(dim3(cdiv(g_.w, GB_MALTA_TILE_W), cdiv(rows, GB_MALTA_TILE_H), 2 * nimg), mix_, kMixMalta);
     note_launch("malta_sums", s_, 2.0 * g_.w * rows * nimg);
-    with_batch<void>(nimg, [&](auto b) {
-      k_tma_malta_sums<decltype(b)::value>
-          <<<grid, block, 0, s_>>>(fused_->slots(diffs6_, 6, GB_MALTA_SW, GB_MALTA_SH, kslot, g_), ac_, pg);
+    const MapReq m = maps(diffs6_, 6, GB_MALTA_SW, GB_MALTA_SH, kslot);
+    with_batch<void>(nimg, mix_, [&](auto b) {
+      constexpr int B = decltype(b)::value;
+      k_tma_malta_sums<B><<<grid, block, 0, s_>>>(m.get<B>(), ac_, geom_arg<B>(pg, mix_, kMixMalta));
     });
     note_launch_end("malta_sums", s_);
   }
   // S8 tail + S9 on block_diff_ac[Y]: blurred noise difference, asymmetric L2 of hf[Y]
-  launch_tma_y<GB_R_NOISE, 1>(s_, fused_->slots(blr_, 1, GBY_TW, GBY_TH + 2 * GB_R_NOISE, kslot, g_), 1, nimg,
-                              t_.blur[kBlurNoise], pg, ht_, kBlurNoise,
+  launch_tma_y<GB_R_NOISE, 1>(s_, maps(blr_, 1, GBY_TW, GBY_TH + 2 * GB_R_NOISE, kslot), 1, nimg,
+                              tab_of(t_, mix_, kBlurNoise), pg, ht_, kBlurNoise,
                               EpiNoise{ps0_ + kHfY * P, ps1_ + kHfY * P, ac_ + P, asym_w0_, asym_w1_, g_.pitch, S, S0},
-                              "noise_fused_y");
+                              "noise_fused_y", mix_, kMixY);
   // y passes + S11 CombineChannels + first half of S12 -> dm_[1]
   {
     typedef MaskYCfg<GB_R_MASKX, GB_R_MASKY0, GB_R_MASKY1> C;
     CombineArgs ca{ps0_, ps1_, ac_, dm_ + P, t_.mask_lut, g_.pitch, P};
-    dim3 grid(cdiv(g_.w, GBY_TW), cdiv(rows, GBY_TH), nimg);
+    const dim3 grid = grid_of(dim3(cdiv(g_.w, GBY_TW), cdiv(rows, GBY_TH), nimg), mix_, kMixY);
     note_launch("mask_y_combine", s_, static_cast<double>(g_.w) * rows * nimg);
-    with_batch<void>(nimg, [&](auto b) {
-      constexpr bool B = decltype(b)::value;
+    const MapReq ma = maps(tmp_, 1, GBY_TW, C::HA, kslot), mb = maps(tmp_ + 2 * P, 1, GBY_TW, C::HB, kslot),
+                 mc = maps(tmp_ + P, 1, GBY_TW, C::HC, kslot);
+    with_batch<void>(nimg, mix_, [&](auto b) {
+      constexpr int B = decltype(b)::value;
       allow_smem(k_tma_mask_y<B, GB_R_MASKX, GB_R_MASKY0, GB_R_MASKY1>, C::kSmemBytes);
       k_tma_mask_y<B, GB_R_MASKX, GB_R_MASKY0, GB_R_MASKY1><<<grid, 256, C::kSmemBytes, s_>>>(
-          fused_->slots(tmp_, 1, GBY_TW, C::HA, kslot, g_), fused_->slots(tmp_ + 2 * P, 1, GBY_TW, C::HB, kslot, g_),
-          fused_->slots(tmp_ + P, 1, GBY_TW, C::HC, kslot, g_), t_.blur[kBlurMaskX].scale_y, t_.blur[kBlurMaskY0].scale_y,
-          t_.blur[kBlurMaskY1].scale_y, pg, make_blurk<GB_R_MASKX>(ht_, kBlurMaskX),
-          make_blurk<GB_R_MASKY0>(ht_, kBlurMaskY0), make_blurk<GB_R_MASKY1>(ht_, kBlurMaskY1), ca);
+          ma.get<B>(), mb.get<B>(), mc.get<B>(), tab_of(t_, mix_, kBlurMaskX).scale_y,
+          tab_of(t_, mix_, kBlurMaskY0).scale_y, tab_of(t_, mix_, kBlurMaskY1).scale_y, geom_arg<B>(pg, mix_, kMixY),
+          make_blurk<GB_R_MASKX>(ht_, kBlurMaskX), make_blurk<GB_R_MASKY0>(ht_, kBlurMaskY0),
+          make_blurk<GB_R_MASKY1>(ht_, kBlurMaskY1), ca);
     });
     note_launch_end("mask_y_combine", s_);
   }
   // S12 second half + S13: blur 1.73, mix, per-block maxima, global maximum (one per image)
-  dev_zero(d_gmax_, sizeof(unsigned int) * nimg, s_);
+  // (a mixed pass: the slots n0 ..; their block maxima keep the batch's block grid, and only the
+  // global maxima are read)
+  dev_zero(d_gmax_ + (mix_ ? mix_->n0 : 0), sizeof(unsigned int) * nimg, s_);
   {
     typedef Blur2dCfg<GB_R_FINAL, 1> C;
     EpiFinal ef{dm_, block_max_, r_.strips() ? nullptr : d_gmax_, g_.pitch, g_.bw, r_.by_lo, r_.by_hi, S, g_.nblocks};
-    launch_tma_2d<GB_R_FINAL, 1>(s_, fused_->slots(dm_ + P, 1, C::SWI, C::HI, kslot, g_), nimg, t_.blur[kBlurFinal], pg, ht_,
-                                 kBlurFinal, ef, "final_fused");
+    launch_tma_2d<GB_R_FINAL, 1>(s_, maps(dm_ + P, 1, C::SWI, C::HI, kslot), nimg, tab_of(t_, mix_, kBlurFinal), pg, ht_,
+                                 kBlurFinal, ef, "final_fused", mix_);
   }
 }
 
@@ -399,6 +493,256 @@ void Butteraugli::fused_compare_batch(const float* rgb0, const float* rgb1, int 
   if (diffmap != nullptr) copy_3d(diffmap, row, g_.h, dm_, pitch, slot_rows, row, g_.h, n, s_);
   // one transfer of the n maxima (float bits); d2h waits for it, and so for everything queued before
   d2h(maxima, d_gmax_, sizeof(float) * n, s_);
+}
+
+// ---- pairs of different sizes (compare_batch_sizes) ----
+// The buffers of the mixed calls, grown to the largest call so far and kept: the tables of a call
+// (images, work items, row counts, pointers and border scales of every pass, one upload), the staging
+// of host images and host diffmaps, and the border scales of every size seen (host libm, once per size).
+struct Butteraugli::Mixed {
+  std::vector<unsigned char> blob;  // host image of `tables`
+  void* tables = nullptr;
+  size_t tables_bytes = 0;
+  std::vector<float> host_in;  // host images, packed
+  float* stage_in = nullptr;
+  size_t stage_in_floats = 0;
+  float* stage_dm = nullptr;
+  size_t stage_dm_floats = 0;
+  std::map<std::pair<int, int>, std::vector<float> > scales;  // size -> [blur][w + h] (scale_x, then scale_y)
+};
+
+void Butteraugli::mixed_release() {
+  if (mixed_ == nullptr) return;
+  dev_free(mixed_->tables);
+  dev_free(mixed_->stage_in);
+  dev_free(mixed_->stage_dm);
+  delete mixed_;
+  mixed_ = nullptr;
+}
+
+namespace {
+// device buffer of at least `want` elements, grown (its contents are not kept)
+template <class T>
+T* grow(T* p, size_t* have, size_t want) {
+  if (want <= *have && p != nullptr) return p;
+  dev_free(p);
+  *have = 0;
+  p = static_cast<T*>(dev_alloc(sizeof(T) * std::max<size_t>(want, 1)));
+  *have = want;
+  return p;
+}
+size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+}  // namespace
+
+void Butteraugli::fused_compare_sizes(const int* w, const int* h, const float* const* rgb0, const float* const* rgb1,
+                                      int n, float* const* diffmap, float* maxima, bool device) {
+  if (mixed_ == nullptr) mixed_ = new Mixed();
+  Mixed& mx = *mixed_;
+  // The per-size caches (border scales here, tensor maps in Fused::maps) are bounded: once they hold more
+  // than kMixCachedSizes sizes, a call starts by dropping them.  No launch of an earlier call reads them
+  // any more (its maps went into its launch parameters), and this call rebuilds what it uses.
+  constexpr size_t kMixCachedSizes = 256;
+  if (mx.scales.size() > kMixCachedSizes) {
+    mx.scales.clear();
+    fused_->drop_other_sizes(g_);
+  }
+  // Slots in the order of the sizes, so that a pass (at most GB_MIX_SHAPES sizes) is a run of slots.
+  std::vector<int> order(n);
+  for (int i = 0; i < n; ++i) order[i] = i;
+  std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return std::make_pair(w[a], h[a]) < std::make_pair(w[b], h[b]); });
+  std::vector<MixPass> passes;
+  for (int k = 0; k < n; ++k) {
+    const std::pair<int, int> sz(w[order[k]], h[order[k]]);
+    const bool new_size = k == 0 || sz != std::make_pair(w[order[k - 1]], h[order[k - 1]]);
+    if (k == 0 || (new_size && passes.back().shapes.size() == GB_MIX_SHAPES)) {
+      passes.emplace_back();
+      passes.back().n0 = k;
+    }
+    MixPass& p = passes.back();
+    if (new_size) p.shapes.push_back(sz);
+    ++p.m;
+  }
+  // Host images: packed once, uploaded in one copy, rgb0 then rgb1 of every pair in slot order.
+  std::vector<size_t> at(n);  // floats before pair k's rgb0 (slot order), in the staging of one side
+  size_t side = 0, dm_floats = 0;
+  for (int k = 0; k < n; ++k) {
+    at[k] = side;
+    side += static_cast<size_t>(3) * w[order[k]] * h[order[k]];
+    dm_floats += static_cast<size_t>(w[order[k]]) * h[order[k]];
+  }
+  if (!device) {
+    mx.stage_in = grow(mx.stage_in, &mx.stage_in_floats, 2 * side);
+    mx.host_in.resize(2 * side);
+    for (int k = 0; k < n; ++k) {
+      const size_t img = static_cast<size_t>(3) * w[order[k]] * h[order[k]];
+      memcpy(&mx.host_in[at[k]], rgb0[order[k]], sizeof(float) * img);
+      memcpy(&mx.host_in[side + at[k]], rgb1[order[k]], sizeof(float) * img);
+    }
+    if (diffmap != nullptr) mx.stage_dm = grow(mx.stage_dm, &mx.stage_dm_floats, dm_floats);
+  }
+  // The tables of every pass, laid out in one blob (offsets first, pointers filled once it has an address).
+  struct Layout {
+    size_t img, tile0, rows_rgb, rows_dm, ext0, ext1, extdm, scales, blur_len;
+  };
+  std::vector<Layout> lay(passes.size());
+  size_t bytes = 0;
+  for (size_t q = 0; q < passes.size(); ++q) {
+    const MixPass& p = passes[q];
+    Layout& l = lay[q];
+    size_t len = 0;
+    for (const std::pair<int, int>& sz : p.shapes) len += sz.first + sz.second;
+    l.blur_len = len;
+    l.img = bytes = align_up(bytes, 32);
+    bytes += sizeof(MixImage) * p.m;
+    l.tile0 = bytes = align_up(bytes, 16);
+    bytes += sizeof(int) * kMixKinds * (p.m + 1);
+    l.rows_rgb = bytes;
+    bytes += sizeof(int) * (p.m + 1);
+    l.rows_dm = bytes;
+    bytes += sizeof(int) * (p.m + 1);
+    l.ext0 = bytes = align_up(bytes, 16);
+    bytes += sizeof(float*) * p.m;
+    l.ext1 = bytes;
+    bytes += sizeof(float*) * p.m;
+    l.extdm = bytes;
+    bytes += sizeof(float*) * p.m;
+    l.scales = bytes = align_up(bytes, 16);
+    bytes += sizeof(float) * kNumBlurs * len;
+  }
+  mx.tables = grow(static_cast<unsigned char*>(mx.tables), &mx.tables_bytes, bytes);
+  mx.blob.assign(bytes, 0);
+  unsigned char* dev = static_cast<unsigned char*>(mx.tables);
+  // tile shapes of the chain's launches (th 0: the image's rolling-blur segment) and images per tile z
+  static const int kTile[kMixKinds][3] = {{GB2_TW, GB2_TH, 1}, {GBR_TW, 0, 3},  {GBR_TW, 0, 1},
+                                          {32, 8, 1},          {GBX_TW, GBX_TH, 4}, {GB_MALTA_TILE_W, GB_MALTA_TILE_H, 2},
+                                          {GBY_TW, GBY_TH, 1}};
+  for (size_t q = 0; q < passes.size(); ++q) {
+    MixPass& p = passes[q];
+    const Layout& l = lay[q];
+    unsigned char* b = mx.blob.data();
+    MixImage* img = reinterpret_cast<MixImage*>(b + l.img);
+    int* tile0 = reinterpret_cast<int*>(b + l.tile0);
+    int* rows_rgb = reinterpret_cast<int*>(b + l.rows_rgb);
+    int* rows_dm = reinterpret_cast<int*>(b + l.rows_dm);
+    float** ext0 = reinterpret_cast<float**>(b + l.ext0);
+    float** ext1 = reinterpret_cast<float**>(b + l.ext1);
+    float** extdm = reinterpret_cast<float**>(b + l.extdm);
+    float* sc = reinterpret_cast<float*>(b + l.scales);
+    // border scales: per blur, scale_x of every size, then scale_y of every size
+    std::vector<int> sxo(p.shapes.size()), syo(p.shapes.size());
+    size_t ox = 0, oy = 0, xsum = 0;
+    for (const std::pair<int, int>& sz : p.shapes) xsum += sz.first;
+    for (size_t s = 0; s < p.shapes.size(); ++s) {
+      const int sw = p.shapes[s].first, sh = p.shapes[s].second;
+      std::vector<float>& cached = mx.scales[p.shapes[s]];
+      if (cached.empty()) {
+        for (int id = 0; id < kNumBlurs; ++id) {
+          const std::vector<float> x = blur_axis_scales(id, sw), y = blur_axis_scales(id, sh);
+          cached.insert(cached.end(), x.begin(), x.end());
+          cached.insert(cached.end(), y.begin(), y.end());
+        }
+      }
+      sxo[s] = static_cast<int>(ox);
+      syo[s] = static_cast<int>(xsum + oy);
+      for (int id = 0; id < kNumBlurs; ++id) {
+        const float* c = &cached[static_cast<size_t>(id) * (sw + sh)];
+        memcpy(sc + id * l.blur_len + sxo[s], c, sizeof(float) * sw);
+        memcpy(sc + id * l.blur_len + syo[s], c + sw, sizeof(float) * sh);
+      }
+      ox += sw;
+      oy += sh;
+    }
+    for (int id = 0; id < kNumBlurs; ++id) {
+      p.tab[id] = t_.blur[id];
+      p.tab[id].scale_x = p.tab[id].scale_y = reinterpret_cast<const float*>(dev + l.scales) + id * l.blur_len;
+    }
+    int shape = -1;
+    rows_rgb[0] = rows_dm[0] = 0;
+    for (int kind = 0; kind < kMixKinds; ++kind) tile0[kind * (p.m + 1)] = 0;
+    for (int j = 0; j < p.m; ++j) {
+      const int slot = p.n0 + j, i = order[slot], iw = w[i], ih = h[i];
+      if (j == 0 || std::make_pair(iw, ih) != p.shapes[shape]) ++shape;
+      MixImage& im = img[j];
+      im.w = iw;
+      im.h = ih;
+      im.shape = shape;
+      im.sx = sxo[shape];
+      im.sy = syo[shape];
+      im.seg = roll_seg(ih);
+      for (int kind = 0; kind < kMixKinds; ++kind) {
+        const int th = kTile[kind][1] ? kTile[kind][1] : im.seg;
+        const long long items = static_cast<long long>(cdiv(iw, kTile[kind][0])) * cdiv(ih, th) * kTile[kind][2];
+        int* t = tile0 + kind * (p.m + 1);
+        if (t[j] + items > 0x7fffffffLL) throw std::runtime_error("butteraugli batch: too many tiles in one call");
+        t[j + 1] = t[j] + static_cast<int>(items);
+      }
+      rows_rgb[j + 1] = rows_rgb[j] + 3 * ih;
+      rows_dm[j + 1] = rows_dm[j] + ih;
+      if (device) {
+        ext0[j] = const_cast<float*>(rgb0[i]);
+        ext1[j] = const_cast<float*>(rgb1[i]);
+        extdm[j] = diffmap != nullptr ? diffmap[i] : nullptr;
+      } else {
+        ext0[j] = mx.stage_in + at[slot];
+        ext1[j] = mx.stage_in + side + at[slot];
+        extdm[j] = diffmap != nullptr ? mx.stage_dm + (at[slot] / 3) : nullptr;
+      }
+    }
+    p.img = reinterpret_cast<const MixImage*>(dev + l.img);
+    p.tile0 = reinterpret_cast<const int*>(dev + l.tile0);
+    p.rows_rgb = reinterpret_cast<const int*>(dev + l.rows_rgb);
+    p.rows_dm = reinterpret_cast<const int*>(dev + l.rows_dm);
+    p.ext0 = reinterpret_cast<float* const*>(dev + l.ext0);
+    p.ext1 = reinterpret_cast<float* const*>(dev + l.ext1);
+    p.extdm = reinterpret_cast<float* const*>(dev + l.extdm);
+    for (int kind = 0; kind < kMixKinds; ++kind) p.total[kind] = tile0[kind * (p.m + 1) + p.m];
+    p.rows_rgb_total = rows_rgb[p.m];
+    p.rows_dm_total = rows_dm[p.m];
+  }
+  h2d(mx.tables, mx.blob.data(), bytes, s_);
+  if (!device) h2d(mx.stage_in, mx.host_in.data(), sizeof(float) * 2 * side, s_);
+  // one pass of the chain per run of at most GB_MIX_SHAPES sizes
+  const PlaneGeom base = fused_geom(g_, 0, g_.h, kslot_, kslot_);
+  struct Clear {  // mix_ is only set while a pass's launches are queued
+    MixPass** p;
+    ~Clear() { *p = nullptr; }
+  } clear{&mix_};
+  for (MixPass& p : passes) {
+    mix_ = &p;
+    PlaneGeomMix pg;
+    static_cast<PlaneGeom&>(pg) = base;
+    pg.mix = p.geom(0);
+    const auto rows = [&](bool to_arena, float* const* ext, const int* row0, int total, float* arena, const char* name) {
+      if (total == 0) return;
+      note_launch(name, s_, static_cast<double>(total));
+      if (to_arena) {
+        k_mix_rows<true><<<cdiv(total, 8), 256, 0, s_>>>(ext, row0, arena, pg);
+      } else {
+        k_mix_rows<false><<<cdiv(total, 8), 256, 0, s_>>>(ext, row0, arena, pg);
+      }
+      note_launch_end(name, s_);
+    };
+    // PsychoImage of every original and its DiffPrecompute neighbour sums, then the Compare chain
+    rows(true, p.ext0, p.rows_rgb, p.rows_rgb_total, lin_, "mix_pack");
+    fused_opsin(lin_, xyb_, p.m, kslot_);
+    fused_separate(xyb_, ps0_, false, p.m, kslot_, kslot_);
+    fused_sup0(p.m, kslot_);
+    rows(true, p.ext1, p.rows_rgb, p.rows_rgb_total, lin_, "mix_pack");
+    fused_compare_launches(p.m, kslot_, kslot_);
+    if (diffmap != nullptr) rows(false, p.extdm, p.rows_dm, p.rows_dm_total, dm_, "mix_unpack");
+  }
+  // one transfer of the n maxima (float bits), which waits for everything queued before
+  std::vector<float> m(n);
+  d2h(m.data(), d_gmax_, sizeof(float) * n, s_);
+  for (int k = 0; k < n; ++k) maxima[order[k]] = m[k];
+  if (diffmap != nullptr && !device) {
+    std::vector<float> dm(dm_floats);
+    d2h(dm.data(), mx.stage_dm, sizeof(float) * dm_floats, s_);
+    for (int k = 0; k < n; ++k) {
+      const int i = order[k];
+      if (diffmap[i] != nullptr) memcpy(diffmap[i], &dm[at[k] / 3], sizeof(float) * w[i] * h[i]);
+    }
+  }
 }
 
 #endif  // !GB200_HOSTSIM

@@ -119,6 +119,19 @@ float border_scale(const std::vector<float>& taps, float weight_no_border, float
 
 }  // namespace
 
+std::vector<float> blur_axis_scales(int id, int n) {
+  float sigma, br;
+  blur_spec(id, &sigma, &br);
+  const std::vector<float> taps = make_blur_taps(sigma);
+  const int len = static_cast<int>(taps.size()), r = len / 2;
+  float weight_no_border = 0.0f;
+  for (int j = 0; j < len; ++j) weight_no_border += taps[j];
+  std::vector<float> sc(n, 0.0f);
+  for (int p = 0; p < n; ++p)
+    if (p < r || p + r >= n) sc[p] = border_scale(taps, weight_no_border, br, p, n);
+  return sc;
+}
+
 const float* upload_srgb_lin(Stream s, std::vector<void*>* owned, HostTables* host) {
   HostTables local;
   HostTables& ht = host ? *host : local;
@@ -199,11 +212,7 @@ Tables build_tables(int w, int h, Stream s, std::vector<void*>* owned, HostTable
     std::vector<float> taps_n = taps;
     for (int j = 0; j < len; ++j) taps_n[j] *= scale_no_border;
     ht.blur_taps_n[id] = taps_n;
-    std::vector<float> sx(w, 0.0f), sy(h, 0.0f);
-    for (int p = 0; p < w; ++p)
-      if (p < r || p + r >= w) sx[p] = border_scale(taps, weight_no_border, br, p, w);
-    for (int p = 0; p < h; ++p)
-      if (p < r || p + r >= h) sy[p] = border_scale(taps, weight_no_border, br, p, h);
+    const std::vector<float> sx = blur_axis_scales(id, w), sy = blur_axis_scales(id, h);
     t.blur[id].taps = upload(taps, s, owned);
     t.blur[id].taps_n = upload(taps_n, s, owned);
     t.blur[id].scale_x = upload(sx, s, owned);

@@ -76,6 +76,8 @@ struct HostTables {
 
 void blur_spec(int id, float* sigma, float* border_ratio);
 std::vector<float> make_blur_taps(float sigma);
+// BlurTab::scale_x / scale_y of blur `id` for an axis of length n (zero where the interior kernel applies)
+std::vector<float> blur_axis_scales(int id, int n);
 
 // Builds all tables for a w x h image and uploads them. Returns the device
 // allocations in *owned so the caller can free them.

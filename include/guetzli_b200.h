@@ -151,6 +151,20 @@ int gb200_butteraugli_batch_diffmap(gb200_butteraugli_batch* b, const float* rgb
  * nothing runs. */
 int gb200_butteraugli_batch_diffmap_device(gb200_butteraugli_batch* b, const float* rgb0_dev, const float* rgb1_dev,
                                            int n, float* diffmap_dev, double* score, void* stream);
+/* ButteraugliInterface per pair, pairs of different sizes: pair i is w[i] x h[i], 8 <= w[i] <= the batch's w,
+ * 8 <= h[i] <= its h; 1 <= n <= capacity.  w, h: host arrays [n].  rgb0[i], rgb1[i]: [3][h[i]][w[i]] in
+ * host memory; diffmap (may be NULL; entries may not be) [i]: [h[i]][w[i]]; score (may be NULL) [n].
+ * All pairs go through one pass of the Compare chain (several where the call has more than 16 distinct
+ * sizes), and each is bit for bit gb200_butteraugli_diffmap of that pair alone. */
+int gb200_butteraugli_batch_diffmap_sizes(gb200_butteraugli_batch* b, const int* w, const int* h,
+                                          const float* const* rgb0, const float* const* rgb1, int n,
+                                          float* const* diffmap, double* score);
+/* The same with every image and diffmap in device memory of the batch's device; stream as in
+ * gb200_butteraugli_batch_diffmap_device.  A host, managed or other device's pointer is refused, nothing
+ * runs. */
+int gb200_butteraugli_batch_diffmap_sizes_device(gb200_butteraugli_batch* b, const int* w, const int* h,
+                                                 const float* const* rgb0_dev, const float* const* rgb1_dev, int n,
+                                                 float* const* diffmap_dev, double* score, void* stream);
 void gb200_butteraugli_batch_destroy(gb200_butteraugli_batch* b);
 
 /* ---- 8-bit sRGB images, scored as the stand-alone `butteraugli` tool scores them ----

@@ -21,7 +21,19 @@ and four more take the same images as 8-bit sRGB (RGB, 3 bytes per pixel), conve
   batch_srgb_cuda, batch_srgb_host                       ButteraugliBatch.diffmap_srgb
   comparator_batch_srgb_cuda, comparator_batch_srgb_host  a comparator made by Comparator.from_srgb
 
-Their scores must equal their float twins' (scores_srgb_equal_float).  The result gains ms per pair or
+Their scores must equal their float twins' (scores_srgb_equal_float).
+
+With --sizes, pairs of different sizes are scored in sets (SIZE_SETS; "uniform" is a same-size set, for the
+mixed-size entry against the same-size one), ms per set, four or five ways:
+
+  sizes_cuda      one ButteraugliBatch (the set's largest width x height) and diffmap_sizes, CUDA tensors
+  sizes_host      the same with numpy arrays
+  grouped_cuda    one ButteraugliBatch per distinct size (made before timing), one diffmap call per size:
+                  the best a caller can do without diffmap_sizes
+  pairwise        one Comparator per pair, made, scored once and closed: scoring the pairs one by one
+  batch_cuda      ("uniform" only) the same-size entry on the same pairs
+
+A set larger than what one batch's arena holds goes in calls of --sizes-capacity pairs.  The result gains ms per pair or
 candidate of the batched modes, MPix/s (scored pixels per second) of every mode, and the device memory
 the batch and the batched comparators (RGB, and RGBA with its two originals) hold after creation and after
 their first 8-bit call (MiB, from torch.cuda.mem_get_info after gb200_trim_memory).  Every call returns once its diffmaps are written, so a host clock around `--n` calls is the
@@ -71,6 +83,11 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--device", type=int, default=0)
     ap.add_argument("--batch", type=int, default=0, help="pairs per call of the batch modes (0: no batch modes)")
+    ap.add_argument("--sizes", action="store_true", help="also time the mixed-size sets (SIZE_SETS)")
+    ap.add_argument("--sizes-only", action="store_true", help="time the mixed-size sets and nothing else")
+    ap.add_argument("--sizes-capacity", type=int, default=64,
+                    help="pairs per call of a set whose largest size is 1920x1080 (the arena of 256 such slots "
+                         "does not fit in 80 GB)")
     ap.add_argument("--out", default=None, help="also write the JSON result here")
     args = ap.parse_args()
 
@@ -81,6 +98,11 @@ def main():
     dev = torch.device("cuda", args.device)
     torch.cuda.set_device(dev)
 
+    if args.sizes_only:
+        result = {"sizes": bench_sizes(args, dev, torch)}
+        result.update(gpu_info(args.device))
+        emit(result, args.out)
+        return
     h, w = args.h, args.w
     base = synth.gradnoise(h, w, 11).astype(int)
     orig = linear(base.astype(np.uint8))
@@ -222,13 +244,110 @@ def main():
         # the 8-bit modes score the converted planes of the float modes' images
         result["scores_srgb_equal_float"] = all(scores[m] == scores[m.replace("_srgb", "")] for m in ms if "_srgb" in m)
         result["device_memory"] = memory
+    if args.sizes:
+        result["sizes"] = bench_sizes(args, dev, torch)
     result.update(gpu_info(args.device))
+    emit(result, args.out)
+
+
+def emit(result, out):
     line = json.dumps(result)
     print(line)
-    if args.out:
-        os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
-        with open(args.out, "w") as f:
+    if out:
+        os.makedirs(os.path.dirname(os.path.abspath(out)), exist_ok=True)
+        with open(out, "w") as f:
             f.write(line + "\n")
+
+
+def size_sets():
+    """name -> [(h, w) of each pair]"""
+    rng = np.random.default_rng(17)
+    return {
+        # Kodak-like: landscape and portrait 768x512 images mixed
+        "kodak": [(512, 768) if i % 3 else (768, 512) for i in range(24)],
+        # 256 pairs of random sizes from 32 to 256
+        "random": [(int(a), int(b)) for a, b in rng.integers(32, 257, size=(256, 2))],
+        # one 1920x1080 pair and 255 pairs of 64x64
+        "hd_small": [(1080, 1920)] + [(64, 64)] * 255,
+        # a same-size set: the mixed-size entry against the same-size one
+        "uniform": [(256, 256)] * 64,
+    }
+
+
+def bench_sizes(args, dev, torch):
+    out = {}
+    for name, shapes in size_sets().items():
+        n = len(shapes)
+        bh, bw = max(s[0] for s in shapes), max(s[1] for s in shapes)
+        cap = min(n, args.sizes_capacity) if bh * bw >= 1920 * 1080 else n
+        a, b = [], []
+        for i, (h, w) in enumerate(shapes):
+            u = synth.gradnoise(h, w, 100 + i).astype(int)
+            a.append(linear(u.astype(np.uint8)))
+            b.append(linear(np.clip(u + synth.noise(h, w, 900 + i) % 7 - 3, 0, 255).astype(np.uint8)))
+        a_dev = [torch.from_numpy(x).to(dev) for x in a]
+        b_dev = [torch.from_numpy(x).to(dev) for x in b]
+        batch = gb.ButteraugliBatch(bh, bw, cap, device=args.device)
+        groups = {}
+        for i, s in enumerate(shapes):
+            groups.setdefault(s, []).append(i)
+        per_size = {s: gb.ButteraugliBatch(s[0], s[1], len(ix), device=args.device) for s, ix in groups.items()}
+        stacked = {s: (torch.stack([a_dev[i] for i in ix]), torch.stack([b_dev[i] for i in ix]))
+                   for s, ix in groups.items()}
+        torch.cuda.synchronize(dev)
+
+        def in_calls(x, y):
+            scores = []
+            for k in range(0, n, cap):
+                scores += batch.diffmap_sizes(x[k:k + cap], y[k:k + cap])[1].tolist()
+            return scores
+
+        def sizes_cuda():
+            return in_calls(a_dev, b_dev)
+
+        def sizes_host():
+            return in_calls(a, b)
+
+        def grouped_cuda():
+            scores = [0.0] * n
+            for s, ix in groups.items():
+                for i, v in zip(ix, per_size[s].diffmap(*stacked[s])[1].tolist()):
+                    scores[i] = v
+            return scores
+
+        def pairwise():
+            scores = []
+            for i in range(n):
+                c = gb.Comparator(a[i], device=args.device)
+                scores.append(c.diffmap(b[i])[1])
+                c.close()
+            return scores
+
+        modes = {"sizes_cuda": sizes_cuda, "sizes_host": sizes_host, "grouped_cuda": grouped_cuda,
+                 "pairwise": pairwise}
+        if len(groups) == 1:
+            modes["batch_cuda"] = grouped_cuda  # one size: grouping is the same-size entry on all pairs
+            del modes["grouped_cuda"]
+        scores = {m: f() for m, f in modes.items()}  # also the warm-up
+        ms = {m: [] for m in modes}
+        for _ in range(args.rounds):
+            for m, f in modes.items():
+                torch.cuda.synchronize(dev)
+                t0 = time.perf_counter()
+                f()
+                torch.cuda.synchronize(dev)
+                ms[m].append((time.perf_counter() - t0) * 1e3)
+        batch.close()
+        for x in per_size.values():
+            x.close()
+        mpix = sum(h * w for h, w in shapes) / 1e6
+        out[name] = {"pairs": n, "distinct_sizes": len(groups), "batch": f"{bw}x{bh}", "capacity": cap,
+                     "mpix": round(mpix, 3),
+                     "ms_per_set": {m: {"median": round(statistics.median(v), 3), "min": round(min(v), 3),
+                                        "max": round(max(v), 3)} for m, v in ms.items()},
+                     "mpix_per_s": {m: round(mpix * 1e3 / statistics.median(v), 1) for m, v in ms.items()},
+                     "scores_identical": all(v == scores["sizes_cuda"] for v in scores.values())}
+    return out
 
 
 if __name__ == "__main__":
