@@ -122,6 +122,12 @@ def load_library(path=None):
                                                          C.c_void_p, C.c_void_p]
     lib.gb200_butteraugli_batch_diffmap_srgb_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                                                                 C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.gb200_butteraugli_batch_diffmap_sizes_srgb.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                               C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                                                               C.c_void_p]
+    lib.gb200_butteraugli_batch_diffmap_sizes_srgb_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p,
+                                                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                                                      C.c_void_p, C.c_void_p, C.c_void_p]
     lib.gb200_butteraugli_comparator_create_srgb.restype = C.c_void_p
     lib.gb200_butteraugli_comparator_create_srgb.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]
     lib.gb200_butteraugli_comparator_diffmap_srgb.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
@@ -647,6 +653,85 @@ class ButteraugliBatch:
             dm = np.empty((n, h, w), dtype=np.float32)
             ok = self.lib.gb200_butteraugli_batch_diffmap_srgb(self._h, a.ctypes.data, b.ctypes.data, n, ch,
                                                                dm.ctypes.data, score.ctypes.data)
+        if not ok:
+            raise RuntimeError(_err(self.lib))
+        return dm, score
+
+    def diffmap_sizes_srgb(self, img0s, img1s):
+        """diffmap_sizes for 8-bit sRGB pairs, each scored as butteraugli_srgb scores it: img0s, img1s
+        equal-length sequences (1 <= n <= capacity) of uint8 [h_i][w_i][C_i] with 8 <= h_i <= h,
+        8 <= w_i <= w and C_i = 3 (RGB) or 4 (RGBA), pair i the same shape on both sides; RGB and RGBA pairs
+        may share a call -> (list of n diffmaps float32 [h_i][w_i], scores float64 [n]).
+
+        The items are all numpy arrays (host memory, packed and uploaded once as bytes) or all CUDA tensors
+        on the batch's device, read in place after the work queued on its current torch stream; the diffmaps
+        come back the same kind.  As in diffmap_sizes(), a tensor on another device is refused by the C entry
+        (RuntimeError); malformed arguments raise ValueError."""
+        img0s, img1s = list(img0s), list(img1s)
+        n = len(img0s)
+        if len(img1s) != n:
+            raise ValueError(f"img0s and img1s differ in length: {n} and {len(img1s)}")
+        if not 1 <= n <= self.capacity:
+            raise ValueError(f"the batch takes 1..{self.capacity} pairs, got {n}")
+        items = img0s + img1s
+        cuda = _is_torch_tensor(items[0]) and items[0].is_cuda
+        if cuda:
+            import torch
+            dev = torch.device("cuda", self.device)
+        ptrs, shapes = [], []
+        for k, x in enumerate(items):  # one pass: a call may hold hundreds of small pairs
+            name = ("img0s", "img1s")[k // n]
+            if isinstance(x, np.ndarray):
+                if cuda:
+                    raise ValueError("the images must all be CUDA tensors or all host arrays")
+                if x.dtype != np.uint8:
+                    raise ValueError(f"{name}[{k % n}] must be uint8, got {x.dtype}")
+                contiguous = x.flags.c_contiguous
+                ptrs.append(x.ctypes.data)
+            elif _is_torch_tensor(x) and x.is_cuda:
+                if not cuda:
+                    raise ValueError("the images must all be CUDA tensors or all host arrays")
+                if x.dtype != torch.uint8:
+                    raise ValueError(f"{name}[{k % n}] must be uint8, got {x.dtype}")
+                contiguous = x.is_contiguous()
+                ptrs.append(x.data_ptr())
+            else:
+                raise ValueError(f"{name}[{k % n}] must be a numpy array or a CUDA tensor, got {type(x).__name__}")
+            shape = tuple(x.shape)
+            if len(shape) != 3:
+                raise ValueError(f"{name}[{k % n}] must be interleaved [h][w][C], got shape {shape}")
+            if shape[2] not in (3, 4):
+                raise ValueError(f"{name}[{k % n}] must have 3 (RGB) or 4 (RGBA) channels in its last axis, "
+                                 f"got shape {shape}")
+            if not contiguous:
+                raise ValueError(f"{name}[{k % n}] must be contiguous")
+            shapes.append(shape)
+        for i in range(n):
+            if shapes[i][2] != shapes[n + i][2]:
+                raise ValueError(f"pair {i}: different number of channels: {shapes[i][2]} and {shapes[n + i][2]}")
+            if shapes[i] != shapes[n + i]:
+                raise ValueError(f"pair {i} differs in shape: {shapes[i]} and {shapes[n + i]}")
+            h, w, _ = shapes[i]
+            if not (8 <= h <= self.h and 8 <= w <= self.w):
+                raise ValueError(f"pair {i} is {h}x{w}; the batch takes 8x8 up to {self.h}x{self.w} "
+                                 "(butteraugli_srgb scores smaller pairs)")
+        ws = np.array([s[1] for s in shapes[:n]], dtype=np.int32)
+        hs = np.array([s[0] for s in shapes[:n]], dtype=np.int32)
+        chs = np.array([s[2] for s in shapes[:n]], dtype=np.int32)
+        P = C.c_void_p * n
+        p0, p1 = P(*ptrs[:n]), P(*ptrs[n:])
+        score = np.empty(n, dtype=np.float64)
+        if cuda:
+            dm = [torch.empty(s[:2], dtype=torch.float32, device=dev) for s in shapes[:n]]
+            stream = torch.cuda.current_stream(dev).cuda_stream
+            ok = self.lib.gb200_butteraugli_batch_diffmap_sizes_srgb_device(
+                self._h, ws.ctypes.data, hs.ctypes.data, chs.ctypes.data, p0, p1, n, P(*[t.data_ptr() for t in dm]),
+                score.ctypes.data, stream)
+        else:
+            dm = [np.empty(s[:2], dtype=np.float32) for s in shapes[:n]]
+            ok = self.lib.gb200_butteraugli_batch_diffmap_sizes_srgb(
+                self._h, ws.ctypes.data, hs.ctypes.data, chs.ctypes.data, p0, p1, n, P(*[d.ctypes.data for d in dm]),
+                score.ctypes.data)
         if not ok:
             raise RuntimeError(_err(self.lib))
         return dm, score

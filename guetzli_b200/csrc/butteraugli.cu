@@ -426,6 +426,30 @@ void Butteraugli::compare_many_srgb(const uint8_t* img1, int n, int channels, Bu
   });
 }
 
+void Butteraugli::compare_batch_sizes_srgb(const int* w, const int* h, const int* channels,
+                                           const uint8_t* const* img0, const uint8_t* const* img1, int n,
+                                           float* const* diffmap, float* maxima, bool device, Stream caller) {
+  if (n < 1 || n > capacity_) throw std::runtime_error("butteraugli batch: n must be in 1..capacity");
+  for (int i = 0; i < n; ++i) {
+    if (w[i] < 8 || h[i] < 8 || w[i] > g_.w || h[i] > g_.h) throw std::runtime_error("butteraugli batch: pair size");
+    check_channels(channels[i]);
+  }
+  bind();
+#if !defined(GB200_HOSTSIM)
+  if (use_fused_) {
+    if (device) stream_wait(s_, caller);
+    fused_compare_sizes_srgb(w, h, channels, img0, img1, n, diffmap, maxima, device);
+    return;
+  }
+#endif
+  // the staged chain and the CPU port: one pair batch per pair, of the pair's size
+  for (int i = 0; i < n; ++i) {
+    Butteraugli pair(w[i], h[i], 1, device_, Slots::kPairs);
+    pair.compare_batch_srgb(img0[i], img1[i], 1, channels[i], diffmap != nullptr ? diffmap[i] : nullptr, &maxima[i],
+                            device, caller);
+  }
+}
+
 void Butteraugli::adaptive_quantization(const float* linear_rgb, float* quant) {
   bind();
   r_.upload_planes(linear_rgb, lin_, 3);

@@ -24,6 +24,7 @@ namespace gb200 {
 
 struct MixPass;  // one pass of a mixed-size call over the fused chain (pipeline.cu)
 struct MapReq;   // the tensor map argument of a fused launch (pipeline.cu)
+struct MixSrc;   // the images of a mixed-size run, float or 8-bit (pipeline.cu)
 
 struct KernelStat {
   std::string name;
@@ -207,6 +208,14 @@ class Butteraugli {
   // for channels 4, `white` is the metric of the same shape whose original it laid over white.
   void compare_many_srgb(const uint8_t* img1, int n, int channels, Butteraugli* white, float* diffmap,
                          float* maxima, bool device, Stream caller);
+  // compare_batch_sizes on 8-bit pairs: img0[i] / img1[i] interleaved [h[i]][w[i]][channels[i]], channels 3
+  // or 4 per pair; diffmap itself and its entries may be null.  The fused chain converts while it packs
+  // the images into the arena (k_mix_srgb): one run over all pairs laid over black, then one over the RGBA
+  // pairs alone laid over white, with passes of their own sizes.  The staged chain and the CPU port score
+  // each pair through compare_batch_srgb of a pair batch of its own size.
+  void compare_batch_sizes_srgb(const int* w, const int* h, const int* channels, const uint8_t* const* img0,
+                                const uint8_t* const* img1, int n, float* const* diffmap, float* maxima, bool device,
+                                Stream caller);
   // ButteraugliComparator::Mask (b/butteraugli.cc:793) of the original at every pixel, on the
   // host: mask, mask_dc [3][h][w].  Leaves the resident PsychoImage as it is.
   void mask(float* mask, float* mask_dc);
@@ -262,6 +271,12 @@ class Butteraugli {
   // compare_batch_sizes on the fused chain; its buffers and tables (allocated on the first call, kept)
   void fused_compare_sizes(const int* w, const int* h, const float* const* rgb0, const float* const* rgb1, int n,
                            float* const* diffmap, float* maxima, bool device);
+  void fused_compare_sizes_srgb(const int* w, const int* h, const int* channels, const uint8_t* const* img0,
+                                const uint8_t* const* img1, int n, float* const* diffmap, float* maxima, bool device);
+  // one run of mixed passes over `pairs` (indices into w, h and src's tables): diffmap of pair i into dst[i]
+  // (device memory, or null), its maximum into maxima[i]
+  void fused_mixed_run(const int* w, const int* h, const std::vector<int>& pairs, const MixSrc& src,
+                       float* const* dst, float* maxima);
   struct Mixed;
   Mixed* mixed_ = nullptr;
   MixPass* mix_ = nullptr;  // set while the launches of a mixed pass are queued

@@ -582,6 +582,57 @@ int batch_diffmap_srgb(gb200_butteraugli_batch* b, const uint8_t* img0, const ui
   });
 }
 
+// 8-bit pairs of different sizes: every argument is checked before anything is queued
+int batch_diffmap_sizes_srgb(gb200_butteraugli_batch* b, const int* w, const int* h, const int* channels,
+                             const uint8_t* const* img0, const uint8_t* const* img1, int n, float* const* diffmap,
+                             double* score, bool device, void* stream) {
+  if (b == nullptr || w == nullptr || h == nullptr || channels == nullptr || img0 == nullptr || img1 == nullptr) {
+    g_err = "butteraugli batch: no batch, no sizes, no channels or no images";
+    return 0;
+  }
+  if (n < 1 || n > b->ba->capacity()) {
+    g_err = "butteraugli batch: n = " + std::to_string(n) + " pairs, the batch takes 1.." +
+            std::to_string(b->ba->capacity());
+    return 0;
+  }
+  const int bw = b->ba->region().g.w, bh = b->ba->region().g.h;
+  for (int i = 0; i < n; ++i) {
+    const std::string pair = "butteraugli batch: pair " + std::to_string(i);
+    if (w[i] < 8 || h[i] < 8 || w[i] > bw || h[i] > bh) {
+      g_err = pair + " is " + std::to_string(w[i]) + "x" + std::to_string(h[i]) + ", the batch takes 8x8 up to " +
+              std::to_string(bw) + "x" + std::to_string(bh);
+      if (w[i] < 8 || h[i] < 8) g_err += " (gb200_butteraugli_diffmap_srgb scores smaller pairs)";
+      return 0;
+    }
+    if (!channels_ok(pair.c_str(), channels[i])) return 0;
+    if (img0[i] == nullptr || img1[i] == nullptr) {
+      g_err = pair + " has a null image pointer";
+      return 0;
+    }
+  }
+  return guarded([&]() {
+    b->ba->bind();
+    gb200::Stream caller = 0;
+    if (device) {
+      for (int i = 0; i < n; ++i) {
+        const void* ptrs[3] = {img0[i], img1[i], diffmap != nullptr ? diffmap[i] : nullptr};
+        const std::string k = "[" + std::to_string(i) + "]";
+        const std::string names[3] = {"img0" + k, "img1" + k, "diffmap" + k};
+        const char* what[3] = {names[0].c_str(), names[1].c_str(), names[2].c_str()};
+        check_device_pointers("butteraugli batch", b->ba->device(), ptrs, what, 3);
+      }
+#if !defined(GB200_HOSTSIM)
+      caller = static_cast<gb200::Stream>(stream);
+#endif
+    }
+    (void)stream;
+    std::vector<float> m(n);
+    b->ba->compare_batch_sizes_srgb(w, h, channels, img0, img1, n, diffmap, m.data(), device, caller);
+    if (score)
+      for (int i = 0; i < n; ++i) score[i] = m[i];
+  });
+}
+
 int comparator_diffmap_srgb(gb200_butteraugli_comparator* c, const uint8_t* img1, int n, float* diffmap, double* score,
                             bool device, void* stream) {
   if (c == nullptr || img1 == nullptr) {
@@ -623,6 +674,20 @@ int gb200_butteraugli_batch_diffmap_srgb_device(gb200_butteraugli_batch* b, cons
                                                 const uint8_t* img1_dev, int n, int channels, float* diffmap_dev,
                                                 double* score, void* stream) {
   return batch_diffmap_srgb(b, img0_dev, img1_dev, n, channels, diffmap_dev, score, true, stream);
+}
+
+int gb200_butteraugli_batch_diffmap_sizes_srgb(gb200_butteraugli_batch* b, const int* w, const int* h,
+                                               const int* channels, const uint8_t* const* img0,
+                                               const uint8_t* const* img1, int n, float* const* diffmap,
+                                               double* score) {
+  return batch_diffmap_sizes_srgb(b, w, h, channels, img0, img1, n, diffmap, score, false, nullptr);
+}
+
+int gb200_butteraugli_batch_diffmap_sizes_srgb_device(gb200_butteraugli_batch* b, const int* w, const int* h,
+                                                      const int* channels, const uint8_t* const* img0_dev,
+                                                      const uint8_t* const* img1_dev, int n,
+                                                      float* const* diffmap_dev, double* score, void* stream) {
+  return batch_diffmap_sizes_srgb(b, w, h, channels, img0_dev, img1_dev, n, diffmap_dev, score, true, stream);
 }
 
 gb200_butteraugli_comparator* gb200_butteraugli_comparator_create_srgb(const uint8_t* img0, int w, int h, int channels,

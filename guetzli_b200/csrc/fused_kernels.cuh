@@ -50,8 +50,9 @@ struct MixImage {
   int w, h;
   int shape;   // index of its tensor maps in the pass's map sets
   int sx, sy;  // offsets of its border scales (x, y) in the pass's scale table of a blur
-  int seg;     // rows of a rolling-blur segment (launch_roll's rule for h rows)
-  int pad[2];  // 32 bytes
+  int seg;       // rows of a rolling-blur segment (launch_roll's rule for h rows)
+  int channels;  // bytes per pixel of an 8-bit image (k_mix_srgb); 3 for float planes
+  int pad;       // 32 bytes
 };
 struct MixGeom {
   const MixImage* img;  // [m]
@@ -1300,6 +1301,22 @@ __global__ void __launch_bounds__(256) k_mix_rows(float* const* ext, const int* 
       e[x] = a[x];
     }
   }
+}
+
+// The same packing for 8-bit images, converted on the way (srgb_over_linear, over `background`): image j
+// has rows [row0[j], row0[j + 1]), h of them, of w pixels of MixImage::channels bytes at src[j].  Row y
+// is read once and written to row y of all three planes of arena slot n0 + j.  A warp per row, 8 rows
+// per block.
+__global__ void __launch_bounds__(256) k_mix_srgb(const uint8_t* const* src, const int* row0, int background,
+                                                  const float* lut, float* arena, PlaneGeomMix g) {
+  const int row = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (row >= __ldg(row0 + g.mix.m)) return;
+  const int j = mix_find(row0, g.mix.m, row);
+  const int w = g.mix.img[j].w, C = g.mix.img[j].channels;
+  const int y = row - __ldg(row0 + j);
+  float* a = arena + slot_offset(g, g.mix.n0 + j) + static_cast<size_t>(y) * g.pitch;
+  const uint8_t* s = src[j] + static_cast<size_t>(y) * w * C;
+  for (int x = lane; x < w; x += 32) srgb_over_linear(s + x * C, C, background, lut, a + x, g.plane);
 }
 
 }  // namespace gb200

@@ -73,11 +73,26 @@ struct LinearizeRgb {
   }
 };
 
-// The stand-alone `butteraugli` tool's input (FromSrgbToLinear, b/butteraugli_main.cc:239-281): u8 sRGB
-// images interleaved [n][h][w][C] -> linear planes [n][3][h][pitch].  C = 4: the pixel is laid over
-// `background` in sRGB space first, in integers: alpha 255 keeps it, alpha 0 gives the background,
-// any other alpha (v a + background (255 - a) + 127) / 255.  lut: Tables::srgb_lin, which equals the
-// tool's table once both are rounded to float.  Launched over w x n*h.
+// The stand-alone `butteraugli` tool's input pixel (FromSrgbToLinear, b/butteraugli_main.cc:239-281):
+// u8 p[0 .. C) -> linear o[0], o[plane], o[2 plane].  C = 4: the pixel is laid over `background` in sRGB
+// space first, in integers: alpha 255 keeps it, alpha 0 gives the background, any other alpha
+// (v a + background (255 - a) + 127) / 255.  lut: Tables::srgb_lin, which equals the tool's table once
+// both are rounded to float.
+GB_HD void srgb_over_linear(const uint8_t* p, int C, int background, const float* lut, float* o, size_t plane) {
+  const int a = C == 4 ? p[3] : 255;
+  for (int c = 0; c < 3; ++c) {
+    int v = p[c];
+    if (a == 0) {
+      v = background;
+    } else if (a != 255) {
+      v = (v * a + background * (255 - a) + 127) / 255;
+    }
+    o[c * plane] = lut[v];
+  }
+}
+
+// u8 sRGB images interleaved [n][h][w][C] -> linear planes [n][3][h][pitch], each pixel by
+// srgb_over_linear.  Launched over w x n*h.
 struct SrgbToLinear {
   const uint8_t* src;
   int C, background;
@@ -86,19 +101,9 @@ struct SrgbToLinear {
   const float* lut;
   GB_HD void operator()(int x, int yy) const {
     const int i = yy / h, y = yy - i * h;
-    const uint8_t* p = src + (static_cast<size_t>(yy) * w + x) * C;
-    const int a = C == 4 ? p[3] : 255;
     const size_t plane = static_cast<size_t>(h) * pitch;
-    float* o = dst + 3 * plane * i + static_cast<size_t>(y) * pitch + x;
-    for (int c = 0; c < 3; ++c) {
-      int v = p[c];
-      if (a == 0) {
-        v = background;
-      } else if (a != 255) {
-        v = (v * a + background * (255 - a) + 127) / 255;
-      }
-      o[c * plane] = lut[v];
-    }
+    srgb_over_linear(src + (static_cast<size_t>(yy) * w + x) * C, C, background, lut,
+                     dst + 3 * plane * i + static_cast<size_t>(y) * pitch + x, plane);
   }
 };
 

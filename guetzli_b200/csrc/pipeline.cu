@@ -80,12 +80,12 @@ struct MixPass {
   const int* tile0 = nullptr;  // [kMixKinds][m + 1]
   int total[kMixKinds];        // work items per tile shape
   BlurTab tab[kNumBlurs];      // border scales of the pass's sizes (MixImage::sx, sy index them)
-  const int* rows_rgb = nullptr;  // [m + 1] 3h rows per image
-  const int* rows_dm = nullptr;   // [m + 1] h rows per image
-  float* const* ext0 = nullptr;   // [m] rgb0 of each image (device memory)
-  float* const* ext1 = nullptr;
+  const int* rows_in = nullptr;   // [m + 1] rows per image packed: 3h of float planes, h of 8-bit pixels
+  const int* rows_dm = nullptr;   // [m + 1] h rows per image with a diffmap, 0 per image without
+  void* const* ext0 = nullptr;  // [m] first image of each pair (device memory: float or 8-bit)
+  void* const* ext1 = nullptr;
   float* const* extdm = nullptr;  // [m] diffmap of each image, or null
-  int rows_rgb_total = 0, rows_dm_total = 0;
+  int rows_in_total = 0, rows_dm_total = 0;
   std::deque<MixMaps> mapsets;  // the map sets of the launches queued so far (stable addresses)
   MixGeom geom(int kind) const { return MixGeom{img, tile0 + kind * (m + 1), m, n0}; }
 };
@@ -496,9 +496,10 @@ void Butteraugli::fused_compare_batch(const float* rgb0, const float* rgb1, int 
 }
 
 // ---- pairs of different sizes (compare_batch_sizes) ----
-// The buffers of the mixed calls, grown to the largest call so far and kept: the tables of a call
+// The buffers of the mixed calls, grown to the largest call so far and kept: the tables of a run
 // (images, work items, row counts, pointers and border scales of every pass, one upload), the staging
-// of host images and host diffmaps, and the border scales of every size seen (host libm, once per size).
+// of host images (float or 8-bit) and of diffmaps (host output; an 8-bit call's diffmaps over white), and
+// the border scales of every size seen (host libm, once per size).
 struct Butteraugli::Mixed {
   std::vector<unsigned char> blob;  // host image of `tables`
   void* tables = nullptr;
@@ -506,6 +507,9 @@ struct Butteraugli::Mixed {
   std::vector<float> host_in;  // host images, packed
   float* stage_in = nullptr;
   size_t stage_in_floats = 0;
+  std::vector<uint8_t> host_u8;  // host 8-bit images, packed
+  uint8_t* stage_u8 = nullptr;
+  size_t stage_u8_bytes = 0;
   float* stage_dm = nullptr;
   size_t stage_dm_floats = 0;
   std::map<std::pair<int, int>, std::vector<float> > scales;  // size -> [blur][w + h] (scale_x, then scale_y)
@@ -515,6 +519,7 @@ void Butteraugli::mixed_release() {
   if (mixed_ == nullptr) return;
   dev_free(mixed_->tables);
   dev_free(mixed_->stage_in);
+  dev_free(mixed_->stage_u8);
   dev_free(mixed_->stage_dm);
   delete mixed_;
   mixed_ = nullptr;
@@ -534,21 +539,151 @@ T* grow(T* p, size_t* have, size_t want) {
 size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 }  // namespace
 
+// The images of a mixed run, per pair index, in memory of this device: float planes [3][h][w] (f), or 8-bit
+// pixels [h][w][channels] (u8) laid over `background`.
+struct MixSrc {
+  const float* const* f[2] = {nullptr, nullptr};
+  const uint8_t* const* u8[2] = {nullptr, nullptr};
+  const int* channels = nullptr;
+  int background = 0;
+};
+
 void Butteraugli::fused_compare_sizes(const int* w, const int* h, const float* const* rgb0, const float* const* rgb1,
                                       int n, float* const* diffmap, float* maxima, bool device) {
   if (mixed_ == nullptr) mixed_ = new Mixed();
   Mixed& mx = *mixed_;
+  std::vector<int> all(n);
+  std::vector<const float*> p0(rgb0, rgb0 + n), p1(rgb1, rgb1 + n);
+  std::vector<float*> dst(n, nullptr);
+  std::vector<size_t> at(n);  // pixels before pair i, in the staging of one side
+  size_t px = 0;
+  for (int i = 0; i < n; ++i) {
+    all[i] = i;
+    at[i] = px;
+    px += static_cast<size_t>(w[i]) * h[i];
+  }
+  if (!device) {  // host images: packed once, uploaded in one copy, rgb0 then rgb1 of every pair
+    mx.stage_in = grow(mx.stage_in, &mx.stage_in_floats, 6 * px);
+    mx.host_in.resize(6 * px);
+    for (int i = 0; i < n; ++i) {
+      const size_t img = static_cast<size_t>(3) * w[i] * h[i];
+      memcpy(&mx.host_in[3 * at[i]], rgb0[i], sizeof(float) * img);
+      memcpy(&mx.host_in[3 * (px + at[i])], rgb1[i], sizeof(float) * img);
+      p0[i] = mx.stage_in + 3 * at[i];
+      p1[i] = mx.stage_in + 3 * (px + at[i]);
+    }
+    h2d(mx.stage_in, mx.host_in.data(), sizeof(float) * 6 * px, s_);
+    if (diffmap != nullptr) mx.stage_dm = grow(mx.stage_dm, &mx.stage_dm_floats, px);
+  }
+  if (diffmap != nullptr)
+    for (int i = 0; i < n; ++i) dst[i] = device ? diffmap[i] : mx.stage_dm + at[i];
+  MixSrc src;
+  src.f[0] = p0.data();
+  src.f[1] = p1.data();
+  fused_mixed_run(w, h, all, src, dst.data(), maxima);
+  if (diffmap != nullptr && !device) {
+    std::vector<float> dm(px);
+    d2h(dm.data(), mx.stage_dm, sizeof(float) * px, s_);
+    for (int i = 0; i < n; ++i)
+      if (diffmap[i] != nullptr) memcpy(diffmap[i], &dm[at[i]], sizeof(float) * w[i] * h[i]);
+  }
+}
+
+void Butteraugli::fused_compare_sizes_srgb(const int* w, const int* h, const int* channels,
+                                           const uint8_t* const* img0, const uint8_t* const* img1, int n,
+                                           float* const* diffmap, float* maxima, bool device) {
+  if (mixed_ == nullptr) mixed_ = new Mixed();
+  Mixed& mx = *mixed_;
+  if (t_.srgb_lin == nullptr) t_.srgb_lin = upload_srgb_lin(s_, &owned_, nullptr);
+  std::vector<int> all(n), rgba;
+  std::vector<const uint8_t*> p0(img0, img0 + n), p1(img1, img1 + n);
+  // diffmap staging: host output, black's diffmaps of every pair, then white's of the RGBA pairs with a
+  // diffmap; device output, white's alone (black's go to the caller's memory)
+  std::vector<size_t> at(n), at_white(n);
+  size_t px = 0, px_white = 0, bytes = 0;
+  for (int i = 0; i < n; ++i) {
+    all[i] = i;
+    at[i] = px;
+    px += static_cast<size_t>(w[i]) * h[i];
+    bytes += static_cast<size_t>(w[i]) * h[i] * channels[i];
+    if (channels[i] != 4) continue;
+    rgba.push_back(i);
+    if (diffmap != nullptr && diffmap[i] != nullptr) {
+      at_white[i] = px_white;
+      px_white += static_cast<size_t>(w[i]) * h[i];
+    }
+  }
+  if (!device) {  // host images: packed once as bytes, uploaded in one copy for both backgrounds
+    mx.stage_u8 = grow(mx.stage_u8, &mx.stage_u8_bytes, 2 * bytes);
+    mx.host_u8.resize(2 * bytes);
+    size_t o = 0;
+    for (int i = 0; i < n; ++i) {
+      const size_t img = static_cast<size_t>(w[i]) * h[i] * channels[i];
+      memcpy(&mx.host_u8[o], img0[i], img);
+      memcpy(&mx.host_u8[bytes + o], img1[i], img);
+      p0[i] = mx.stage_u8 + o;
+      p1[i] = mx.stage_u8 + bytes + o;
+      o += img;
+    }
+    h2d(mx.stage_u8, mx.host_u8.data(), 2 * bytes, s_);
+  }
+  const size_t black = diffmap != nullptr && !device ? px : 0;
+  if (black + px_white > 0) mx.stage_dm = grow(mx.stage_dm, &mx.stage_dm_floats, black + px_white);
+  std::vector<float*> dst(n, nullptr), dst_white(n, nullptr);
+  if (diffmap != nullptr)
+    for (int i = 0; i < n; ++i) {
+      if (diffmap[i] == nullptr) continue;
+      dst[i] = device ? diffmap[i] : mx.stage_dm + at[i];
+      if (channels[i] == 4) dst_white[i] = mx.stage_dm + black + at_white[i];
+    }
+  MixSrc src;
+  src.u8[0] = p0.data();
+  src.u8[1] = p1.data();
+  src.channels = channels;
+  fused_mixed_run(w, h, all, src, dst.data(), maxima);
+  // RGBA pairs over white: a run of their own (their sizes make its passes); where white scores strictly
+  // higher, its score and diffmap win (a tie keeps black, butteraugli_main.cc:414)
+  std::vector<char> white_won(n, 0);
+  if (!rgba.empty()) {
+    std::vector<float> m_white(n);
+    src.background = 255;
+    fused_mixed_run(w, h, rgba, src, dst_white.data(), m_white.data());
+    bool copied = false;
+    for (int i : rgba) {
+      if (!(m_white[i] > maxima[i])) continue;
+      maxima[i] = m_white[i];
+      white_won[i] = 1;
+      if (device && dst_white[i] != nullptr) {
+        d2d(diffmap[i], dst_white[i], sizeof(float) * w[i] * h[i], s_);
+        copied = true;
+      }
+    }
+    if (copied) stream_sync(s_);  // the white diffmaps copied into the caller's memory
+  }
+  if (diffmap != nullptr && !device) {
+    std::vector<float> dm(black + px_white);
+    d2h(dm.data(), mx.stage_dm, sizeof(float) * dm.size(), s_);
+    for (int i = 0; i < n; ++i)
+      if (diffmap[i] != nullptr)
+        memcpy(diffmap[i], &dm[white_won[i] ? black + at_white[i] : at[i]], sizeof(float) * w[i] * h[i]);
+  }
+}
+
+void Butteraugli::fused_mixed_run(const int* w, const int* h, const std::vector<int>& pairs, const MixSrc& src,
+                                  float* const* dst, float* maxima) {
+  Mixed& mx = *mixed_;
+  const bool u8 = src.u8[0] != nullptr;
   // The per-size caches (border scales here, tensor maps in Fused::maps) are bounded: once they hold more
-  // than kMixCachedSizes sizes, a call starts by dropping them.  No launch of an earlier call reads them
-  // any more (its maps went into its launch parameters), and this call rebuilds what it uses.
+  // than kMixCachedSizes sizes, a run starts by dropping them.  No launch of an earlier run reads them
+  // any more (its maps went into its launch parameters), and this run rebuilds what it uses.
   constexpr size_t kMixCachedSizes = 256;
   if (mx.scales.size() > kMixCachedSizes) {
     mx.scales.clear();
     fused_->drop_other_sizes(g_);
   }
   // Slots in the order of the sizes, so that a pass (at most GB_MIX_SHAPES sizes) is a run of slots.
-  std::vector<int> order(n);
-  for (int i = 0; i < n; ++i) order[i] = i;
+  const int n = static_cast<int>(pairs.size());
+  std::vector<int> order(pairs);
   std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return std::make_pair(w[a], h[a]) < std::make_pair(w[b], h[b]); });
   std::vector<MixPass> passes;
   for (int k = 0; k < n; ++k) {
@@ -562,27 +697,9 @@ void Butteraugli::fused_compare_sizes(const int* w, const int* h, const float* c
     if (new_size) p.shapes.push_back(sz);
     ++p.m;
   }
-  // Host images: packed once, uploaded in one copy, rgb0 then rgb1 of every pair in slot order.
-  std::vector<size_t> at(n);  // floats before pair k's rgb0 (slot order), in the staging of one side
-  size_t side = 0, dm_floats = 0;
-  for (int k = 0; k < n; ++k) {
-    at[k] = side;
-    side += static_cast<size_t>(3) * w[order[k]] * h[order[k]];
-    dm_floats += static_cast<size_t>(w[order[k]]) * h[order[k]];
-  }
-  if (!device) {
-    mx.stage_in = grow(mx.stage_in, &mx.stage_in_floats, 2 * side);
-    mx.host_in.resize(2 * side);
-    for (int k = 0; k < n; ++k) {
-      const size_t img = static_cast<size_t>(3) * w[order[k]] * h[order[k]];
-      memcpy(&mx.host_in[at[k]], rgb0[order[k]], sizeof(float) * img);
-      memcpy(&mx.host_in[side + at[k]], rgb1[order[k]], sizeof(float) * img);
-    }
-    if (diffmap != nullptr) mx.stage_dm = grow(mx.stage_dm, &mx.stage_dm_floats, dm_floats);
-  }
   // The tables of every pass, laid out in one blob (offsets first, pointers filled once it has an address).
   struct Layout {
-    size_t img, tile0, rows_rgb, rows_dm, ext0, ext1, extdm, scales, blur_len;
+    size_t img, tile0, rows_in, rows_dm, ext0, ext1, extdm, scales, blur_len;
   };
   std::vector<Layout> lay(passes.size());
   size_t bytes = 0;
@@ -596,14 +713,14 @@ void Butteraugli::fused_compare_sizes(const int* w, const int* h, const float* c
     bytes += sizeof(MixImage) * p.m;
     l.tile0 = bytes = align_up(bytes, 16);
     bytes += sizeof(int) * kMixKinds * (p.m + 1);
-    l.rows_rgb = bytes;
+    l.rows_in = bytes;
     bytes += sizeof(int) * (p.m + 1);
     l.rows_dm = bytes;
     bytes += sizeof(int) * (p.m + 1);
     l.ext0 = bytes = align_up(bytes, 16);
-    bytes += sizeof(float*) * p.m;
+    bytes += sizeof(void*) * p.m;
     l.ext1 = bytes;
-    bytes += sizeof(float*) * p.m;
+    bytes += sizeof(void*) * p.m;
     l.extdm = bytes;
     bytes += sizeof(float*) * p.m;
     l.scales = bytes = align_up(bytes, 16);
@@ -622,10 +739,10 @@ void Butteraugli::fused_compare_sizes(const int* w, const int* h, const float* c
     unsigned char* b = mx.blob.data();
     MixImage* img = reinterpret_cast<MixImage*>(b + l.img);
     int* tile0 = reinterpret_cast<int*>(b + l.tile0);
-    int* rows_rgb = reinterpret_cast<int*>(b + l.rows_rgb);
+    int* rows_in = reinterpret_cast<int*>(b + l.rows_in);
     int* rows_dm = reinterpret_cast<int*>(b + l.rows_dm);
-    float** ext0 = reinterpret_cast<float**>(b + l.ext0);
-    float** ext1 = reinterpret_cast<float**>(b + l.ext1);
+    void** ext0 = reinterpret_cast<void**>(b + l.ext0);
+    void** ext1 = reinterpret_cast<void**>(b + l.ext1);
     float** extdm = reinterpret_cast<float**>(b + l.extdm);
     float* sc = reinterpret_cast<float*>(b + l.scales);
     // border scales: per blur, scale_x of every size, then scale_y of every size
@@ -657,10 +774,10 @@ void Butteraugli::fused_compare_sizes(const int* w, const int* h, const float* c
       p.tab[id].scale_x = p.tab[id].scale_y = reinterpret_cast<const float*>(dev + l.scales) + id * l.blur_len;
     }
     int shape = -1;
-    rows_rgb[0] = rows_dm[0] = 0;
+    rows_in[0] = rows_dm[0] = 0;
     for (int kind = 0; kind < kMixKinds; ++kind) tile0[kind * (p.m + 1)] = 0;
     for (int j = 0; j < p.m; ++j) {
-      const int slot = p.n0 + j, i = order[slot], iw = w[i], ih = h[i];
+      const int i = order[p.n0 + j], iw = w[i], ih = h[i];
       if (j == 0 || std::make_pair(iw, ih) != p.shapes[shape]) ++shape;
       MixImage& im = img[j];
       im.w = iw;
@@ -669,6 +786,7 @@ void Butteraugli::fused_compare_sizes(const int* w, const int* h, const float* c
       im.sx = sxo[shape];
       im.sy = syo[shape];
       im.seg = roll_seg(ih);
+      im.channels = u8 ? src.channels[i] : 3;
       for (int kind = 0; kind < kMixKinds; ++kind) {
         const int th = kTile[kind][1] ? kTile[kind][1] : im.seg;
         const long long items = static_cast<long long>(cdiv(iw, kTile[kind][0])) * cdiv(ih, th) * kTile[kind][2];
@@ -676,31 +794,28 @@ void Butteraugli::fused_compare_sizes(const int* w, const int* h, const float* c
         if (t[j] + items > 0x7fffffffLL) throw std::runtime_error("butteraugli batch: too many tiles in one call");
         t[j + 1] = t[j] + static_cast<int>(items);
       }
-      rows_rgb[j + 1] = rows_rgb[j] + 3 * ih;
-      rows_dm[j + 1] = rows_dm[j] + ih;
-      if (device) {
-        ext0[j] = const_cast<float*>(rgb0[i]);
-        ext1[j] = const_cast<float*>(rgb1[i]);
-        extdm[j] = diffmap != nullptr ? diffmap[i] : nullptr;
-      } else {
-        ext0[j] = mx.stage_in + at[slot];
-        ext1[j] = mx.stage_in + side + at[slot];
-        extdm[j] = diffmap != nullptr ? mx.stage_dm + (at[slot] / 3) : nullptr;
+      // packing rows: 3h plane rows of float planes, h pixel rows of 8-bit images; unpacking: h rows of
+      // the images with a diffmap
+      rows_in[j + 1] = rows_in[j] + (u8 ? ih : 3 * ih);
+      rows_dm[j + 1] = rows_dm[j] + (dst[i] != nullptr ? ih : 0);
+      for (int side = 0; side < 2; ++side) {
+        void* e = u8 ? static_cast<void*>(const_cast<uint8_t*>(src.u8[side][i])) : const_cast<float*>(src.f[side][i]);
+        (side ? ext1 : ext0)[j] = e;
       }
+      extdm[j] = dst[i];
     }
     p.img = reinterpret_cast<const MixImage*>(dev + l.img);
     p.tile0 = reinterpret_cast<const int*>(dev + l.tile0);
-    p.rows_rgb = reinterpret_cast<const int*>(dev + l.rows_rgb);
+    p.rows_in = reinterpret_cast<const int*>(dev + l.rows_in);
     p.rows_dm = reinterpret_cast<const int*>(dev + l.rows_dm);
-    p.ext0 = reinterpret_cast<float* const*>(dev + l.ext0);
-    p.ext1 = reinterpret_cast<float* const*>(dev + l.ext1);
+    p.ext0 = reinterpret_cast<void* const*>(dev + l.ext0);
+    p.ext1 = reinterpret_cast<void* const*>(dev + l.ext1);
     p.extdm = reinterpret_cast<float* const*>(dev + l.extdm);
     for (int kind = 0; kind < kMixKinds; ++kind) p.total[kind] = tile0[kind * (p.m + 1) + p.m];
-    p.rows_rgb_total = rows_rgb[p.m];
+    p.rows_in_total = rows_in[p.m];
     p.rows_dm_total = rows_dm[p.m];
   }
   h2d(mx.tables, mx.blob.data(), bytes, s_);
-  if (!device) h2d(mx.stage_in, mx.host_in.data(), sizeof(float) * 2 * side, s_);
   // one pass of the chain per run of at most GB_MIX_SHAPES sizes
   const PlaneGeom base = fused_geom(g_, 0, g_.h, kslot_, kslot_);
   struct Clear {  // mix_ is only set while a pass's launches are queued
@@ -712,37 +827,37 @@ void Butteraugli::fused_compare_sizes(const int* w, const int* h, const float* c
     PlaneGeomMix pg;
     static_cast<PlaneGeom&>(pg) = base;
     pg.mix = p.geom(0);
-    const auto rows = [&](bool to_arena, float* const* ext, const int* row0, int total, float* arena, const char* name) {
-      if (total == 0) return;
-      note_launch(name, s_, static_cast<double>(total));
-      if (to_arena) {
-        k_mix_rows<true><<<cdiv(total, 8), 256, 0, s_>>>(ext, row0, arena, pg);
+    // one side's images into the lin planes of the pass's slots
+    const auto pack = [&](void* const* ext) {
+      const int total = p.rows_in_total;
+      if (u8) {
+        note_launch("mix_pack_srgb", s_, static_cast<double>(total));
+        k_mix_srgb<<<cdiv(total, 8), 256, 0, s_>>>(reinterpret_cast<const uint8_t* const*>(ext), p.rows_in,
+                                                   src.background, t_.srgb_lin, lin_, pg);
+        note_launch_end("mix_pack_srgb", s_);
       } else {
-        k_mix_rows<false><<<cdiv(total, 8), 256, 0, s_>>>(ext, row0, arena, pg);
+        note_launch("mix_pack", s_, static_cast<double>(total));
+        k_mix_rows<true><<<cdiv(total, 8), 256, 0, s_>>>(reinterpret_cast<float* const*>(ext), p.rows_in, lin_, pg);
+        note_launch_end("mix_pack", s_);
       }
-      note_launch_end(name, s_);
     };
     // PsychoImage of every original and its DiffPrecompute neighbour sums, then the Compare chain
-    rows(true, p.ext0, p.rows_rgb, p.rows_rgb_total, lin_, "mix_pack");
+    pack(p.ext0);
     fused_opsin(lin_, xyb_, p.m, kslot_);
     fused_separate(xyb_, ps0_, false, p.m, kslot_, kslot_);
     fused_sup0(p.m, kslot_);
-    rows(true, p.ext1, p.rows_rgb, p.rows_rgb_total, lin_, "mix_pack");
+    pack(p.ext1);
     fused_compare_launches(p.m, kslot_, kslot_);
-    if (diffmap != nullptr) rows(false, p.extdm, p.rows_dm, p.rows_dm_total, dm_, "mix_unpack");
+    if (p.rows_dm_total > 0) {
+      note_launch("mix_unpack", s_, static_cast<double>(p.rows_dm_total));
+      k_mix_rows<false><<<cdiv(p.rows_dm_total, 8), 256, 0, s_>>>(p.extdm, p.rows_dm, dm_, pg);
+      note_launch_end("mix_unpack", s_);
+    }
   }
   // one transfer of the n maxima (float bits), which waits for everything queued before
   std::vector<float> m(n);
   d2h(m.data(), d_gmax_, sizeof(float) * n, s_);
   for (int k = 0; k < n; ++k) maxima[order[k]] = m[k];
-  if (diffmap != nullptr && !device) {
-    std::vector<float> dm(dm_floats);
-    d2h(dm.data(), mx.stage_dm, sizeof(float) * dm_floats, s_);
-    for (int k = 0; k < n; ++k) {
-      const int i = order[k];
-      if (diffmap[i] != nullptr) memcpy(diffmap[i], &dm[at[k] / 3], sizeof(float) * w[i] * h[i]);
-    }
-  }
 }
 
 #endif  // !GB200_HOSTSIM

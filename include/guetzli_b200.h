@@ -191,6 +191,24 @@ int gb200_butteraugli_batch_diffmap_srgb(gb200_butteraugli_batch* b, const uint8
 int gb200_butteraugli_batch_diffmap_srgb_device(gb200_butteraugli_batch* b, const uint8_t* img0_dev,
                                                 const uint8_t* img1_dev, int n, int channels, float* diffmap_dev,
                                                 double* score, void* stream);
+/* gb200_butteraugli_batch_diffmap_sizes on 8-bit pairs: pair i is w[i] x h[i] with channels[i] (3 or 4), 8 <=
+ * w[i] <= the batch's w, 8 <= h[i] <= its h (gb200_butteraugli_diffmap_srgb scores smaller pairs); RGB and
+ * RGBA pairs may share a call.  w, h, channels: host arrays [n].  img0[i], img1[i]: [h[i]][w[i]][channels[i]]
+ * in host memory, packed and uploaded once as bytes whatever the channels.  diffmap (may be NULL, and so may
+ * its entries) [i]: [h[i]][w[i]]; score (may be NULL) [n].  Each pair is bit for bit
+ * gb200_butteraugli_diffmap_srgb of that pair alone.  The bytes are converted as the Compare chain packs them;
+ * RGBA pairs are scored over black with the RGB pairs, then over white in passes of their own. */
+int gb200_butteraugli_batch_diffmap_sizes_srgb(gb200_butteraugli_batch* b, const int* w, const int* h,
+                                               const int* channels, const uint8_t* const* img0,
+                                               const uint8_t* const* img1, int n, float* const* diffmap,
+                                               double* score);
+/* The same with every image and diffmap in device memory of the batch's device, read in place; stream as in
+ * gb200_butteraugli_batch_diffmap_device.  A host, managed or other device's pointer is refused, nothing
+ * runs. */
+int gb200_butteraugli_batch_diffmap_sizes_srgb_device(gb200_butteraugli_batch* b, const int* w, const int* h,
+                                                      const int* channels, const uint8_t* const* img0_dev,
+                                                      const uint8_t* const* img1_dev, int n,
+                                                      float* const* diffmap_dev, double* score, void* stream);
 /* A comparator (gb200_butteraugli_comparator_create_batch) whose original img0 [h][w][channels] is given
  * in host memory, at least 8x8; 1 <= capacity <= 16383.  With channels 4 it keeps two resident
  * originals, over black and over white.  It takes 8-bit candidates with its own channels only (the

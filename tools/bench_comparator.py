@@ -33,6 +33,17 @@ mixed-size entry against the same-size one), ms per set, four or five ways:
   pairwise        one Comparator per pair, made, scored once and closed: scoring the pairs one by one
   batch_cuda      ("uniform" only) the same-size entry on the same pairs
 
+and each float mode of the mixed-size entry is followed by its 8-bit twin on the same images as RGB bytes:
+
+  sizes_srgb_cuda ButteraugliBatch.diffmap_sizes_srgb, uint8 CUDA tensors
+  sizes_srgb_host the same with numpy arrays
+
+The set "kodak_rgba" has Kodak-like shapes with alpha on half the pairs.  Its float modes score the pairs
+over black and the RGBA pairs over white as well, and keep the larger score (black on a tie), as the 8-bit
+entry does; grouping and pairwise scoring are not timed there.  Per set, the result reports whether the
+8-bit scores equal the float scores (scores_srgb_equal_float) and the device memory the batch holds after
+creation and what its first 8-bit mixed call adds.
+
 A set larger than what one batch's arena holds goes in calls of --sizes-capacity pairs.  The result gains ms per pair or
 candidate of the batched modes, MPix/s (scored pixels per second) of every mode, and the device memory
 the batch and the batched comparators (RGB, and RGBA with its two originals) hold after creation and after
@@ -259,6 +270,16 @@ def emit(result, out):
             f.write(line + "\n")
 
 
+def over(img, bg):
+    """uint8 [h][w][4] laid over the background bg in sRGB space, in integers, as the butteraugli tool does
+    (butteraugli_main.cc:264-275) -> [h][w][3]; [h][w][3] as it is."""
+    if img.shape[2] == 3:
+        return img
+    rgb, al = img[..., :3].astype(int), img[..., 3:].astype(int)
+    v = (rgb * al + bg * (255 - al) + 127) // 255
+    return np.where(al == 255, rgb, np.where(al == 0, bg, v)).astype(np.uint8)
+
+
 def size_sets():
     """name -> [(h, w) of each pair]"""
     rng = np.random.default_rng(17)
@@ -271,6 +292,8 @@ def size_sets():
         "hd_small": [(1080, 1920)] + [(64, 64)] * 255,
         # a same-size set: the mixed-size entry against the same-size one
         "uniform": [(256, 256)] * 64,
+        # the Kodak-like shapes with alpha on every other pair
+        "kodak_rgba": [(512, 768) if i % 3 else (768, 512) for i in range(24)],
     }
 
 
@@ -280,33 +303,73 @@ def bench_sizes(args, dev, torch):
         n = len(shapes)
         bh, bw = max(s[0] for s in shapes), max(s[1] for s in shapes)
         cap = min(n, args.sizes_capacity) if bh * bw >= 1920 * 1080 else n
-        a, b = [], []
+        alpha = name.endswith("_rgba")
+        u0, u1 = [], []  # the 8-bit images
         for i, (h, w) in enumerate(shapes):
             u = synth.gradnoise(h, w, 100 + i).astype(int)
-            a.append(linear(u.astype(np.uint8)))
-            b.append(linear(np.clip(u + synth.noise(h, w, 900 + i) % 7 - 3, 0, 255).astype(np.uint8)))
+            v = np.clip(u + synth.noise(h, w, 900 + i) % 7 - 3, 0, 255).astype(np.uint8)
+            u = u.astype(np.uint8)
+            if alpha and i % 2:  # every alpha value; the candidate's alpha as the original's
+                al = (synth.noise(h, w, 500 + i)[..., :1].astype(int) * 37 % 256).astype(np.uint8)
+                u, v = np.concatenate([u, al], axis=2), np.concatenate([v, al], axis=2)
+            u0.append(u)
+            u1.append(v)
+        rgba = [i for i in range(n) if u0[i].shape[2] == 4]
+        # the float images: the pairs over black, and the RGBA pairs over white
+        a, b = [linear(over(x, 0)) for x in u0], [linear(over(x, 0)) for x in u1]
+        aw, bw_ = [linear(over(u0[i], 255)) for i in rgba], [linear(over(u1[i], 255)) for i in rgba]
         a_dev = [torch.from_numpy(x).to(dev) for x in a]
         b_dev = [torch.from_numpy(x).to(dev) for x in b]
+        aw_dev = [torch.from_numpy(x).to(dev) for x in aw]
+        bw_dev = [torch.from_numpy(x).to(dev) for x in bw_]
+        u0_dev = [torch.from_numpy(x).to(dev) for x in u0]
+        u1_dev = [torch.from_numpy(x).to(dev) for x in u1]
+        torch.cuda.synchronize(dev)
+
+        def free_mib():
+            gb.load_library().gb200_trim_memory()
+            torch.cuda.synchronize(dev)
+            return torch.cuda.mem_get_info(dev)[0] / 2**20
+
+        f0 = free_mib()
         batch = gb.ButteraugliBatch(bh, bw, cap, device=args.device)
+        f1 = free_mib()
+        batch.diffmap_sizes_srgb(u0[:cap], u1[:cap])
+        f2 = free_mib()
         groups = {}
         for i, s in enumerate(shapes):
             groups.setdefault(s, []).append(i)
-        per_size = {s: gb.ButteraugliBatch(s[0], s[1], len(ix), device=args.device) for s, ix in groups.items()}
+        timed_groups = {} if alpha else groups  # the RGBA set times no grouping
+        per_size = {s: gb.ButteraugliBatch(s[0], s[1], len(ix), device=args.device) for s, ix in timed_groups.items()}
         stacked = {s: (torch.stack([a_dev[i] for i in ix]), torch.stack([b_dev[i] for i in ix]))
-                   for s, ix in groups.items()}
+                   for s, ix in timed_groups.items()}
         torch.cuda.synchronize(dev)
 
-        def in_calls(x, y):
+        def in_calls(f, x, y):
             scores = []
-            for k in range(0, n, cap):
-                scores += batch.diffmap_sizes(x[k:k + cap], y[k:k + cap])[1].tolist()
+            for k in range(0, len(x), cap):
+                scores += f(x[k:k + cap], y[k:k + cap])[1].tolist()
+            return scores
+
+        def with_white(x, y, xw, yw):
+            """the float scores over black, and for the RGBA pairs the larger one (black on a tie)"""
+            scores = in_calls(batch.diffmap_sizes, x, y)
+            if rgba:
+                for i, v in zip(rgba, in_calls(batch.diffmap_sizes, xw, yw)):
+                    scores[i] = v if v > scores[i] else scores[i]
             return scores
 
         def sizes_cuda():
-            return in_calls(a_dev, b_dev)
+            return with_white(a_dev, b_dev, aw_dev, bw_dev)
+
+        def sizes_srgb_cuda():
+            return in_calls(batch.diffmap_sizes_srgb, u0_dev, u1_dev)
 
         def sizes_host():
-            return in_calls(a, b)
+            return with_white(a, b, aw, bw_)
+
+        def sizes_srgb_host():
+            return in_calls(batch.diffmap_sizes_srgb, u0, u1)
 
         def grouped_cuda():
             scores = [0.0] * n
@@ -323,9 +386,11 @@ def bench_sizes(args, dev, torch):
                 c.close()
             return scores
 
-        modes = {"sizes_cuda": sizes_cuda, "sizes_host": sizes_host, "grouped_cuda": grouped_cuda,
-                 "pairwise": pairwise}
-        if len(groups) == 1:
+        modes = {"sizes_cuda": sizes_cuda, "sizes_srgb_cuda": sizes_srgb_cuda, "sizes_host": sizes_host,
+                 "sizes_srgb_host": sizes_srgb_host, "grouped_cuda": grouped_cuda, "pairwise": pairwise}
+        if alpha:
+            del modes["grouped_cuda"], modes["pairwise"]
+        elif len(groups) == 1:
             modes["batch_cuda"] = grouped_cuda  # one size: grouping is the same-size entry on all pairs
             del modes["grouped_cuda"]
         scores = {m: f() for m, f in modes.items()}  # also the warm-up
@@ -346,7 +411,11 @@ def bench_sizes(args, dev, torch):
                      "ms_per_set": {m: {"median": round(statistics.median(v), 3), "min": round(min(v), 3),
                                         "max": round(max(v), 3)} for m, v in ms.items()},
                      "mpix_per_s": {m: round(mpix * 1e3 / statistics.median(v), 1) for m, v in ms.items()},
-                     "scores_identical": all(v == scores["sizes_cuda"] for v in scores.values())}
+                     "scores_identical": all(v == scores["sizes_cuda"] for m, v in scores.items() if "_srgb" not in m),
+                     "scores_srgb_equal_float": all(v == scores[m.replace("_srgb", "")] for m, v in scores.items()
+                                                    if "_srgb" in m),
+                     "rgba_pairs": len(rgba),
+                     "device_memory": {"batch_mib": round(f0 - f1, 1), "sizes_srgb_buffers_mib": round(f1 - f2, 1)}}
     return out
 
 
