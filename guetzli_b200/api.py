@@ -90,6 +90,9 @@ def load_library(path=None):
     lib.gb200_counters.argtypes = [P(C.c_long), P(C.c_longlong), P(C.c_longlong)]
     lib.gb200_profile_enable.argtypes = [C.c_int]
     lib.gb200_profile_get.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
+    lib.gb200_debug_read_jpeg.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t]
+    lib.gb200_butteraugli_diffmap.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                              P(C.c_double)]
     lib.gb200_butteraugli_comparator_create.restype = C.c_void_p
     lib.gb200_butteraugli_comparator_create.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int]
     lib.gb200_butteraugli_comparator_diffmap.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, P(C.c_double)]
@@ -142,6 +145,53 @@ def _err(lib):
     return (lib.gb200_last_error() or b"").decode(errors="replace")
 
 
+def _raise_device_error(lib):
+    """A failed encode without output: the device's failures raise, the reference's own (bad input,
+    no JPEG found) are returned as (False, b"") as guetzli::Process returns them."""
+    msg = _err(lib)
+    if "CUDA" in msg or "no CUDA device" in msg or "out of memory" in msg:
+        raise RuntimeError(msg)
+
+
+def _cparams(params):
+    return _CParams(params.butteraugli_target, int(params.clear_metadata), int(params.try_420),
+                    int(params.force_420), int(params.use_silver_screen),
+                    int(params.zeroing_greedy_lookahead), int(params.new_zeroing_model))
+
+
+def _take(lib, out, out_len):
+    data = C.string_at(out, out_len.value) if out_len.value else b""
+    if out:
+        lib.gb200_free(out)
+    return data
+
+
+def _log_sink(stats):
+    """The C log callback feeding stats.debug_output and stats.debug_output_file; null when neither is set."""
+    if stats is None or (stats.debug_output is None and stats.debug_output_file is None):
+        return C.cast(None, _LOG_FN)
+
+    def _sink(_user, text):
+        s = text.decode(errors="replace")
+        if stats.debug_output is not None:
+            stats.debug_output.append(s)
+        if stats.debug_output_file is not None:
+            stats.debug_output_file.write(s)
+
+    return _LOG_FN(_sink)
+
+
+def _fill_stats(stats, cs, directions=True):
+    """The counters of an encode into stats (if not None); directions: the up and down iterations as well."""
+    if stats is None:
+        return
+    stats.counters["number of iterations"] = cs.iterations
+    if directions:
+        stats.counters["number of iterations up"] = cs.iterations_up
+        stats.counters["number of iterations down"] = cs.iterations_down
+    stats.device = {k: getattr(cs, k) for k, _ in _CStats._fields_}
+
+
 @dataclass
 class Params:
     """guetzli::Params (guetzli/processor.h:29-37)."""
@@ -183,36 +233,15 @@ def process(params, stats, rgb, w, h, device=0, lib=None):
         import sys
         sys.stderr.write("Could not create jpg data from rgb pixels\n")
         return False, b""
-    cp = _CParams(params.butteraugli_target, int(params.clear_metadata), int(params.try_420),
-                  int(params.force_420), int(params.use_silver_screen),
-                  int(params.zeroing_greedy_lookahead), int(params.new_zeroing_model))
-    cs = _CStats()
-    want_log = stats is not None and (stats.debug_output is not None or stats.debug_output_file is not None)
-
-    def _sink(_user, text):
-        s = text.decode(errors="replace")
-        if stats.debug_output is not None:
-            stats.debug_output.append(s)
-        if stats.debug_output_file is not None:
-            stats.debug_output_file.write(s)
-
-    cb = _LOG_FN(_sink) if want_log else C.cast(None, _LOG_FN)
-    out = C.POINTER(C.c_uint8)()
-    out_len = C.c_size_t()
+    cp, cs = _cparams(params), _CStats()
+    cb = _log_sink(stats)
+    out, out_len = C.POINTER(C.c_uint8)(), C.c_size_t()
     ok = lib.gb200_process_rgb(C.byref(cp), buf.ctypes.data, w, h, device, cb, None,
                                C.byref(out), C.byref(out_len), C.byref(cs))
-    data = C.string_at(out, out_len.value) if out_len.value else b""
-    if out:
-        lib.gb200_free(out)
-    if stats is not None:
-        stats.counters["number of iterations"] = cs.iterations
-        stats.counters["number of iterations up"] = cs.iterations_up
-        stats.counters["number of iterations down"] = cs.iterations_down
-        stats.device = {k: getattr(cs, k) for k, _ in _CStats._fields_}
+    data = _take(lib, out, out_len)
+    _fill_stats(stats, cs)
     if not ok and not data:
-        msg = _err(lib)
-        if "CUDA" in msg or "no CUDA device" in msg or "out of memory" in msg:
-            raise RuntimeError(msg)
+        _raise_device_error(lib)
     return bool(ok), data
 
 
@@ -222,31 +251,14 @@ def process_jpeg(params, stats, jpeg_in, device=0, lib=None):
     lib = lib or load_library()
     buf = np.frombuffer(bytes(jpeg_in), dtype=np.uint8)
     cp, cs = _cparams(params), _CStats()
-    want_log = stats is not None and (stats.debug_output is not None or stats.debug_output_file is not None)
-
-    def _sink(_user, text):
-        s = text.decode(errors="replace")
-        if stats.debug_output is not None:
-            stats.debug_output.append(s)
-        if stats.debug_output_file is not None:
-            stats.debug_output_file.write(s)
-
-    cb = _LOG_FN(_sink) if want_log else C.cast(None, _LOG_FN)
+    cb = _log_sink(stats)
     out, out_len = C.POINTER(C.c_uint8)(), C.c_size_t()
     ok = lib.gb200_process_jpeg(C.byref(cp), buf.ctypes.data if buf.size else None, buf.size, device, cb, None,
                                 C.byref(out), C.byref(out_len), C.byref(cs))
-    data = C.string_at(out, out_len.value) if out_len.value else b""
-    if out:
-        lib.gb200_free(out)
-    if stats is not None:
-        stats.counters["number of iterations"] = cs.iterations
-        stats.counters["number of iterations up"] = cs.iterations_up
-        stats.counters["number of iterations down"] = cs.iterations_down
-        stats.device = {k: getattr(cs, k) for k, _ in _CStats._fields_}
+    data = _take(lib, out, out_len)
+    _fill_stats(stats, cs)
     if not ok and not data:
-        msg = _err(lib)
-        if "CUDA" in msg or "no CUDA device" in msg or "out of memory" in msg:
-            raise RuntimeError(msg)
+        _raise_device_error(lib)
     return bool(ok), data
 
 
@@ -257,7 +269,6 @@ def read_jpeg(jpeg_in, lib=None):
     dims = (C.c_int * 11)()
     cap = 1 << 24
     out = np.zeros(cap, dtype=np.int16)
-    lib.gb200_debug_read_jpeg.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t]
     ok = lib.gb200_debug_read_jpeg(buf.ctypes.data, buf.size, dims, out.ctypes.data, cap)
     d = list(dims)
     n = sum(d[3 + 2 * c] * d[4 + 2 * c] * 64 for c in range(d[2])) if ok else 0
@@ -276,16 +287,43 @@ def butteraugli_diffmap(rgb0, rgb1, device=0, lib=None):
     _, h, w = a.shape
     dm = np.zeros((h, w), dtype=np.float32)
     score = C.c_double()
-    lib.gb200_butteraugli_diffmap.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p,
-                                              C.POINTER(C.c_double)]
     if not lib.gb200_butteraugli_diffmap(a.ctypes.data, b.ctypes.data, w, h, device, dm.ctypes.data, C.byref(score)):
         raise RuntimeError(_err(lib))
     return dm, score.value
 
 
+class _Handle:
+    """Owns one C object of `lib`, destroyed by the C function named _destroy on close() or collection."""
+    _destroy = None
+    _h = None
+
+    def close(self):
+        if self._h:
+            getattr(self.lib, self._destroy)(self._h)
+            self._h = None
+
+    def __del__(self):
+        self.close()
+
+    def _ck(self, ok):
+        if not ok:
+            raise RuntimeError(_err(self.lib))
+
+
 def _is_torch_tensor(x):
     # without importing torch: a caller that passes a tensor has imported it already
     return type(x).__module__.split(".")[0] == "torch"
+
+
+def _outputs(device, shapes):
+    """float32 outputs of the given shapes: CUDA tensors on the torch device `device`, or host arrays where
+    it is None -> (outputs, their pointers, the device's current torch stream or None)."""
+    if device is None:
+        out = [np.empty(s, dtype=np.float32) for s in shapes]
+        return out, [o.ctypes.data for o in out], None
+    import torch
+    out = [torch.empty(s, dtype=torch.float32, device=device) for s in shapes]
+    return out, [o.data_ptr() for o in out], torch.cuda.current_stream(device).cuda_stream
 
 
 def _srgb_images(name, x, ranks, cuda_ok=True):
@@ -334,7 +372,7 @@ def butteraugli_srgb(img0, img1, device=0, lib=None):
     return dm, score.value
 
 
-class Comparator:
+class Comparator(_Handle):
     """butteraugli::ButteraugliComparator (butteraugli.h:425) on one GPU: the original rgb0, planar
     linear RGB float32 [3][h][w], nominally in 0..255 and at least 8x8, stays resident and is scored
     against any number of images, up to `capacity` (1..16383) of them per diffmap() call in one pass of
@@ -342,20 +380,18 @@ class Comparator:
     them, bit for bit; this is tested from -300 to 4500.  NaN and infinities must not be passed: the
     reference's result is undefined for them."""
 
+    _destroy = "gb200_butteraugli_comparator_destroy"
+
     def __init__(self, rgb0, device=0, capacity=1, lib=None):
         self.lib = lib or load_library()
-        self._h = None
         self.channels = 0  # made from float planes
         a = np.ascontiguousarray(rgb0, dtype=np.float32)
         if a.ndim != 3 or a.shape[0] != 3:
             raise ValueError(f"rgb0 must be planar [3][h][w], got shape {a.shape}")
         _, self.h, self.w = a.shape
         self.device, self.capacity = device, int(capacity)
-        if self.capacity == 1:
-            self._h = self.lib.gb200_butteraugli_comparator_create(a.ctypes.data, self.w, self.h, device)
-        else:
-            self._h = self.lib.gb200_butteraugli_comparator_create_batch(a.ctypes.data, self.w, self.h,
-                                                                         self.capacity, device)
+        self._h = self.lib.gb200_butteraugli_comparator_create_batch(a.ctypes.data, self.w, self.h, self.capacity,
+                                                                     device)
         if not self._h:
             raise RuntimeError("gb200_butteraugli_comparator_create failed: " + _err(self.lib))
 
@@ -367,7 +403,6 @@ class Comparator:
         [n][h][w][C] with the same C, numpy or CUDA tensors, and nothing else; mask() refuses RGBA."""
         self = cls.__new__(cls)
         self.lib = lib or load_library()
-        self._h = None
         a, _ = _srgb_images("img0", img0, (3,), cuda_ok=False)
         self.h, self.w, self.channels = a.shape
         self.device, self.capacity = device, int(capacity)
@@ -376,18 +411,6 @@ class Comparator:
         if not self._h:
             raise RuntimeError("gb200_butteraugli_comparator_create_srgb failed: " + _err(self.lib))
         return self
-
-    def close(self):
-        if self._h:
-            self.lib.gb200_butteraugli_comparator_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        self.close()
-
-    def _ck(self, ok):
-        if not ok:
-            raise RuntimeError(_err(self.lib))
 
     def diffmap(self, rgb1):
         """ButteraugliComparator::Diffmap + ButteraugliScoreFromDiffmap -> (diffmap [h][w], score).
@@ -409,10 +432,9 @@ class Comparator:
         a = np.ascontiguousarray(rgb1, dtype=np.float32)
         if a.shape != (3, self.h, self.w):
             raise ValueError(f"rgb1 must have shape {(3, self.h, self.w)}, got {a.shape}")
-        dm = np.empty((self.h, self.w), dtype=np.float32)
+        [dm], [dp], _ = _outputs(None, [(self.h, self.w)])
         score = C.c_double()
-        self._ck(self.lib.gb200_butteraugli_comparator_diffmap(self._h, a.ctypes.data, dm.ctypes.data,
-                                                               C.byref(score)))
+        self._ck(self.lib.gb200_butteraugli_comparator_diffmap(self._h, a.ctypes.data, dp, C.byref(score)))
         return dm, score.value
 
     def _diffmap_device(self, t):
@@ -420,11 +442,10 @@ class Comparator:
         if t.dtype != torch.float32 or tuple(t.shape) != (3, self.h, self.w):
             raise ValueError(f"rgb1 must be float32 of shape {(3, self.h, self.w)}, got {t.dtype} {tuple(t.shape)}")
         t = t.contiguous()
-        dm = torch.empty((self.h, self.w), dtype=torch.float32, device=t.device)
+        [dm], [dp], stream = _outputs(t.device, [(self.h, self.w)])
         score = C.c_double()
-        stream = torch.cuda.current_stream(t.device).cuda_stream
-        self._ck(self.lib.gb200_butteraugli_comparator_diffmap_device(self._h, t.data_ptr(), dm.data_ptr(),
-                                                                      C.byref(score), stream))
+        self._ck(self.lib.gb200_butteraugli_comparator_diffmap_device(self._h, t.data_ptr(), dp, C.byref(score),
+                                                                      stream))
         return dm, score.value
 
     def _diffmap_batch(self, rgb1):
@@ -439,18 +460,16 @@ class Comparator:
             if rgb1.dtype != torch.float32:
                 raise ValueError(f"rgb1 must be float32, got {rgb1.dtype}")
             t = rgb1.contiguous()
-            dm = torch.empty((n, self.h, self.w), dtype=torch.float32, device=t.device)
-            stream = torch.cuda.current_stream(t.device).cuda_stream
-            self._ck(self.lib.gb200_butteraugli_comparator_diffmap_batch_device(self._h, t.data_ptr(), n, dm.data_ptr(),
+            [dm], [dp], stream = _outputs(t.device, [(n, self.h, self.w)])
+            self._ck(self.lib.gb200_butteraugli_comparator_diffmap_batch_device(self._h, t.data_ptr(), n, dp,
                                                                                 score.ctypes.data, stream))
             return dm, score
         a = np.asarray(rgb1)
         if a.dtype != np.float32:
             raise ValueError(f"rgb1 must be float32, got {a.dtype}")
         a = np.ascontiguousarray(a)
-        dm = np.empty((n, self.h, self.w), dtype=np.float32)
-        self._ck(self.lib.gb200_butteraugli_comparator_diffmap_batch(self._h, a.ctypes.data, n, dm.ctypes.data,
-                                                                     score.ctypes.data))
+        [dm], [dp], _ = _outputs(None, [(n, self.h, self.w)])
+        self._ck(self.lib.gb200_butteraugli_comparator_diffmap_batch(self._h, a.ctypes.data, n, dp, score.ctypes.data))
         return dm, score
 
     def _diffmap_srgb(self, img1):
@@ -462,15 +481,12 @@ class Comparator:
             raise ValueError(f"img1 must have shape [{self.h}, {self.w}, {self.channels}] or [n, {self.h}, {self.w}, "
                              f"{self.channels}] with 1 <= n <= {self.capacity}, got {tuple(x.shape)}")
         score = np.empty(n, dtype=np.float64)
+        [dm], [dp], stream = _outputs(x.device if cuda else None, [(n, self.h, self.w)])
         if cuda:
-            import torch
-            dm = torch.empty((n, self.h, self.w), dtype=torch.float32, device=x.device)
-            stream = torch.cuda.current_stream(x.device).cuda_stream
-            self._ck(self.lib.gb200_butteraugli_comparator_diffmap_srgb_device(self._h, x.data_ptr(), n, dm.data_ptr(),
+            self._ck(self.lib.gb200_butteraugli_comparator_diffmap_srgb_device(self._h, x.data_ptr(), n, dp,
                                                                                score.ctypes.data, stream))
         else:
-            dm = np.empty((n, self.h, self.w), dtype=np.float32)
-            self._ck(self.lib.gb200_butteraugli_comparator_diffmap_srgb(self._h, x.ctypes.data, n, dm.ctypes.data,
+            self._ck(self.lib.gb200_butteraugli_comparator_diffmap_srgb(self._h, x.ctypes.data, n, dp,
                                                                         score.ctypes.data))
         return (dm[0], float(score[0])) if single else (dm, score)
 
@@ -482,7 +498,7 @@ class Comparator:
         return m, mdc
 
 
-class ButteraugliBatch:
+class ButteraugliBatch(_Handle):
     """butteraugli::ButteraugliInterface on up to `capacity` same-size pairs per call, on one GPU: each
     pair (rgb0[i], rgb1[i]) is scored as gb.butteraugli_diffmap scores it alone, bit for bit, with the
     pairs going through the Compare chain together.  Images are planar linear RGB float32, nominally in
@@ -490,21 +506,14 @@ class ButteraugliBatch:
     them, bit for bit; this is tested from -300 to 4500.  NaN and infinities must not be passed: the
     reference's result is undefined for them."""
 
+    _destroy = "gb200_butteraugli_batch_destroy"
+
     def __init__(self, h, w, capacity, device=0, lib=None):
         self.lib = lib or load_library()
-        self._h = None
         self.h, self.w, self.capacity, self.device = int(h), int(w), int(capacity), device
         self._h = self.lib.gb200_butteraugli_batch_create(self.w, self.h, self.capacity, device)
         if not self._h:
             raise RuntimeError("gb200_butteraugli_batch_create failed: " + _err(self.lib))
-
-    def close(self):
-        if self._h:
-            self.lib.gb200_butteraugli_batch_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        self.close()
 
     def _shape_of(self, shape):
         if len(shape) != 4 or tuple(shape[1:]) != (3, self.h, self.w) or not 1 <= shape[0] <= self.capacity:
@@ -530,11 +539,10 @@ class ButteraugliBatch:
             raise ValueError(f"rgb0 and rgb1 differ in shape: {a.shape} and {b.shape}")
         n = self._shape_of(a.shape)
         a, b = np.ascontiguousarray(a), np.ascontiguousarray(b)
-        dm = np.empty((n, self.h, self.w), dtype=np.float32)
+        [dm], [dp], _ = _outputs(None, [(n, self.h, self.w)])
         score = np.empty(n, dtype=np.float64)
-        if not self.lib.gb200_butteraugli_batch_diffmap(self._h, a.ctypes.data, b.ctypes.data, n, dm.ctypes.data,
-                                                        score.ctypes.data):
-            raise RuntimeError(_err(self.lib))
+        self._ck(self.lib.gb200_butteraugli_batch_diffmap(self._h, a.ctypes.data, b.ctypes.data, n, dp,
+                                                          score.ctypes.data))
         return dm, score
 
     def _diffmap_device(self, t0, t1):
@@ -547,13 +555,56 @@ class ButteraugliBatch:
             raise ValueError(f"rgb0 and rgb1 are on different devices: {t0.device} and {t1.device}")
         n = self._shape_of(tuple(t0.shape))
         t0, t1 = t0.contiguous(), t1.contiguous()
-        dm = torch.empty((n, self.h, self.w), dtype=torch.float32, device=t0.device)
+        [dm], [dp], stream = _outputs(t0.device, [(n, self.h, self.w)])
         score = np.empty(n, dtype=np.float64)
-        stream = torch.cuda.current_stream(t0.device).cuda_stream
-        if not self.lib.gb200_butteraugli_batch_diffmap_device(self._h, t0.data_ptr(), t1.data_ptr(), n, dm.data_ptr(),
-                                                               score.ctypes.data, stream):
-            raise RuntimeError(_err(self.lib))
+        self._ck(self.lib.gb200_butteraugli_batch_diffmap_device(self._h, t0.data_ptr(), t1.data_ptr(), n, dp,
+                                                                 score.ctypes.data, stream))
         return dm, score
+
+    def _sizes_items(self, names, items0, items1, dtype, shape_error):
+        """The images of a diffmap_sizes* call, checked in one pass (a call may hold hundreds of small
+        pairs): equal-length sequences named `names`, 1..capacity pairs, all numpy arrays or all CUDA
+        tensors, each of `dtype` ("float32" or "uint8"), contiguous, its shape passing shape_error (which
+        returns what is wrong with a shape, or None) -> (n, the batch's torch device for CUDA tensors or
+        None, pointers of items0 then items1, their shapes)."""
+        items0, items1 = list(items0), list(items1)
+        n = len(items0)
+        if len(items1) != n:
+            raise ValueError(f"{names[0]} and {names[1]} differ in length: {n} and {len(items1)}")
+        if not 1 <= n <= self.capacity:
+            raise ValueError(f"the batch takes 1..{self.capacity} pairs, got {n}")
+        items = items0 + items1
+        cuda = _is_torch_tensor(items[0]) and items[0].is_cuda
+        if cuda:
+            import torch
+            torch_dtype = getattr(torch, dtype)
+        ptrs, shapes = [], []
+        for k, x in enumerate(items):
+            name = names[k // n]
+            if isinstance(x, np.ndarray):
+                if cuda:
+                    raise ValueError("the images must all be CUDA tensors or all host arrays")
+                if x.dtype != dtype:
+                    raise ValueError(f"{name}[{k % n}] must be {dtype}, got {x.dtype}")
+                contiguous = x.flags.c_contiguous
+                ptrs.append(x.ctypes.data)
+            elif _is_torch_tensor(x) and x.is_cuda:
+                if not cuda:
+                    raise ValueError("the images must all be CUDA tensors or all host arrays")
+                if x.dtype != torch_dtype:
+                    raise ValueError(f"{name}[{k % n}] must be {dtype}, got {x.dtype}")
+                contiguous = x.is_contiguous()
+                ptrs.append(x.data_ptr())
+            else:
+                raise ValueError(f"{name}[{k % n}] must be a numpy array or a CUDA tensor, got {type(x).__name__}")
+            shape = tuple(x.shape)
+            wrong = shape_error(shape)
+            if wrong:
+                raise ValueError(f"{name}[{k % n}] {wrong}, got shape {shape}")
+            if not contiguous:
+                raise ValueError(f"{name}[{k % n}] must be contiguous")
+            shapes.append(shape)
+        return n, torch.device("cuda", self.device) if cuda else None, ptrs, shapes
 
     def diffmap_sizes(self, rgb0s, rgb1s):
         """Pairs of different sizes in one call: rgb0s, rgb1s equal-length sequences (1 <= n <= capacity) of
@@ -564,42 +615,9 @@ class ButteraugliBatch:
         the batch device's current torch stream; the diffmaps come back the same kind, CUDA tensors on the
         batch's device.  As in diffmap(), a tensor on another device is refused by the C entry (RuntimeError,
         naming the argument and its device); malformed arguments raise ValueError."""
-        rgb0s, rgb1s = list(rgb0s), list(rgb1s)
-        n = len(rgb0s)
-        if len(rgb1s) != n:
-            raise ValueError(f"rgb0s and rgb1s differ in length: {n} and {len(rgb1s)}")
-        if not 1 <= n <= self.capacity:
-            raise ValueError(f"the batch takes 1..{self.capacity} pairs, got {n}")
-        items = rgb0s + rgb1s
-        cuda = _is_torch_tensor(items[0]) and items[0].is_cuda
-        if cuda:
-            import torch
-            dev = torch.device("cuda", self.device)
-        ptrs, shapes = [], []
-        for k, x in enumerate(items):  # one pass: a call may hold hundreds of small pairs
-            name = ("rgb0s", "rgb1s")[k // n]
-            if isinstance(x, np.ndarray):
-                if cuda:
-                    raise ValueError("the images must all be CUDA tensors or all host arrays")
-                if x.dtype != np.float32:
-                    raise ValueError(f"{name}[{k % n}] must be float32, got {x.dtype}")
-                contiguous = x.flags.c_contiguous
-                ptrs.append(x.ctypes.data)
-            elif _is_torch_tensor(x) and x.is_cuda:
-                if not cuda:
-                    raise ValueError("the images must all be CUDA tensors or all host arrays")
-                if x.dtype != torch.float32:
-                    raise ValueError(f"{name}[{k % n}] must be float32, got {x.dtype}")
-                contiguous = x.is_contiguous()
-                ptrs.append(x.data_ptr())
-            else:
-                raise ValueError(f"{name}[{k % n}] must be a numpy array or a CUDA tensor, got {type(x).__name__}")
-            shape = tuple(x.shape)
-            if len(shape) != 3 or shape[0] != 3:
-                raise ValueError(f"{name}[{k % n}] must be planar [3][h][w], got shape {shape}")
-            if not contiguous:
-                raise ValueError(f"{name}[{k % n}] must be contiguous")
-            shapes.append(shape)
+        n, dev, ptrs, shapes = self._sizes_items(
+            ("rgb0s", "rgb1s"), rgb0s, rgb1s, "float32",
+            lambda s: "must be planar [3][h][w]" if len(s) != 3 or s[0] != 3 else None)
         for i in range(n):
             if shapes[i] != shapes[n + i]:
                 raise ValueError(f"pair {i} differs in shape: {shapes[i]} and {shapes[n + i]}")
@@ -609,20 +627,13 @@ class ButteraugliBatch:
         ws = np.array([s[2] for s in shapes[:n]], dtype=np.int32)
         hs = np.array([s[1] for s in shapes[:n]], dtype=np.int32)
         P = C.c_void_p * n
-        p0, p1 = P(*ptrs[:n]), P(*ptrs[n:])
+        dm, dps, stream = _outputs(dev, [s[1:] for s in shapes[:n]])
         score = np.empty(n, dtype=np.float64)
-        if cuda:
-            dm = [torch.empty(s[1:], dtype=torch.float32, device=dev) for s in shapes[:n]]
-            stream = torch.cuda.current_stream(dev).cuda_stream
-            ok = self.lib.gb200_butteraugli_batch_diffmap_sizes_device(
-                self._h, ws.ctypes.data, hs.ctypes.data, p0, p1, n, P(*[t.data_ptr() for t in dm]), score.ctypes.data,
-                stream)
+        args = (self._h, ws.ctypes.data, hs.ctypes.data, P(*ptrs[:n]), P(*ptrs[n:]), n, P(*dps), score.ctypes.data)
+        if dev is not None:
+            self._ck(self.lib.gb200_butteraugli_batch_diffmap_sizes_device(*args, stream))
         else:
-            dm = [np.empty(s[1:], dtype=np.float32) for s in shapes[:n]]
-            ok = self.lib.gb200_butteraugli_batch_diffmap_sizes(self._h, ws.ctypes.data, hs.ctypes.data, p0, p1, n,
-                                                                P(*[d.ctypes.data for d in dm]), score.ctypes.data)
-        if not ok:
-            raise RuntimeError(_err(self.lib))
+            self._ck(self.lib.gb200_butteraugli_batch_diffmap_sizes(*args))
         return dm, score
 
     def diffmap_srgb(self, img0, img1):
@@ -640,21 +651,16 @@ class ButteraugliBatch:
         if (h, w) != (self.h, self.w) or not 1 <= n <= self.capacity:
             raise ValueError(f"img0 and img1 must have shape [n, {self.h}, {self.w}, C] with 1 <= n <= "
                              f"{self.capacity}, got {tuple(a.shape)}")
+        if cuda0 and a.device != b.device:
+            raise ValueError(f"img0 and img1 are on different devices: {a.device} and {b.device}")
+        [dm], [dp], stream = _outputs(a.device if cuda0 else None, [(n, h, w)])
         score = np.empty(n, dtype=np.float64)
         if cuda0:
-            import torch
-            if a.device != b.device:
-                raise ValueError(f"img0 and img1 are on different devices: {a.device} and {b.device}")
-            dm = torch.empty((n, h, w), dtype=torch.float32, device=a.device)
-            stream = torch.cuda.current_stream(a.device).cuda_stream
-            ok = self.lib.gb200_butteraugli_batch_diffmap_srgb_device(self._h, a.data_ptr(), b.data_ptr(), n, ch,
-                                                                      dm.data_ptr(), score.ctypes.data, stream)
+            self._ck(self.lib.gb200_butteraugli_batch_diffmap_srgb_device(self._h, a.data_ptr(), b.data_ptr(), n, ch,
+                                                                          dp, score.ctypes.data, stream))
         else:
-            dm = np.empty((n, h, w), dtype=np.float32)
-            ok = self.lib.gb200_butteraugli_batch_diffmap_srgb(self._h, a.ctypes.data, b.ctypes.data, n, ch,
-                                                               dm.ctypes.data, score.ctypes.data)
-        if not ok:
-            raise RuntimeError(_err(self.lib))
+            self._ck(self.lib.gb200_butteraugli_batch_diffmap_srgb(self._h, a.ctypes.data, b.ctypes.data, n, ch, dp,
+                                                                   score.ctypes.data))
         return dm, score
 
     def diffmap_sizes_srgb(self, img0s, img1s):
@@ -667,45 +673,10 @@ class ButteraugliBatch:
         on the batch's device, read in place after the work queued on its current torch stream; the diffmaps
         come back the same kind.  As in diffmap_sizes(), a tensor on another device is refused by the C entry
         (RuntimeError); malformed arguments raise ValueError."""
-        img0s, img1s = list(img0s), list(img1s)
-        n = len(img0s)
-        if len(img1s) != n:
-            raise ValueError(f"img0s and img1s differ in length: {n} and {len(img1s)}")
-        if not 1 <= n <= self.capacity:
-            raise ValueError(f"the batch takes 1..{self.capacity} pairs, got {n}")
-        items = img0s + img1s
-        cuda = _is_torch_tensor(items[0]) and items[0].is_cuda
-        if cuda:
-            import torch
-            dev = torch.device("cuda", self.device)
-        ptrs, shapes = [], []
-        for k, x in enumerate(items):  # one pass: a call may hold hundreds of small pairs
-            name = ("img0s", "img1s")[k // n]
-            if isinstance(x, np.ndarray):
-                if cuda:
-                    raise ValueError("the images must all be CUDA tensors or all host arrays")
-                if x.dtype != np.uint8:
-                    raise ValueError(f"{name}[{k % n}] must be uint8, got {x.dtype}")
-                contiguous = x.flags.c_contiguous
-                ptrs.append(x.ctypes.data)
-            elif _is_torch_tensor(x) and x.is_cuda:
-                if not cuda:
-                    raise ValueError("the images must all be CUDA tensors or all host arrays")
-                if x.dtype != torch.uint8:
-                    raise ValueError(f"{name}[{k % n}] must be uint8, got {x.dtype}")
-                contiguous = x.is_contiguous()
-                ptrs.append(x.data_ptr())
-            else:
-                raise ValueError(f"{name}[{k % n}] must be a numpy array or a CUDA tensor, got {type(x).__name__}")
-            shape = tuple(x.shape)
-            if len(shape) != 3:
-                raise ValueError(f"{name}[{k % n}] must be interleaved [h][w][C], got shape {shape}")
-            if shape[2] not in (3, 4):
-                raise ValueError(f"{name}[{k % n}] must have 3 (RGB) or 4 (RGBA) channels in its last axis, "
-                                 f"got shape {shape}")
-            if not contiguous:
-                raise ValueError(f"{name}[{k % n}] must be contiguous")
-            shapes.append(shape)
+        n, dev, ptrs, shapes = self._sizes_items(
+            ("img0s", "img1s"), img0s, img1s, "uint8",
+            lambda s: ("must be interleaved [h][w][C]" if len(s) != 3 else
+                       "must have 3 (RGB) or 4 (RGBA) channels in its last axis" if s[2] not in (3, 4) else None))
         for i in range(n):
             if shapes[i][2] != shapes[n + i][2]:
                 raise ValueError(f"pair {i}: different number of channels: {shapes[i][2]} and {shapes[n + i][2]}")
@@ -719,21 +690,14 @@ class ButteraugliBatch:
         hs = np.array([s[0] for s in shapes[:n]], dtype=np.int32)
         chs = np.array([s[2] for s in shapes[:n]], dtype=np.int32)
         P = C.c_void_p * n
-        p0, p1 = P(*ptrs[:n]), P(*ptrs[n:])
+        dm, dps, stream = _outputs(dev, [s[:2] for s in shapes[:n]])
         score = np.empty(n, dtype=np.float64)
-        if cuda:
-            dm = [torch.empty(s[:2], dtype=torch.float32, device=dev) for s in shapes[:n]]
-            stream = torch.cuda.current_stream(dev).cuda_stream
-            ok = self.lib.gb200_butteraugli_batch_diffmap_sizes_srgb_device(
-                self._h, ws.ctypes.data, hs.ctypes.data, chs.ctypes.data, p0, p1, n, P(*[t.data_ptr() for t in dm]),
-                score.ctypes.data, stream)
-        else:
-            dm = [np.empty(s[:2], dtype=np.float32) for s in shapes[:n]]
-            ok = self.lib.gb200_butteraugli_batch_diffmap_sizes_srgb(
-                self._h, ws.ctypes.data, hs.ctypes.data, chs.ctypes.data, p0, p1, n, P(*[d.ctypes.data for d in dm]),
+        args = (self._h, ws.ctypes.data, hs.ctypes.data, chs.ctypes.data, P(*ptrs[:n]), P(*ptrs[n:]), n, P(*dps),
                 score.ctypes.data)
-        if not ok:
-            raise RuntimeError(_err(self.lib))
+        if dev is not None:
+            self._ck(self.lib.gb200_butteraugli_batch_diffmap_sizes_srgb_device(*args, stream))
+        else:
+            self._ck(self.lib.gb200_butteraugli_batch_diffmap_sizes_srgb(*args))
         return dm, score
 
 
@@ -762,19 +726,6 @@ def counters(lib=None):
     n, a, b = C.c_long(), C.c_longlong(), C.c_longlong()
     lib.gb200_counters(C.byref(n), C.byref(a), C.byref(b))
     return n.value, a.value, b.value
-
-
-def _cparams(params):
-    return _CParams(params.butteraugli_target, int(params.clear_metadata), int(params.try_420),
-                    int(params.force_420), int(params.use_silver_screen),
-                    int(params.zeroing_greedy_lookahead), int(params.new_zeroing_model))
-
-
-def _take(lib, out, out_len):
-    data = C.string_at(out, out_len.value) if out_len.value else b""
-    if out:
-        lib.gb200_free(out)
-    return data
 
 
 def process_tiled_threads(params, rgb, w, h, world, device=0, lib=None):
@@ -825,9 +776,7 @@ def process_tiled(params, stats, rgb, w, h, lib=None):
     ok = lib.gb200_process_rgb_tiled(C.byref(cp), buf.ctypes.data, w, h, C.cast(None, _LOG_FN), None,
                                      C.byref(out), C.byref(out_len), C.byref(cs))
     data = _take(lib, out, out_len)
-    if stats is not None:
-        stats.counters["number of iterations"] = cs.iterations
-        stats.device = {k: getattr(cs, k) for k, _ in _CStats._fields_}
+    _fill_stats(stats, cs, directions=False)
     if not ok and not data:
         raise RuntimeError(_err(lib))
     return bool(ok), data
@@ -837,18 +786,17 @@ def write_jpeg(coeffs, w, h, q, lib=None):
     lib = lib or load_library()
     coeffs = np.ascontiguousarray(coeffs, dtype=np.int16)
     q = np.ascontiguousarray(q, dtype=np.int32)
-    out = C.POINTER(C.c_uint8)()
-    out_len = C.c_size_t()
+    out, out_len = C.POINTER(C.c_uint8)(), C.c_size_t()
     if not lib.gb200_write_jpeg(coeffs.ctypes.data, w, h, q.ctypes.data, C.byref(out), C.byref(out_len)):
         raise RuntimeError(_err(lib))
-    data = C.string_at(out, out_len.value)
-    lib.gb200_free(out)
-    return data
+    return _take(lib, out, out_len)
 
 
-class DeviceImage:
+class DeviceImage(_Handle):
     """One image resident on one GPU (gb200_image_*): the reference's Comparator /
     OutputImage pair moved onto device memory.  Used by the parity tests."""
+
+    _destroy = "gb200_image_destroy"
 
     def __init__(self, rgb, device=0, lib=None, prepare=True):
         self.lib = lib or load_library()
@@ -859,17 +807,6 @@ class DeviceImage:
             raise RuntimeError("gb200_image_create failed: " + _err(self.lib))
         self.nblocks = self.lib.gb200_image_num_blocks(self._h)
 
-    def close(self):
-        if self._h:
-            self.lib.gb200_image_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        self.close()
-
-    def _ck(self, ok):
-        if not ok:
-            raise RuntimeError(_err(self.lib))
 
     def reset(self):
         """Forget the one-time results: the next process() repeats the whole job."""
@@ -877,22 +814,12 @@ class DeviceImage:
 
     def process(self, params, stats=None):
         """guetzli::Process on the resident image -> (ok, jpeg bytes)."""
-        cp = _CParams(params.butteraugli_target, int(params.clear_metadata), int(params.try_420),
-                      int(params.force_420), int(params.use_silver_screen),
-                      int(params.zeroing_greedy_lookahead), int(params.new_zeroing_model))
-        cs = _CStats()
-        out = C.POINTER(C.c_uint8)()
-        out_len = C.c_size_t()
+        cp, cs = _cparams(params), _CStats()
+        out, out_len = C.POINTER(C.c_uint8)(), C.c_size_t()
         ok = self.lib.gb200_image_process(self._h, C.byref(cp), C.cast(None, _LOG_FN), None,
                                           C.byref(out), C.byref(out_len), C.byref(cs))
-        data = C.string_at(out, out_len.value) if out_len.value else b""
-        if out:
-            self.lib.gb200_free(out)
-        if stats is not None:
-            stats.counters["number of iterations"] = cs.iterations
-            stats.counters["number of iterations up"] = cs.iterations_up
-            stats.counters["number of iterations down"] = cs.iterations_down
-            stats.device = {k: getattr(cs, k) for k, _ in _CStats._fields_}
+        data = _take(self.lib, out, out_len)
+        _fill_stats(stats, cs)
         if not ok and not data:
             raise RuntimeError("gb200_image_process failed: " + _err(self.lib))
         return bool(ok), data
@@ -923,12 +850,9 @@ class DeviceImage:
     def save_jpeg(self, q):
         """SaveToJpegData + WriteJpeg of the current candidate, entropy-coded and assembled on the device."""
         q = np.ascontiguousarray(q, dtype=np.int32)
-        out = C.POINTER(C.c_uint8)()
-        out_len = C.c_size_t()
+        out, out_len = C.POINTER(C.c_uint8)(), C.c_size_t()
         self._ck(self.lib.gb200_image_save_jpeg(self._h, q.ctypes.data, C.byref(out), C.byref(out_len)))
-        data = C.string_at(out, out_len.value)
-        self.lib.gb200_free(out)
-        return data
+        return _take(self.lib, out, out_len)
 
     def compare(self):
         d = C.c_float()

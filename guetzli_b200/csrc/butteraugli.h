@@ -26,6 +26,10 @@ struct MixPass;  // one pass of a mixed-size call over the fused chain (pipeline
 struct MapReq;   // the tensor map argument of a fused launch (pipeline.cu)
 struct MixSrc;   // the images of a mixed-size run, float or 8-bit (pipeline.cu)
 
+// The stand-alone tool's choice for an RGBA image scored over black and over white: white wins only
+// where it scores strictly higher; a tie keeps black (butteraugli_main.cc:414).
+inline bool white_wins(float white, float black) { return white > black; }
+
 struct KernelStat {
   std::string name;
   long launches;
@@ -268,11 +272,12 @@ class Butteraugli {
   void fused_sup0(int nimg, int kslot);
   // n pairs, or with rgb0 null n candidates against the resident original
   void fused_compare_batch(const float* rgb0, const float* rgb1, int n, float* diffmap, float* maxima);
-  // compare_batch_sizes on the fused chain; its buffers and tables (allocated on the first call, kept)
-  void fused_compare_sizes(const int* w, const int* h, const float* const* rgb0, const float* const* rgb1, int n,
-                           float* const* diffmap, float* maxima, bool device);
-  void fused_compare_sizes_srgb(const int* w, const int* h, const int* channels, const uint8_t* const* img0,
-                                const uint8_t* const* img1, int n, float* const* diffmap, float* maxima, bool device);
+  // n and the pair sizes of compare_batch_sizes*, which the C entries have checked with their messages
+  void check_sizes(const int* w, const int* h, int n) const;
+  // compare_batch_sizes (channels null: float planes) and compare_batch_sizes_srgb on the fused chain; its
+  // buffers and tables (allocated on the first call, kept)
+  void fused_compare_sizes(const int* w, const int* h, const int* channels, const void* const* in0,
+                           const void* const* in1, int n, float* const* diffmap, float* maxima, bool device);
   // one run of mixed passes over `pairs` (indices into w, h and src's tables): diffmap of pair i into dst[i]
   // (device memory, or null), its maximum into maxima[i]
   void fused_mixed_run(const int* w, const int* h, const std::vector<int>& pairs, const MixSrc& src,
