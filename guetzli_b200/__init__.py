@@ -8,9 +8,10 @@ behind Guetzli's own API surface.  See DESIGN.md / INTEGRATION.md.
 from .api import (Params, ProcessStats, process, process_jpeg, butteraugli_score_for_quality,
                   DeviceImage, load_library, library_path, write_jpeg, counters,
                   process_tiled_threads, process_tiled, dist_unique_id, dist_init, dist_shutdown,
-                  last_error, Comparator, ButteraugliBatch, adaptive_quantization, butteraugli_srgb)
+                  last_error, Comparator, ComparatorSet, ButteraugliBatch, adaptive_quantization,
+                  butteraugli_srgb)
 
 __all__ = ["Params", "ProcessStats", "process", "process_jpeg", "butteraugli_score_for_quality",
            "DeviceImage", "load_library", "library_path", "write_jpeg", "counters",
            "process_tiled_threads", "process_tiled", "dist_unique_id", "dist_init", "dist_shutdown", "last_error",
-           "Comparator", "ButteraugliBatch", "adaptive_quantization", "butteraugli_srgb"]
+           "Comparator", "ComparatorSet", "ButteraugliBatch", "adaptive_quantization", "butteraugli_srgb"]

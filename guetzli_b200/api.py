@@ -137,6 +137,18 @@ def load_library(path=None):
                                                               C.c_void_p]
     lib.gb200_butteraugli_comparator_diffmap_srgb_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
                                                                      C.c_void_p, C.c_void_p]
+    lib.gb200_butteraugli_comparator_set_create.restype = C.c_void_p
+    lib.gb200_butteraugli_comparator_set_create.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                                            C.c_int]
+    lib.gb200_butteraugli_comparator_set_create_srgb.restype = C.c_void_p
+    lib.gb200_butteraugli_comparator_set_create_srgb.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                                 C.c_int, C.c_int, C.c_int]
+    for name in ("", "_srgb"):
+        set_diffmap = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+        entry = "gb200_butteraugli_comparator_set_diffmap" + name
+        getattr(lib, entry).argtypes = set_diffmap
+        getattr(lib, entry + "_device").argtypes = set_diffmap + [C.c_void_p]
+    lib.gb200_butteraugli_comparator_set_destroy.argtypes = [C.c_void_p]
     _libs[path] = lib
     return lib
 
@@ -372,6 +384,66 @@ def butteraugli_srgb(img0, img1, device=0, lib=None):
     return dm, score.value
 
 
+def _planar_error(shape):
+    return "must be planar [3][h][w]" if len(shape) != 3 or shape[0] != 3 else None
+
+
+def _interleaved_error(shape):
+    if len(shape) != 3:
+        return "must be interleaved [h][w][C]"
+    return "must have 3 (RGB) or 4 (RGBA) channels in its last axis" if shape[2] not in (3, 4) else None
+
+
+def _sizes_items(names, seqs, n_error, dtype, shape_error, device, cuda_ok=True):
+    """The images of a call on images of sizes of their own, checked in one pass (a call may hold hundreds of
+    small images): equal-length sequences `seqs` named `names`, whose length passes n_error (which returns what
+    is wrong with it, or None), all numpy arrays or all CUDA tensors (numpy arrays only, where not cuda_ok),
+    each of `dtype` ("float32" or "uint8"), contiguous, its shape passing shape_error (which returns what is
+    wrong with a shape, or None) -> (n, the torch device `device` for CUDA tensors or None, the pointers of
+    every sequence in turn, their shapes)."""
+    seqs = [list(x) for x in seqs]
+    n = len(seqs[0])
+    for name, x in zip(names[1:], seqs[1:]):
+        if len(x) != n:
+            raise ValueError(f"{names[0]} and {name} differ in length: {n} and {len(x)}")
+    wrong = n_error(n)
+    if wrong:
+        raise ValueError(wrong)
+    items = [x for seq in seqs for x in seq]
+    cuda = cuda_ok and _is_torch_tensor(items[0]) and items[0].is_cuda
+    if cuda:
+        import torch
+        torch_dtype = getattr(torch, dtype)
+    kinds = "a numpy array or a CUDA tensor" if cuda_ok else "a numpy array (host memory)"
+    ptrs, shapes = [], []
+    for k, x in enumerate(items):
+        name = names[k // n]
+        if isinstance(x, np.ndarray):
+            if cuda:
+                raise ValueError("the images must all be CUDA tensors or all host arrays")
+            if x.dtype != dtype:
+                raise ValueError(f"{name}[{k % n}] must be {dtype}, got {x.dtype}")
+            contiguous = x.flags.c_contiguous
+            ptrs.append(x.ctypes.data)
+        elif cuda_ok and _is_torch_tensor(x) and x.is_cuda:
+            if not cuda:
+                raise ValueError("the images must all be CUDA tensors or all host arrays")
+            if x.dtype != torch_dtype:
+                raise ValueError(f"{name}[{k % n}] must be {dtype}, got {x.dtype}")
+            contiguous = x.is_contiguous()
+            ptrs.append(x.data_ptr())
+        else:
+            raise ValueError(f"{name}[{k % n}] must be {kinds}, got {type(x).__name__}")
+        shape = tuple(x.shape)
+        wrong = shape_error(shape)
+        if wrong:
+            raise ValueError(f"{name}[{k % n}] {wrong}, got shape {shape}")
+        if not contiguous:
+            raise ValueError(f"{name}[{k % n}] must be contiguous")
+        shapes.append(shape)
+    return n, torch.device("cuda", device) if cuda else None, ptrs, shapes
+
+
 class Comparator(_Handle):
     """butteraugli::ButteraugliComparator (butteraugli.h:425) on one GPU: the original rgb0, planar
     linear RGB float32 [3][h][w], nominally in 0..255 and at least 8x8, stays resident and is scored
@@ -561,50 +633,8 @@ class ButteraugliBatch(_Handle):
                                                                  score.ctypes.data, stream))
         return dm, score
 
-    def _sizes_items(self, names, items0, items1, dtype, shape_error):
-        """The images of a diffmap_sizes* call, checked in one pass (a call may hold hundreds of small
-        pairs): equal-length sequences named `names`, 1..capacity pairs, all numpy arrays or all CUDA
-        tensors, each of `dtype` ("float32" or "uint8"), contiguous, its shape passing shape_error (which
-        returns what is wrong with a shape, or None) -> (n, the batch's torch device for CUDA tensors or
-        None, pointers of items0 then items1, their shapes)."""
-        items0, items1 = list(items0), list(items1)
-        n = len(items0)
-        if len(items1) != n:
-            raise ValueError(f"{names[0]} and {names[1]} differ in length: {n} and {len(items1)}")
-        if not 1 <= n <= self.capacity:
-            raise ValueError(f"the batch takes 1..{self.capacity} pairs, got {n}")
-        items = items0 + items1
-        cuda = _is_torch_tensor(items[0]) and items[0].is_cuda
-        if cuda:
-            import torch
-            torch_dtype = getattr(torch, dtype)
-        ptrs, shapes = [], []
-        for k, x in enumerate(items):
-            name = names[k // n]
-            if isinstance(x, np.ndarray):
-                if cuda:
-                    raise ValueError("the images must all be CUDA tensors or all host arrays")
-                if x.dtype != dtype:
-                    raise ValueError(f"{name}[{k % n}] must be {dtype}, got {x.dtype}")
-                contiguous = x.flags.c_contiguous
-                ptrs.append(x.ctypes.data)
-            elif _is_torch_tensor(x) and x.is_cuda:
-                if not cuda:
-                    raise ValueError("the images must all be CUDA tensors or all host arrays")
-                if x.dtype != torch_dtype:
-                    raise ValueError(f"{name}[{k % n}] must be {dtype}, got {x.dtype}")
-                contiguous = x.is_contiguous()
-                ptrs.append(x.data_ptr())
-            else:
-                raise ValueError(f"{name}[{k % n}] must be a numpy array or a CUDA tensor, got {type(x).__name__}")
-            shape = tuple(x.shape)
-            wrong = shape_error(shape)
-            if wrong:
-                raise ValueError(f"{name}[{k % n}] {wrong}, got shape {shape}")
-            if not contiguous:
-                raise ValueError(f"{name}[{k % n}] must be contiguous")
-            shapes.append(shape)
-        return n, torch.device("cuda", self.device) if cuda else None, ptrs, shapes
+    def _n_error(self, n):
+        return None if 1 <= n <= self.capacity else f"the batch takes 1..{self.capacity} pairs, got {n}"
 
     def diffmap_sizes(self, rgb0s, rgb1s):
         """Pairs of different sizes in one call: rgb0s, rgb1s equal-length sequences (1 <= n <= capacity) of
@@ -615,9 +645,8 @@ class ButteraugliBatch(_Handle):
         the batch device's current torch stream; the diffmaps come back the same kind, CUDA tensors on the
         batch's device.  As in diffmap(), a tensor on another device is refused by the C entry (RuntimeError,
         naming the argument and its device); malformed arguments raise ValueError."""
-        n, dev, ptrs, shapes = self._sizes_items(
-            ("rgb0s", "rgb1s"), rgb0s, rgb1s, "float32",
-            lambda s: "must be planar [3][h][w]" if len(s) != 3 or s[0] != 3 else None)
+        n, dev, ptrs, shapes = _sizes_items(("rgb0s", "rgb1s"), (rgb0s, rgb1s), self._n_error, "float32",
+                                            _planar_error, self.device)
         for i in range(n):
             if shapes[i] != shapes[n + i]:
                 raise ValueError(f"pair {i} differs in shape: {shapes[i]} and {shapes[n + i]}")
@@ -673,10 +702,8 @@ class ButteraugliBatch(_Handle):
         on the batch's device, read in place after the work queued on its current torch stream; the diffmaps
         come back the same kind.  As in diffmap_sizes(), a tensor on another device is refused by the C entry
         (RuntimeError); malformed arguments raise ValueError."""
-        n, dev, ptrs, shapes = self._sizes_items(
-            ("img0s", "img1s"), img0s, img1s, "uint8",
-            lambda s: ("must be interleaved [h][w][C]" if len(s) != 3 else
-                       "must have 3 (RGB) or 4 (RGBA) channels in its last axis" if s[2] not in (3, 4) else None))
+        n, dev, ptrs, shapes = _sizes_items(("img0s", "img1s"), (img0s, img1s), self._n_error, "uint8",
+                                            _interleaved_error, self.device)
         for i in range(n):
             if shapes[i][2] != shapes[n + i][2]:
                 raise ValueError(f"pair {i}: different number of channels: {shapes[i][2]} and {shapes[n + i][2]}")
@@ -698,6 +725,94 @@ class ButteraugliBatch(_Handle):
             self._ck(self.lib.gb200_butteraugli_batch_diffmap_sizes_srgb_device(*args, stream))
         else:
             self._ck(self.lib.gb200_butteraugli_batch_diffmap_sizes_srgb(*args))
+        return dm, score
+
+
+class ComparatorSet(_Handle):
+    """Many resident originals of sizes of their own, each scored against any number of candidates: the
+    originals rgb0s, a sequence of planar linear RGB float32 [3][h_i][w_i] in host memory, each at least 8x8,
+    are analysed once on one GPU and kept there (40 bytes per pixel).  diffmap() scores up to `capacity`
+    (1..16383) candidates per call, each against the original it names, in one pass of the Compare chain;
+    each result is bit for bit ButteraugliBatch.diffmap_sizes' on the pair (original, candidate), whatever
+    else the call holds.  Used by one thread at a time."""
+
+    _destroy = "gb200_butteraugli_comparator_set_destroy"
+
+    def __init__(self, rgb0s, capacity=1, device=0, lib=None):
+        self._make(rgb0s, capacity, device, lib, srgb=False)
+
+    @classmethod
+    def from_srgb(cls, img0s, capacity=1, device=0, lib=None):
+        """A set of 8-bit sRGB originals, uint8 [h_i][w_i][C_i] in host memory with C_i = 3 (RGB) or 4
+        (RGBA), each at least 8x8, scored as butteraugli_srgb scores them (an RGBA original is kept twice,
+        laid over black and over white).  diffmap() then takes uint8 [h][w][C] candidates with their
+        original's shape, and nothing else."""
+        self = cls.__new__(cls)
+        self._make(img0s, capacity, device, lib, srgb=True)
+        return self
+
+    def _make(self, items, capacity, device, lib, srgb):
+        self.lib = lib or load_library()
+        self.device, self.capacity, self.srgb = device, int(capacity), srgb
+        name = "img0s" if srgb else "rgb0s"
+        n, _, ptrs, self.shapes = _sizes_items(
+            (name,), (items,), lambda n: None if n >= 1 else "a set holds at least 1 original, got 0",
+            "uint8" if srgb else "float32", _interleaved_error if srgb else _planar_error, device, cuda_ok=False)
+        hw = [s[:2] if srgb else s[1:] for s in self.shapes]
+        for i, (h, w) in enumerate(hw):
+            if not (8 <= h < 65536 and 8 <= w < 65536):
+                raise ValueError(f"{name}[{i}] is {h}x{w}; originals must be at least 8x8 (and below 65536)")
+        hs = np.array([x[0] for x in hw], dtype=np.int32)
+        ws = np.array([x[1] for x in hw], dtype=np.int32)
+        P = C.c_void_p * n
+        if srgb:
+            chs = np.array([s[2] for s in self.shapes], dtype=np.int32)
+            self._h = self.lib.gb200_butteraugli_comparator_set_create_srgb(ws.ctypes.data, hs.ctypes.data,
+                                                                            chs.ctypes.data, P(*ptrs), n,
+                                                                            self.capacity, device)
+        else:
+            self._h = self.lib.gb200_butteraugli_comparator_set_create(ws.ctypes.data, hs.ctypes.data, P(*ptrs), n,
+                                                                       self.capacity, device)
+        if not self._h:
+            raise RuntimeError("gb200_butteraugli_comparator_set_create failed: " + _err(self.lib))
+
+    def diffmap(self, index, candidates):
+        """Candidate i against original index[i] -> (list of n diffmaps float32 [h_i][w_i], scores float64 [n]).
+
+        index: a sequence of n ints in 0..len(originals) - 1, originals in any order, any number of times;
+        candidates: n images (1 <= n <= capacity), candidate i of original index[i]'s shape.  They are all
+        numpy arrays (host memory) or all CUDA tensors on the set's device, scored after the work queued on
+        its current torch stream; the diffmaps come back the same kind.  A tensor on another device is refused
+        by the C entry (RuntimeError); malformed arguments raise ValueError."""
+        idx = np.asarray(index)
+        if idx.ndim != 1 or not np.issubdtype(idx.dtype, np.integer):
+            raise ValueError(f"index must be a sequence of ints, got {type(index).__name__} of {idx.dtype}")
+        name = "img1s" if self.srgb else "rgb1s"
+        n, dev, ptrs, shapes = _sizes_items(
+            (name,), (candidates,),
+            lambda n: None if 1 <= n <= self.capacity else f"the set takes 1..{self.capacity} candidates, got {n}",
+            "uint8" if self.srgb else "float32", _interleaved_error if self.srgb else _planar_error, self.device)
+        if len(idx) != n:
+            raise ValueError(f"index and {name} differ in length: {len(idx)} and {n}")
+        count = len(self.shapes)
+        for i, o in enumerate(idx.tolist()):
+            if not 0 <= o < count:
+                raise ValueError(f"index[{i}] = {o}, the set holds originals 0..{count - 1}")
+            if self.srgb and shapes[i][2] != self.shapes[o][2]:
+                raise ValueError(f"{name}[{i}]: different number of channels: {shapes[i][2]}, its original {o} has "
+                                 f"{self.shapes[o][2]}")
+            if shapes[i] != self.shapes[o]:
+                raise ValueError(f"{name}[{i}] must have original {o}'s shape {self.shapes[o]}, got {shapes[i]}")
+        orig = idx.astype(np.int32)
+        P = C.c_void_p * n
+        dm, dps, stream = _outputs(dev, [s[:2] if self.srgb else s[1:] for s in shapes])
+        score = np.empty(n, dtype=np.float64)
+        args = (self._h, orig.ctypes.data, P(*ptrs), n, P(*dps), score.ctypes.data)
+        entry = "gb200_butteraugli_comparator_set_diffmap" + ("_srgb" if self.srgb else "")
+        if dev is not None:
+            self._ck(getattr(self.lib, entry + "_device")(*args, stream))
+        else:
+            self._ck(getattr(self.lib, entry)(*args))
         return dm, score
 
 

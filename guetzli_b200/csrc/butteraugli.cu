@@ -444,6 +444,131 @@ void Butteraugli::compare_batch_sizes_srgb(const int* w, const int* h, const int
   }
 }
 
+// ---- comparator sets (butteraugli.h) ----
+ComparatorSet::ComparatorSet(const int* w, const int* h, const int* channels, const void* const* img0, int count,
+                             int capacity, int device)
+    : w_(w, w + count), h_(h, h + count) {
+  if (channels != nullptr) {
+    channels_.assign(channels, channels + count);
+    for (int c : channels_) check_channels(c);
+  }
+  ba_.reset(new Butteraugli(*std::max_element(w_.begin(), w_.end()), *std::max_element(h_.begin(), h_.end()),
+                            capacity, device, Butteraugli::Slots::kPairs));
+  const bool fused = ba_->fused();
+  // the store: each original's analyses (fused chain) or its input, 16-byte aligned
+  size_t bytes = 0;
+  const auto take = [&](size_t n) {
+    const size_t at = bytes;
+    bytes = (bytes + n + 15) / 16 * 16;
+    return at;
+  };
+  for (size_t b = 0; b < 2; ++b) at_[b].assign(count, kNone);
+  for (int i = 0; i < count; ++i) {
+    const size_t px = static_cast<size_t>(w[i]) * h[i];
+    if (fused) {
+      at_[0][i] = take(sizeof(float) * kStoredPlanes * px);
+      if (srgb() && channels[i] == 4) at_[1][i] = take(sizeof(float) * kStoredPlanes * px);
+    } else {
+      const size_t in = px * (srgb() ? channels[i] : 3 * sizeof(float));
+      at_[0][i] = take(in);
+      const unsigned char* p = static_cast<const unsigned char*>(img0[i]);
+      host_.emplace_back(p, p + in);
+    }
+  }
+  ba_->bind();
+  store_ = dev_alloc(bytes);
+  try {
+    unsigned char* base = static_cast<unsigned char*>(store_);
+#if !defined(GB200_HOSTSIM)
+    if (fused) {
+      // mixed passes of up to `capacity` originals: every original over black, then the RGBA ones over white
+      for (int bg = 0; bg < 2; ++bg) {
+        std::vector<int> all;
+        for (int i = 0; i < count; ++i)
+          if (at_[bg][i] != kNone) all.push_back(i);
+        for (size_t k = 0; k < all.size(); k += capacity) {
+          const size_t m = std::min(all.size() - k, static_cast<size_t>(capacity));
+          std::vector<int> cw(m), ch(m), cc(m);
+          std::vector<const void*> in(m);
+          std::vector<float*> to(m);
+          for (size_t j = 0; j < m; ++j) {
+            const int i = all[k + j];
+            cw[j] = w_[i];
+            ch[j] = h_[i];
+            cc[j] = srgb() ? channels_[i] : 3;
+            in[j] = img0[i];
+            to[j] = reinterpret_cast<float*>(base + at_[bg][i]);
+          }
+          ba_->analyse_originals(cw.data(), ch.data(), srgb() ? cc.data() : nullptr, in.data(), static_cast<int>(m),
+                                 bg == 0 ? 0 : 255, to.data());
+        }
+      }
+      return;
+    }
+#endif
+    // a copy of the inputs in device memory, for candidates in device memory
+    for (int i = 0; i < count; ++i) h2d(base + at_[0][i], host_[i].data(), host_[i].size(), ba_->region().s);
+    stream_sync(ba_->region().s);
+  } catch (...) {
+    dev_free(store_);
+    throw;
+  }
+}
+
+ComparatorSet::~ComparatorSet() {
+  try {
+    ba_->bind();
+    stream_sync(ba_->region().s);
+  } catch (...) {
+    // as in Butteraugli::release: a failed device cannot be waited for
+  }
+  dev_free(store_);
+}
+
+void ComparatorSet::compare(const int* original, const void* const* img1, int n, float* const* diffmap, float* maxima,
+                            bool device, Stream caller) {
+  std::vector<int> w(n), h(n), ch(n, 3);
+  unsigned char* base = static_cast<unsigned char*>(store_);
+  for (int i = 0; i < n; ++i) {
+    const int o = original[i];
+    w[i] = w_[o];
+    h[i] = h_[o];
+    if (srgb()) ch[i] = channels_[o];
+  }
+  const int* channels = srgb() ? ch.data() : nullptr;
+#if !defined(GB200_HOSTSIM)
+  if (ba_->fused()) {
+    std::vector<float*> stored[2];
+    for (int b = 0; b < 2; ++b)
+      for (int i = 0; i < n; ++i) {
+        const size_t at = at_[b][original[i]];
+        stored[b].push_back(at == kNone ? nullptr : reinterpret_cast<float*>(base + at));
+      }
+    float* const* const st[2] = {stored[0].data(), stored[1].data()};
+    ba_->compare_originals(w.data(), h.data(), channels, st, img1, n, diffmap, maxima, device, caller);
+    return;
+  }
+#endif
+  // the staged chain and the CPU port: the pairs (original, candidate), from the inputs' copy on the
+  // candidates' side
+  std::vector<const unsigned char*> in0(n), in1(n);
+  for (int i = 0; i < n; ++i) {
+    in0[i] = device ? base + at_[0][original[i]] : host_[original[i]].data();
+    in1[i] = static_cast<const unsigned char*>(img1[i]);
+  }
+  if (srgb()) {
+    ba_->compare_batch_sizes_srgb(w.data(), h.data(), channels, in0.data(), in1.data(), n, diffmap, maxima, device,
+                                  caller);
+  } else {
+    std::vector<const float*> f0(n), f1(n);
+    for (int i = 0; i < n; ++i) {
+      f0[i] = reinterpret_cast<const float*>(in0[i]);
+      f1[i] = reinterpret_cast<const float*>(in1[i]);
+    }
+    ba_->compare_batch_sizes(w.data(), h.data(), f0.data(), f1.data(), n, diffmap, maxima, device, caller);
+  }
+}
+
 void Butteraugli::adaptive_quantization(const float* linear_rgb, float* quant) {
   bind();
   r_.upload_planes(linear_rgb, lin_, 3);

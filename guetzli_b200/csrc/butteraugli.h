@@ -2,11 +2,13 @@
 // chain it is checked against), the float planes it works on, and the analysis of the original.
 // One Butteraugli scores one image -- the encoder's candidate (ImageContext holds one) or a
 // stand-alone comparator's -- or a batch of same-size pairs, or a batch of same-size candidates
-// against one original.  It owns the stream and the tables,
+// against one original (ComparatorSet: against resident originals of sizes of their own).  It owns the
+// stream and the tables,
 // which the encoder's kernels use as well.  See DESIGN.md §4 and §5.1.
 #pragma once
 #include <stddef.h>
 
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -220,6 +222,18 @@ class Butteraugli {
   void compare_batch_sizes_srgb(const int* w, const int* h, const int* channels, const uint8_t* const* img0,
                                 const uint8_t* const* img1, int n, float* const* diffmap, float* maxima, bool device,
                                 Stream caller);
+  // A comparator set's originals (ComparatorSet; fused chain only, on a pair batch).  analyse_originals: n <=
+  // capacity originals of sizes w[i] x h[i] in host memory, float planes (channels null) or 8-bit pixels laid
+  // over `background`, analysed in mixed passes; the kStoredPlanes planes of original i go to store[i]
+  // (device memory, [kStoredPlanes][h[i]][w[i]]).  Returns when they are there.
+  void analyse_originals(const int* w, const int* h, const int* channels, const void* const* img0, int n,
+                         int background, float* const* store);
+  // compare_batch_sizes (channels null) or compare_batch_sizes_srgb with pair i's original taken from the
+  // store: stored[0][i] its analysis (over black), stored[1][i] over white (RGBA) or null.
+  void compare_originals(const int* w, const int* h, const int* channels, float* const* const* stored,
+                         const void* const* img1, int n, float* const* diffmap, float* maxima, bool device,
+                         Stream caller);
+  bool fused() const { return use_fused_; }
   // ButteraugliComparator::Mask (b/butteraugli.cc:793) of the original at every pixel, on the
   // host: mask, mask_dc [3][h][w].  Leaves the resident PsychoImage as it is.
   void mask(float* mask, float* mask_dc);
@@ -275,11 +289,18 @@ class Butteraugli {
   // n and the pair sizes of compare_batch_sizes*, which the C entries have checked with their messages
   void check_sizes(const int* w, const int* h, int n) const;
   // compare_batch_sizes (channels null: float planes) and compare_batch_sizes_srgb on the fused chain; its
-  // buffers and tables (allocated on the first call, kept)
+  // buffers and tables (allocated on the first call, kept).  stored: compare_originals (in0 null).
   void fused_compare_sizes(const int* w, const int* h, const int* channels, const void* const* in0,
-                           const void* const* in1, int n, float* const* diffmap, float* maxima, bool device);
-  // one run of mixed passes over `pairs` (indices into w, h and src's tables): diffmap of pair i into dst[i]
-  // (device memory, or null), its maximum into maxima[i]
+                           const void* const* in1, int n, float* const* diffmap, float* maxima, bool device,
+                           float* const* const* stored = nullptr);
+  // the passes of a mixed run over `pairs` (indices into w, h and src's tables), with their tables uploaded:
+  // the pairs sorted by size into *order, pair i's diffmap into dst[i] (dst null: none)
+  std::vector<MixPass> mixed_passes(const int* w, const int* h, const std::vector<int>& pairs, const MixSrc& src,
+                                    float* const* dst, std::vector<int>* order);
+  void mixed_pack(const MixPass& p, void* const* ext, const MixSrc& src);
+  void mixed_original(const MixPass& p, bool to_arena);
+  // one run of mixed passes over `pairs`: diffmap of pair i into dst[i] (device memory, or null), its maximum
+  // into maxima[i]
   void fused_mixed_run(const int* w, const int* h, const std::vector<int>& pairs, const MixSrc& src,
                        float* const* dst, float* maxima);
   struct Mixed;
@@ -335,6 +356,40 @@ class Butteraugli {
   uint8_t* srgb_u8_ = nullptr;                 // [per_slot][capacity][h][w][4] host input, uploaded
   float* srgb_lin_ = nullptr;                  // [per_slot][capacity][3][h][w] converted planes
   float* srgb_dm_[2] = {nullptr, nullptr};     // [capacity][h][w] diffmaps: host output; over white
+};
+
+// A comparator set: `count` originals of sizes of their own, each analysed once when the set is made, and
+// candidates scored against the original each names (DESIGN.md §4).  On the fused chain the analyses stay in
+// one device buffer, the store: kStoredPlanes planes [h][w] per original, an RGBA original of an 8-bit set
+// twice (over black, then over white).  A call gathers them into the slots of one pair batch of the largest
+// width x largest height.  The staged chain and the CPU port keep the originals' inputs instead and score a
+// call through that batch's compare_batch_sizes*.
+class ComparatorSet {
+ public:
+  // w, h [count], each at least 8x8; channels null: img0[i] float planes [3][h][w], else 8-bit
+  // [h][w][channels[i]]; all in host memory
+  ComparatorSet(const int* w, const int* h, const int* channels, const void* const* img0, int count, int capacity,
+                int device);
+  ~ComparatorSet();
+  ComparatorSet(const ComparatorSet&) = delete;
+  ComparatorSet& operator=(const ComparatorSet&) = delete;
+  Butteraugli& metric() { return *ba_; }
+  int count() const { return static_cast<int>(w_.size()); }
+  bool srgb() const { return !channels_.empty(); }
+  // candidate i against original[i] (0 <= original[i] < count), img1[i] of that original's size and channels;
+  // outputs, device and caller as in compare_batch_sizes
+  void compare(const int* original, const void* const* img1, int n, float* const* diffmap, float* maxima,
+               bool device, Stream caller);
+
+ private:
+  std::vector<int> w_, h_, channels_;
+  std::unique_ptr<Butteraugli> ba_;
+  void* store_ = nullptr;
+  // byte offsets in store_ of each original's analysis over black and over white (kNone: none); staged chain
+  // and CPU port: of its input, at_[0] only
+  static constexpr size_t kNone = ~static_cast<size_t>(0);
+  std::vector<size_t> at_[2];
+  std::vector<std::vector<unsigned char> > host_;  // staged chain and CPU port: the inputs
 };
 
 #if defined(__CUDACC__) && !defined(GB200_HOSTSIM)

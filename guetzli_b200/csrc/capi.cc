@@ -68,13 +68,20 @@ struct gb200_butteraugli_batch {
   gb200::Butteraugli* ba;
 };
 
+struct gb200_butteraugli_comparator_set {
+  gb200::ComparatorSet* set;
+};
+
 namespace {
-// A comparator made from float planes takes float images, one made from 8-bit images 8-bit images.
-bool comparator_takes(const gb200_butteraugli_comparator* c, bool srgb) {
-  if ((c->channels != 0) == srgb) return true;
-  g_err = srgb ? "butteraugli comparator: made from float planes, it takes float images, not 8-bit ones"
-               : "butteraugli comparator: made from 8-bit images, it takes 8-bit images, not float planes";
+// A comparator (or set) made from float planes takes float images, one made from 8-bit images 8-bit images.
+bool made_takes(const char* who, bool made_srgb, bool srgb) {
+  if (made_srgb == srgb) return true;
+  g_err = std::string(who) + (srgb ? ": made from float planes, it takes float images, not 8-bit ones"
+                                   : ": made from 8-bit images, it takes 8-bit images, not float planes");
   return false;
+}
+bool comparator_takes(const gb200_butteraugli_comparator* c, bool srgb) {
+  return made_takes("butteraugli comparator", c->channels != 0, srgb);
 }
 
 // device pointers of a *_device entry: memory of `device`, else a message naming the argument
@@ -89,16 +96,17 @@ void check_device_pointers(const char* who, int device, const void* const* ptrs,
   }
 }
 
-// the same for the per-pair pointers of a mixed-size call, named rgb0[i], diffmap[i], ...
+// the same for the per-pair pointers of a mixed-size call, named rgb0[i], diffmap[i], ... (im0 null: a
+// comparator set's call, whose originals are its own)
 template <class T>
 void check_pair_pointers(const gb200::Butteraugli& ba, const char* name0, const char* name1, const T* const* im0,
-                         const T* const* im1, float* const* diffmap, int n) {
+                         const T* const* im1, float* const* diffmap, int n, const char* who = "butteraugli batch") {
   for (int i = 0; i < n; ++i) {
-    const void* ptrs[3] = {im0[i], im1[i], diffmap != nullptr ? diffmap[i] : nullptr};
+    const void* ptrs[3] = {im0 != nullptr ? im0[i] : nullptr, im1[i], diffmap != nullptr ? diffmap[i] : nullptr};
     const std::string k = "[" + std::to_string(i) + "]";
     const std::string names[3] = {name0 + k, name1 + k, "diffmap" + k};
     const char* what[3] = {names[0].c_str(), names[1].c_str(), names[2].c_str()};
-    check_device_pointers("butteraugli batch", ba.device(), ptrs, what, 3);
+    check_device_pointers(who, ba.device(), ptrs, what, 3);
   }
 }
 
@@ -115,10 +123,14 @@ gb200::Stream caller_stream(void* stream) {
 // sizes a metric is made for: the reference computes nothing below 8 pixels in a dimension
 // (b/butteraugli.cc:788), and the batched Compare chain folds the image into blockIdx.z, four z per
 // image in its widest launch
-void check_create(const char* who, const char* images, int w, int h, int capacity) {
-  if (w < 8 || h < 8 || w >= 65536 || h >= 65536)
-    throw std::runtime_error(std::string(who) + ": the " + images + " must be at least 8x8 (and below 65536)");
+bool create_size_ok(int w, int h) { return w >= 8 && h >= 8 && w < 65536 && h < 65536; }
+void check_capacity(const char* who, int capacity) {
   if (capacity < 1 || capacity > 16383) throw std::runtime_error(std::string(who) + ": the capacity must be in 1..16383");
+}
+void check_create(const char* who, const char* images, int w, int h, int capacity) {
+  if (!create_size_ok(w, h))
+    throw std::runtime_error(std::string(who) + ": the " + images + " must be at least 8x8 (and below 65536)");
+  check_capacity(who, capacity);
 }
 
 // n of a batched call: `kind` is "batch" or "comparator", `items` "pairs" or "images"
@@ -641,6 +653,119 @@ int gb200_butteraugli_comparator_diffmap_srgb(gb200_butteraugli_comparator* c, c
 int gb200_butteraugli_comparator_diffmap_srgb_device(gb200_butteraugli_comparator* c, const uint8_t* img1_dev, int n,
                                                      float* diffmap_dev, double* score, void* stream) {
   return comparator_diffmap_srgb(c, img1_dev, n, diffmap_dev, score, true, stream);
+}
+
+// ---- comparator sets: originals of sizes of their own, resident, each candidate scored against the
+// original it names (ButteraugliInterface per pair) ----
+namespace {
+const char* const kSet = "butteraugli comparator set";
+
+gb200_butteraugli_comparator_set* set_create(const int* w, const int* h, const int* channels, const void* const* img0,
+                                             int count, int capacity, int device, bool srgb) {
+  if (w == nullptr || h == nullptr || img0 == nullptr || (srgb && channels == nullptr)) {
+    g_err = std::string(kSet) + (srgb ? ": no sizes, no channels or no images" : ": no sizes or no images");
+    return nullptr;
+  }
+  if (count < 1) {
+    g_err = std::string(kSet) + ": count = " + std::to_string(count) + ", a set holds at least 1 original";
+    return nullptr;
+  }
+  for (int i = 0; i < count; ++i) {
+    const std::string orig = std::string(kSet) + ": original " + std::to_string(i);
+    if (!create_size_ok(w[i], h[i])) {
+      g_err = orig + " is " + std::to_string(w[i]) + "x" + std::to_string(h[i]) +
+              ", the originals must be at least 8x8 (and below 65536)";
+      return nullptr;
+    }
+    if (srgb && !channels_ok(orig.c_str(), channels[i])) return nullptr;
+    if (img0[i] == nullptr) {
+      g_err = orig + " has a null image pointer";
+      return nullptr;
+    }
+  }
+  gb200_butteraugli_comparator_set* s = nullptr;
+  guarded([&]() {
+    check_capacity(kSet, capacity);
+    std::unique_ptr<gb200::ComparatorSet> set(new gb200::ComparatorSet(w, h, srgb ? channels : nullptr, img0, count,
+                                                                       capacity, device));
+    s = new gb200_butteraugli_comparator_set;
+    s->set = set.release();
+  });
+  return s;
+}
+
+// every argument is checked before anything is queued
+int set_diffmap(gb200_butteraugli_comparator_set* s, const int* original, const void* const* img1, int n,
+                float* const* diffmap, double* score, bool srgb, bool device, void* stream) {
+  if (s == nullptr || original == nullptr || img1 == nullptr) {
+    g_err = std::string(kSet) + ": no set, no indices or no images";
+    return 0;
+  }
+  if (!made_takes(kSet, s->set->srgb(), srgb)) return 0;
+  gb200::Butteraugli& ba = s->set->metric();
+  if (!n_ok("comparator set", "images", n, ba)) return 0;
+  const int count = s->set->count();
+  for (int i = 0; i < n; ++i) {
+    if (original[i] < 0 || original[i] >= count) {
+      g_err = std::string(kSet) + ": original[" + std::to_string(i) + "] = " + std::to_string(original[i]) +
+              ", the set holds originals 0.." + std::to_string(count - 1);
+      return 0;
+    }
+    if (img1[i] == nullptr) {
+      g_err = std::string(kSet) + ": image " + std::to_string(i) + " has a null pointer";
+      return 0;
+    }
+  }
+  return scored(&ba, n, score, [&](float* m) {
+    if (device)
+      check_pair_pointers<void>(ba, "", srgb ? "img1" : "rgb1", nullptr, img1, diffmap, n, kSet);
+    s->set->compare(original, img1, n, diffmap, m, device, caller_stream(stream));
+  });
+}
+}  // namespace
+
+gb200_butteraugli_comparator_set* gb200_butteraugli_comparator_set_create(const int* w, const int* h,
+                                                                          const float* const* rgb0, int count,
+                                                                          int capacity, int device) {
+  return set_create(w, h, nullptr, reinterpret_cast<const void* const*>(rgb0), count, capacity, device, false);
+}
+
+gb200_butteraugli_comparator_set* gb200_butteraugli_comparator_set_create_srgb(const int* w, const int* h,
+                                                                               const int* channels,
+                                                                               const uint8_t* const* img0, int count,
+                                                                               int capacity, int device) {
+  return set_create(w, h, channels, reinterpret_cast<const void* const*>(img0), count, capacity, device, true);
+}
+
+int gb200_butteraugli_comparator_set_diffmap(gb200_butteraugli_comparator_set* s, const int* original,
+                                             const float* const* rgb1, int n, float* const* diffmap, double* score) {
+  return set_diffmap(s, original, reinterpret_cast<const void* const*>(rgb1), n, diffmap, score, false, false, nullptr);
+}
+
+int gb200_butteraugli_comparator_set_diffmap_device(gb200_butteraugli_comparator_set* s, const int* original,
+                                                    const float* const* rgb1_dev, int n, float* const* diffmap_dev,
+                                                    double* score, void* stream) {
+  return set_diffmap(s, original, reinterpret_cast<const void* const*>(rgb1_dev), n, diffmap_dev, score, false, true,
+                     stream);
+}
+
+int gb200_butteraugli_comparator_set_diffmap_srgb(gb200_butteraugli_comparator_set* s, const int* original,
+                                                  const uint8_t* const* img1, int n, float* const* diffmap,
+                                                  double* score) {
+  return set_diffmap(s, original, reinterpret_cast<const void* const*>(img1), n, diffmap, score, true, false, nullptr);
+}
+
+int gb200_butteraugli_comparator_set_diffmap_srgb_device(gb200_butteraugli_comparator_set* s, const int* original,
+                                                         const uint8_t* const* img1_dev, int n,
+                                                         float* const* diffmap_dev, double* score, void* stream) {
+  return set_diffmap(s, original, reinterpret_cast<const void* const*>(img1_dev), n, diffmap_dev, score, true, true,
+                     stream);
+}
+
+void gb200_butteraugli_comparator_set_destroy(gb200_butteraugli_comparator_set* s) {
+  if (!s) return;
+  guarded([&]() { delete s->set; });
+  delete s;
 }
 
 // ButteraugliComparator::Mask (b/butteraugli.cc:793)

@@ -1319,4 +1319,46 @@ __global__ void __launch_bounds__(256) k_mix_srgb(const uint8_t* const* src, con
   for (int x = lane; x < w; x += 32) srgb_over_linear(s + x * C, C, background, lut, a + x, g.plane);
 }
 
+// Comparator sets: an original's analysis between the set's store and arena slot n0 + j, all images of a
+// pass in one launch.  Image j has rows [row0[j], row0[j + 1]), kStoredPlanes * h of them, of w floats at
+// store[j]; row r is row r % h of stored plane r / h.  The stored planes are the eight of ps0 that the
+// Compare chain reads (EpiMf: mf X, Y; EpiHf: uhf, hf of X and Y; EpiNoise: hf Y; CombineArgs: lf X, B),
+// then sup0's two.  TO_ARENA: the gather before a Compare; else the store after the analysis.  A warp per
+// row, 8 rows per block; float4 where the row is 16-byte aligned on both sides (arena rows always are: the
+// pitch is a multiple of 32 floats; store rows are where w is a multiple of 4).
+static_assert(kUhfX == 0 && kUhfY == 1 && kHfX == 2 && kHfY == 3 && kMfX == 4 && kMfY == 5 && kLfX == 7 &&
+                  kLfB == 9,
+              "stored plane c < 6 is ps0 plane c, 6 and 7 are lf X and lf B");
+template <bool TO_ARENA>
+__global__ void __launch_bounds__(256) k_mix_original(float* const* store, const int* row0, float* ps0, float* sup0,
+                                                      PlaneGeomMix g) {
+  const int row = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (row >= __ldg(row0 + g.mix.m)) return;
+  const int j = mix_find(row0, g.mix.m, row);
+  const int w = g.mix.img[j].w, h = g.mix.img[j].h;
+  const int r = row - __ldg(row0 + j), c = r / h, y = r - c * h;
+  const int pl = c < 6 ? c : c < 8 ? 2 * c - 5 : c - 8;
+  float* a = (c < 8 ? ps0 : sup0) + slot_offset(g, g.mix.n0 + j) + pl * g.plane + static_cast<size_t>(y) * g.pitch;
+  float* e = store[j] + static_cast<size_t>(r) * w;
+  if (((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(e)) & 15) == 0 && (w & 3) == 0) {
+    float4* a4 = reinterpret_cast<float4*>(a);
+    float4* e4 = reinterpret_cast<float4*>(e);
+    for (int x = lane; x < (w >> 2); x += 32) {
+      if (TO_ARENA) {
+        a4[x] = e4[x];
+      } else {
+        e4[x] = a4[x];
+      }
+    }
+    return;
+  }
+  for (int x = lane; x < w; x += 32) {
+    if (TO_ARENA) {
+      a[x] = e[x];
+    } else {
+      e[x] = a[x];
+    }
+  }
+}
+
 }  // namespace gb200

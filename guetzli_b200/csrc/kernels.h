@@ -257,6 +257,9 @@ struct OpsinPx {
 // SeparateFrequencies (b/butteraugli.cc:489-622).  PsychoImage plane order in
 // one contiguous group of 10: uhf[X,Y], hf[X,Y], mf[X,Y,B], lf[X,Y,B].
 enum PsychoPlane { kUhfX = 0, kUhfY, kHfX, kHfY, kMfX, kMfY, kMfB, kLfX, kLfY, kLfB, kPsychoPlanes };
+// planes of an original that a comparator set stores (k_mix_original): the Compare chain reads every
+// plane of its PsychoImage but mf[B] and lf[Y], and its two DiffPrecompute neighbour sums
+constexpr int kStoredPlanes = kPsychoPlanes - 2 + 2;
 
 // mf = xyb - lf for 3 planes (:509-513); launched over w x 3h.
 struct SubPlanes {

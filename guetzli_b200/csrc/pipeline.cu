@@ -69,7 +69,8 @@ inline int roll_seg(int rows) {
 
 }  // namespace
 
-// One pass of a mixed-size call (Butteraugli::fused_compare_sizes): its images, slots n0 .. n0 + m - 1,
+// One pass of a mixed-size call (Butteraugli::fused_compare_sizes, and a comparator set's analysis and
+// scoring): its images, slots n0 .. n0 + m - 1,
 // have at most GB_MIX_SHAPES distinct sizes.  Device tables: the images, and per tile shape of the
 // chain's launches the first work item of each image.
 enum MixKind { kMix2d, kMixRollLf, kMixRollMf, kMixPx, kMixX4, kMixMalta, kMixY, kMixKinds };
@@ -85,7 +86,10 @@ struct MixPass {
   void* const* ext0 = nullptr;  // [m] first image of each pair (device memory: float or 8-bit)
   void* const* ext1 = nullptr;
   float* const* extdm = nullptr;  // [m] diffmap of each image, or null
-  int rows_in_total = 0, rows_dm_total = 0;
+  // a comparator set's run: kStoredPlanes * h rows per image, and its original's analysis in the store
+  const int* rows_org = nullptr;  // [m + 1]
+  float* const* extorg = nullptr;  // [m]
+  int rows_in_total = 0, rows_dm_total = 0, rows_org_total = 0;
   std::deque<MixMaps> mapsets;  // the map sets of the launches queued so far (stable addresses)
   MixGeom geom(int kind) const { return MixGeom{img, tile0 + kind * (m + 1), m, n0}; }
 };
@@ -536,24 +540,28 @@ size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 }  // namespace
 
 // The images of a mixed run, per pair index, in memory of this device: float planes [3][h][w] (channels
-// null), or 8-bit pixels [h][w][channels] laid over `background`.
+// null), or 8-bit pixels [h][w][channels] laid over `background`.  store: a comparator set's run, the
+// analysis of pair i's original in the set's store (kStoredPlanes planes [h][w]); img[0] is then unused.
 struct MixSrc {
   const void* const* img[2] = {nullptr, nullptr};
   const int* channels = nullptr;
   int background = 0;
+  float* const* store = nullptr;
 };
 
 void Butteraugli::fused_compare_sizes(const int* w, const int* h, const int* channels, const void* const* in0,
                                       const void* const* in1, int n, float* const* diffmap, float* maxima,
-                                      bool device) {
+                                      bool device, float* const* const* stored) {
   if (mixed_ == nullptr) mixed_ = new Mixed();
   Mixed& mx = *mixed_;
   if (channels != nullptr && t_.srgb_lin == nullptr) t_.srgb_lin = upload_srgb_lin(s_, &owned_, nullptr);
   const auto in_bytes = [&](int i) {  // of one image of pair i
     return static_cast<size_t>(w[i]) * h[i] * (channels != nullptr ? channels[i] : 3 * sizeof(float));
   };
+  const int sides = stored != nullptr ? 1 : 2;  // a comparator set's originals are in its store
   std::vector<int> all(n), rgba;
-  std::vector<const void*> p0(in0, in0 + n), p1(in1, in1 + n);
+  std::vector<const void*> p0(n), p1(in1, in1 + n);
+  if (in0 != nullptr) p0.assign(in0, in0 + n);
   // input staging: byte offset of pair i on one side; diffmap staging: host output, black's diffmaps of
   // every pair, then white's of the RGBA pairs with a diffmap; device output, white's alone (black's go to
   // the caller's memory)
@@ -573,15 +581,18 @@ void Butteraugli::fused_compare_sizes(const int* w, const int* h, const int* cha
     }
   }
   if (!device) {  // host images: packed once, uploaded in one copy (for both backgrounds), side 0 then side 1
-    mx.stage_in = grow(mx.stage_in, &mx.stage_in_bytes, 2 * bytes);
-    mx.host_in.resize(2 * bytes);
+    const size_t at1 = (sides - 1) * bytes;
+    mx.stage_in = grow(mx.stage_in, &mx.stage_in_bytes, sides * bytes);
+    mx.host_in.resize(sides * bytes);
     for (int i = 0; i < n; ++i) {
-      memcpy(&mx.host_in[in_at[i]], in0[i], in_bytes(i));
-      memcpy(&mx.host_in[bytes + in_at[i]], in1[i], in_bytes(i));
-      p0[i] = mx.stage_in + in_at[i];
-      p1[i] = mx.stage_in + bytes + in_at[i];
+      if (sides == 2) {
+        memcpy(&mx.host_in[in_at[i]], in0[i], in_bytes(i));
+        p0[i] = mx.stage_in + in_at[i];
+      }
+      memcpy(&mx.host_in[at1 + in_at[i]], in1[i], in_bytes(i));
+      p1[i] = mx.stage_in + at1 + in_at[i];
     }
-    h2d(mx.stage_in, mx.host_in.data(), 2 * bytes, s_);
+    h2d(mx.stage_in, mx.host_in.data(), sides * bytes, s_);
   }
   const size_t black = diffmap != nullptr && !device ? px : 0;
   if (black + px_white > 0) mx.stage_dm = grow(mx.stage_dm, &mx.stage_dm_floats, black + px_white);
@@ -596,6 +607,7 @@ void Butteraugli::fused_compare_sizes(const int* w, const int* h, const int* cha
   src.img[0] = p0.data();
   src.img[1] = p1.data();
   src.channels = channels;
+  if (stored != nullptr) src.store = stored[0];
   fused_mixed_run(w, h, all, src, dst.data(), maxima);
   // RGBA pairs over white: a run of their own (their sizes make its passes); where white wins, its score
   // and diffmap replace black's
@@ -603,6 +615,7 @@ void Butteraugli::fused_compare_sizes(const int* w, const int* h, const int* cha
   if (!rgba.empty()) {
     std::vector<float> m_white(n);
     src.background = 255;
+    if (stored != nullptr) src.store = stored[1];
     fused_mixed_run(w, h, rgba, src, dst_white.data(), m_white.data());
     bool copied = false;
     for (int i : rgba) {
@@ -625,8 +638,23 @@ void Butteraugli::fused_compare_sizes(const int* w, const int* h, const int* cha
   }
 }
 
-void Butteraugli::fused_mixed_run(const int* w, const int* h, const std::vector<int>& pairs, const MixSrc& src,
-                                  float* const* dst, float* maxima) {
+namespace {
+// the geometry argument of a row-copy launch over a mixed pass's images
+PlaneGeomMix mix_geom(const Geom& g, int kslot, const MixPass& p) {
+  PlaneGeomMix pg;
+  static_cast<PlaneGeom&>(pg) = fused_geom(g, 0, g.h, kslot, kslot);
+  pg.mix = p.geom(0);
+  return pg;
+}
+// mix_ is only set while a pass's launches are queued
+struct MixScope {
+  MixPass** p;
+  ~MixScope() { *p = nullptr; }
+};
+}  // namespace
+
+std::vector<MixPass> Butteraugli::mixed_passes(const int* w, const int* h, const std::vector<int>& pairs,
+                                               const MixSrc& src, float* const* dst, std::vector<int>* order_out) {
   Mixed& mx = *mixed_;
   const bool u8 = src.channels != nullptr;
   // The per-size caches (border scales here, tensor maps in Fused::maps) are bounded: once they hold more
@@ -639,7 +667,8 @@ void Butteraugli::fused_mixed_run(const int* w, const int* h, const std::vector<
   }
   // Slots in the order of the sizes, so that a pass (at most GB_MIX_SHAPES sizes) is a run of slots.
   const int n = static_cast<int>(pairs.size());
-  std::vector<int> order(pairs);
+  std::vector<int>& order = *order_out;
+  order = pairs;
   std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return std::make_pair(w[a], h[a]) < std::make_pair(w[b], h[b]); });
   std::vector<MixPass> passes;
   for (int k = 0; k < n; ++k) {
@@ -654,8 +683,9 @@ void Butteraugli::fused_mixed_run(const int* w, const int* h, const std::vector<
     ++p.m;
   }
   // The tables of every pass, laid out in one blob (offsets first, pointers filled once it has an address).
+  // A comparator set's run adds the rows and pointers of its originals' analyses at the end.
   struct Layout {
-    size_t img, tile0, rows_in, rows_dm, ext0, ext1, extdm, scales, blur_len;
+    size_t img, tile0, rows_in, rows_dm, ext0, ext1, extdm, scales, blur_len, rows_org, extorg;
   };
   std::vector<Layout> lay(passes.size());
   size_t bytes = 0;
@@ -681,6 +711,12 @@ void Butteraugli::fused_mixed_run(const int* w, const int* h, const std::vector<
     bytes += sizeof(float*) * p.m;
     l.scales = bytes = align_up(bytes, 16);
     bytes += sizeof(float) * kNumBlurs * len;
+    if (src.store != nullptr) {
+      l.rows_org = bytes;
+      bytes += sizeof(int) * (p.m + 1);
+      l.extorg = bytes = align_up(bytes, 16);
+      bytes += sizeof(float*) * p.m;
+    }
   }
   mx.tables = grow(static_cast<unsigned char*>(mx.tables), &mx.tables_bytes, bytes);
   mx.blob.assign(bytes, 0);
@@ -701,6 +737,8 @@ void Butteraugli::fused_mixed_run(const int* w, const int* h, const std::vector<
     void** ext1 = reinterpret_cast<void**>(b + l.ext1);
     float** extdm = reinterpret_cast<float**>(b + l.extdm);
     float* sc = reinterpret_cast<float*>(b + l.scales);
+    int* rows_org = src.store != nullptr ? reinterpret_cast<int*>(b + l.rows_org) : nullptr;
+    float** extorg = src.store != nullptr ? reinterpret_cast<float**>(b + l.extorg) : nullptr;
     // border scales: per blur, scale_x of every size, then scale_y of every size
     std::vector<int> sxo(p.shapes.size()), syo(p.shapes.size());
     size_t ox = 0, oy = 0, xsum = 0;
@@ -731,6 +769,7 @@ void Butteraugli::fused_mixed_run(const int* w, const int* h, const std::vector<
     }
     int shape = -1;
     rows_in[0] = rows_dm[0] = 0;
+    if (rows_org != nullptr) rows_org[0] = 0;
     for (int kind = 0; kind < kMixKinds; ++kind) tile0[kind * (p.m + 1)] = 0;
     for (int j = 0; j < p.m; ++j) {
       const int i = order[p.n0 + j], iw = w[i], ih = h[i];
@@ -752,11 +791,16 @@ void Butteraugli::fused_mixed_run(const int* w, const int* h, const std::vector<
       }
       // packing rows: 3h plane rows of float planes, h pixel rows of 8-bit images; unpacking: h rows of
       // the images with a diffmap
+      const bool has_dm = dst != nullptr && dst[i] != nullptr;
       rows_in[j + 1] = rows_in[j] + (u8 ? ih : 3 * ih);
-      rows_dm[j + 1] = rows_dm[j] + (dst[i] != nullptr ? ih : 0);
-      ext0[j] = const_cast<void*>(src.img[0][i]);
-      ext1[j] = const_cast<void*>(src.img[1][i]);
-      extdm[j] = dst[i];
+      rows_dm[j + 1] = rows_dm[j] + (has_dm ? ih : 0);
+      ext0[j] = src.img[0] != nullptr ? const_cast<void*>(src.img[0][i]) : nullptr;
+      ext1[j] = src.img[1] != nullptr ? const_cast<void*>(src.img[1][i]) : nullptr;
+      extdm[j] = has_dm ? dst[i] : nullptr;
+      if (rows_org != nullptr) {
+        rows_org[j + 1] = rows_org[j] + kStoredPlanes * ih;
+        extorg[j] = src.store[i];
+      }
     }
     p.img = reinterpret_cast<const MixImage*>(dev + l.img);
     p.tile0 = reinterpret_cast<const int*>(dev + l.tile0);
@@ -768,50 +812,125 @@ void Butteraugli::fused_mixed_run(const int* w, const int* h, const std::vector<
     for (int kind = 0; kind < kMixKinds; ++kind) p.total[kind] = tile0[kind * (p.m + 1) + p.m];
     p.rows_in_total = rows_in[p.m];
     p.rows_dm_total = rows_dm[p.m];
+    if (rows_org != nullptr) {
+      p.rows_org = reinterpret_cast<const int*>(dev + l.rows_org);
+      p.extorg = reinterpret_cast<float* const*>(dev + l.extorg);
+      p.rows_org_total = rows_org[p.m];
+    }
   }
   h2d(mx.tables, mx.blob.data(), bytes, s_);
+  return passes;
+}
+
+// one side's images into the lin planes of the pass's slots
+void Butteraugli::mixed_pack(const MixPass& p, void* const* ext, const MixSrc& src) {
+  const PlaneGeomMix pg = mix_geom(g_, kslot_, p);
+  const int total = p.rows_in_total;
+  if (src.channels != nullptr) {
+    note_launch("mix_pack_srgb", s_, static_cast<double>(total));
+    k_mix_srgb<<<cdiv(total, 8), 256, 0, s_>>>(reinterpret_cast<const uint8_t* const*>(ext), p.rows_in,
+                                               src.background, t_.srgb_lin, lin_, pg);
+    note_launch_end("mix_pack_srgb", s_);
+  } else {
+    note_launch("mix_pack", s_, static_cast<double>(total));
+    k_mix_rows<true><<<cdiv(total, 8), 256, 0, s_>>>(reinterpret_cast<float* const*>(ext), p.rows_in, lin_, pg);
+    note_launch_end("mix_pack", s_);
+  }
+}
+
+// the analyses of a comparator set's originals between its store and the ps0 and sup0 planes of the pass's
+// slots
+void Butteraugli::mixed_original(const MixPass& p, bool to_arena) {
+  const PlaneGeomMix pg = mix_geom(g_, kslot_, p);
+  const int rows = p.rows_org_total;
+  const char* name = to_arena ? "mix_gather_original" : "mix_store_original";
+  note_launch(name, s_, static_cast<double>(rows));
+  if (to_arena) {
+    k_mix_original<true><<<cdiv(rows, 8), 256, 0, s_>>>(p.extorg, p.rows_org, ps0_, sup0_, pg);
+  } else {
+    k_mix_original<false><<<cdiv(rows, 8), 256, 0, s_>>>(p.extorg, p.rows_org, ps0_, sup0_, pg);
+  }
+  note_launch_end(name, s_);
+}
+
+void Butteraugli::fused_mixed_run(const int* w, const int* h, const std::vector<int>& pairs, const MixSrc& src,
+                                  float* const* dst, float* maxima) {
+  std::vector<int> order;
+  std::vector<MixPass> passes = mixed_passes(w, h, pairs, src, dst, &order);
   // one pass of the chain per run of at most GB_MIX_SHAPES sizes
-  const PlaneGeom base = fused_geom(g_, 0, g_.h, kslot_, kslot_);
-  struct Clear {  // mix_ is only set while a pass's launches are queued
-    MixPass** p;
-    ~Clear() { *p = nullptr; }
-  } clear{&mix_};
+  MixScope scope{&mix_};
   for (MixPass& p : passes) {
     mix_ = &p;
-    PlaneGeomMix pg;
-    static_cast<PlaneGeom&>(pg) = base;
-    pg.mix = p.geom(0);
-    // one side's images into the lin planes of the pass's slots
-    const auto pack = [&](void* const* ext) {
-      const int total = p.rows_in_total;
-      if (u8) {
-        note_launch("mix_pack_srgb", s_, static_cast<double>(total));
-        k_mix_srgb<<<cdiv(total, 8), 256, 0, s_>>>(reinterpret_cast<const uint8_t* const*>(ext), p.rows_in,
-                                                   src.background, t_.srgb_lin, lin_, pg);
-        note_launch_end("mix_pack_srgb", s_);
-      } else {
-        note_launch("mix_pack", s_, static_cast<double>(total));
-        k_mix_rows<true><<<cdiv(total, 8), 256, 0, s_>>>(reinterpret_cast<float* const*>(ext), p.rows_in, lin_, pg);
-        note_launch_end("mix_pack", s_);
-      }
-    };
-    // PsychoImage of every original and its DiffPrecompute neighbour sums, then the Compare chain
-    pack(p.ext0);
-    fused_opsin(lin_, xyb_, p.m, kslot_);
-    fused_separate(xyb_, ps0_, false, p.m, kslot_, kslot_);
-    fused_sup0(p.m, kslot_);
-    pack(p.ext1);
+    if (src.store != nullptr) {  // a comparator set's originals, analysed when it was made
+      mixed_original(p, true);
+    } else {  // PsychoImage of every original and its DiffPrecompute neighbour sums
+      mixed_pack(p, p.ext0, src);
+      fused_opsin(lin_, xyb_, p.m, kslot_);
+      fused_separate(xyb_, ps0_, false, p.m, kslot_, kslot_);
+      fused_sup0(p.m, kslot_);
+    }
+    mixed_pack(p, p.ext1, src);
     fused_compare_launches(p.m, kslot_, kslot_);
     if (p.rows_dm_total > 0) {
       note_launch("mix_unpack", s_, static_cast<double>(p.rows_dm_total));
-      k_mix_rows<false><<<cdiv(p.rows_dm_total, 8), 256, 0, s_>>>(p.extdm, p.rows_dm, dm_, pg);
+      k_mix_rows<false><<<cdiv(p.rows_dm_total, 8), 256, 0, s_>>>(p.extdm, p.rows_dm, dm_, mix_geom(g_, kslot_, p));
       note_launch_end("mix_unpack", s_);
     }
   }
   // one transfer of the n maxima (float bits), which waits for everything queued before
+  const int n = static_cast<int>(pairs.size());
   std::vector<float> m(n);
   d2h(m.data(), d_gmax_, sizeof(float) * n, s_);
   for (int k = 0; k < n; ++k) maxima[order[k]] = m[k];
+}
+
+void Butteraugli::analyse_originals(const int* w, const int* h, const int* channels, const void* const* img0, int n,
+                                    int background, float* const* store) {
+  check_sizes(w, h, n);
+  bind();
+  if (mixed_ == nullptr) mixed_ = new Mixed();
+  Mixed& mx = *mixed_;
+  if (channels != nullptr && t_.srgb_lin == nullptr) t_.srgb_lin = upload_srgb_lin(s_, &owned_, nullptr);
+  // the originals packed and uploaded in one copy
+  std::vector<size_t> at(n + 1, 0);
+  for (int i = 0; i < n; ++i)
+    at[i + 1] = at[i] + static_cast<size_t>(w[i]) * h[i] * (channels != nullptr ? channels[i] : 3 * sizeof(float));
+  mx.stage_in = grow(mx.stage_in, &mx.stage_in_bytes, at[n]);
+  mx.host_in.resize(at[n]);
+  std::vector<const void*> p0(n);
+  std::vector<int> all(n);
+  for (int i = 0; i < n; ++i) {
+    memcpy(&mx.host_in[at[i]], img0[i], at[i + 1] - at[i]);
+    p0[i] = mx.stage_in + at[i];
+    all[i] = i;
+  }
+  h2d(mx.stage_in, mx.host_in.data(), at[n], s_);
+  MixSrc src;
+  src.img[0] = p0.data();
+  src.channels = channels;
+  src.background = background;
+  src.store = store;
+  std::vector<int> order;
+  std::vector<MixPass> passes = mixed_passes(w, h, all, src, nullptr, &order);
+  MixScope scope{&mix_};
+  for (MixPass& p : passes) {
+    mix_ = &p;
+    mixed_pack(p, p.ext0, src);
+    fused_opsin(lin_, xyb_, p.m, kslot_);
+    fused_separate(xyb_, ps0_, false, p.m, kslot_, kslot_);
+    fused_sup0(p.m, kslot_);
+    mixed_original(p, false);
+  }
+  stream_sync(s_);
+}
+
+void Butteraugli::compare_originals(const int* w, const int* h, const int* channels, float* const* const* stored,
+                                    const void* const* img1, int n, float* const* diffmap, float* maxima, bool device,
+                                    Stream caller) {
+  check_sizes(w, h, n);
+  bind();
+  if (device) stream_wait(s_, caller);
+  fused_compare_sizes(w, h, channels, nullptr, img1, n, diffmap, maxima, device, stored);
 }
 
 #endif  // !GB200_HOSTSIM

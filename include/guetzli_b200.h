@@ -224,6 +224,50 @@ int gb200_butteraugli_comparator_diffmap_srgb(gb200_butteraugli_comparator* c, c
 int gb200_butteraugli_comparator_diffmap_srgb_device(gb200_butteraugli_comparator* c, const uint8_t* img1_dev, int n,
                                                      float* diffmap_dev, double* score, void* stream);
 
+/* ---- comparator sets: many resident originals of sizes of their own ----
+ * A set holds `count` >= 1 originals, each at least 8x8 and below 65536 in each dimension, of sizes that may
+ * differ.  Each is analysed once, when the set is made, and its analysis stays in device memory (40 bytes
+ * per pixel; an RGBA original twice, over black and over white).  A call scores 1 <= n <= capacity
+ * candidates: candidate i names its original by index, original[i] in 0..count-1, and has that original's
+ * size (and channels).  Each candidate's diffmap and score are bit for bit what
+ * gb200_butteraugli_batch_diffmap_sizes (float set) or gb200_butteraugli_batch_diffmap_sizes_srgb (8-bit
+ * set) give for the pair (original, candidate), whatever else the call holds.  All candidates go through one
+ * pass of the Compare chain (several where the call has more than 16 distinct sizes).  A set is used by one
+ * thread at a time; separate sets may run concurrently.  Every call returns once its outputs are written. */
+typedef struct gb200_butteraugli_comparator_set gb200_butteraugli_comparator_set;
+/* w, h: host arrays [count]; rgb0[i]: planar linear RGB floats [3][h[i]][w[i]] in host memory;
+ * 1 <= capacity <= 16383.  NULL on failure (gb200_last_error), with nothing left allocated. */
+gb200_butteraugli_comparator_set* gb200_butteraugli_comparator_set_create(const int* w, const int* h,
+                                                                          const float* const* rgb0, int count,
+                                                                          int capacity, int device);
+/* The same for 8-bit originals: img0[i] interleaved [h[i]][w[i]][channels[i]] in host memory, channels 3 (RGB)
+ * or 4 (RGBA) per original, RGB and RGBA in one set.  It takes 8-bit candidates only. */
+gb200_butteraugli_comparator_set* gb200_butteraugli_comparator_set_create_srgb(const int* w, const int* h,
+                                                                               const int* channels,
+                                                                               const uint8_t* const* img0, int count,
+                                                                               int capacity, int device);
+/* original: host array [n]; rgb1[i]: [3][h][w] of original[i]'s size, in host memory; diffmap (may be NULL,
+ * and so may its entries) [i]: [h][w]; score (may be NULL) [n].  A set made from 8-bit images refuses it. */
+int gb200_butteraugli_comparator_set_diffmap(gb200_butteraugli_comparator_set* s, const int* original,
+                                             const float* const* rgb1, int n, float* const* diffmap, double* score);
+/* The same with every candidate and diffmap in device memory of the set's device, read in place; stream as in
+ * gb200_butteraugli_batch_diffmap_device.  A host, managed or other device's pointer is refused, nothing
+ * runs. */
+int gb200_butteraugli_comparator_set_diffmap_device(gb200_butteraugli_comparator_set* s, const int* original,
+                                                    const float* const* rgb1_dev, int n, float* const* diffmap_dev,
+                                                    double* score, void* stream);
+/* 8-bit candidates: img1[i] [h][w][channels] of original[i]'s size and channels, in host memory, uploaded
+ * once as bytes; outputs as in gb200_butteraugli_comparator_set_diffmap.  A float set refuses it. */
+int gb200_butteraugli_comparator_set_diffmap_srgb(gb200_butteraugli_comparator_set* s, const int* original,
+                                                  const uint8_t* const* img1, int n, float* const* diffmap,
+                                                  double* score);
+/* The same with every candidate and diffmap in device memory of the set's device, read in place; stream and
+ * refusals as in gb200_butteraugli_comparator_set_diffmap_device. */
+int gb200_butteraugli_comparator_set_diffmap_srgb_device(gb200_butteraugli_comparator_set* s, const int* original,
+                                                         const uint8_t* const* img1_dev, int n,
+                                                         float* const* diffmap_dev, double* score, void* stream);
+void gb200_butteraugli_comparator_set_destroy(gb200_butteraugli_comparator_set* s);
+
 /* butteraugli::ButteraugliAdaptiveQuantization (butteraugli.cc:1880): the Y plane of Mask(rgb, rgb),
  * [h][w] into quant.  rgb in host memory.  Fails below 16x16, where the reference returns false. */
 int gb200_butteraugli_adaptive_quantization(const float* rgb, int w, int h, int device, float* quant);

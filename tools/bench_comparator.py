@@ -51,7 +51,22 @@ their first 8-bit call (MiB, from torch.cuda.mem_get_info after gb200_trim_memor
 time of the work.  The modes run in turn for `--rounds` rounds (the spread between rounds is part of the
 result), after `--warmup` untimed calls each.  The card's name and power limit are read in the
 same run (nvidia-smi, read-only queries).  Prints one JSON line; --out also writes it to a file.
-There is no CPU mode: without a GPU the script fails."""
+There is no CPU mode: without a GPU the script fails.
+
+With --set, two rate-distortion sweeps (SET_WORKLOADS: K originals of sizes of their own, Q candidates
+each) are scored in calls of --sizes-capacity candidates, ms per candidate, in modes that alternate in
+every round:
+
+  set_cuda          one ComparatorSet of all K originals (made before timing), CUDA tensors
+  set_host          the same set, numpy arrays
+  sizes_cuda        the same pairs through ButteraugliBatch.diffmap_sizes, CUDA tensors: every call
+                    analyses and uploads its originals again
+  sizes_host        the same with numpy arrays
+  comparators_cuda  ("kodak" only) one Comparator of capacity Q per original, made before timing, one call
+                    per original
+
+It reports the device memory each holds after gb200_trim_memory, the bytes each host mode uploads per
+candidate, and whether every mode's scores are equal."""
 import argparse
 import json
 import os
@@ -99,6 +114,7 @@ def main():
     ap.add_argument("--sizes-capacity", type=int, default=64,
                     help="pairs per call of a set whose largest size is 1920x1080 (the arena of 256 such slots "
                          "does not fit in 80 GB)")
+    ap.add_argument("--set", action="store_true", help="time the comparator-set sweeps and nothing else")
     ap.add_argument("--out", default=None, help="also write the JSON result here")
     args = ap.parse_args()
 
@@ -109,6 +125,11 @@ def main():
     dev = torch.device("cuda", args.device)
     torch.cuda.set_device(dev)
 
+    if args.set:
+        result = {"set": bench_set(args, dev, torch)}
+        result.update(gpu_info(args.device))
+        emit(result, args.out)
+        return
     if args.sizes_only:
         result = {"sizes": bench_sizes(args, dev, torch)}
         result.update(gpu_info(args.device))
@@ -416,6 +437,105 @@ def bench_sizes(args, dev, torch):
                                                     if "_srgb" in m),
                      "rgba_pairs": len(rgba),
                      "device_memory": {"batch_mib": round(f0 - f1, 1), "sizes_srgb_buffers_mib": round(f1 - f2, 1)}}
+    return out
+
+
+def set_workloads():
+    """name -> ([(h, w) of each original], candidates per original)"""
+    rng = np.random.default_rng(23)
+    return {
+        # Kodak-like: 24 landscape and portrait 768x512 images, 8 quality settings each
+        "kodak": ([(512, 768) if i % 3 else (768, 512) for i in range(24)], 8),
+        # a folder of thumbnails: 1024 images of random sizes from 32 to 256, 4 quality settings each
+        "thumbnails": ([(int(a), int(b)) for a, b in rng.integers(32, 257, size=(1024, 2))], 4),
+    }
+
+
+def bench_set(args, dev, torch):
+    lib = gb.load_library()
+    out = {}
+    for name, (shapes, q) in set_workloads().items():
+        k = len(shapes)
+        cap = args.sizes_capacity
+        u0 = [synth.gradnoise(h, w, 100 + i).astype(int) for i, (h, w) in enumerate(shapes)]
+        orig = [linear(x.astype(np.uint8)) for x in u0]
+        index = [i for i in range(k) for _ in range(q)]  # the candidates of an original are consecutive
+        cands = [linear(np.clip(u0[i] + synth.noise(*shapes[i], 900 + j) % (3 + 2 * (j % q)) - (1 + j % q), 0, 255)
+                        .astype(np.uint8)) for j, i in enumerate(index)]
+        orig_dev = [torch.from_numpy(x).to(dev) for x in orig]
+        cands_dev = [torch.from_numpy(x).to(dev) for x in cands]
+        torch.cuda.synchronize(dev)
+        n = len(index)
+        bh, bw = max(s[0] for s in shapes), max(s[1] for s in shapes)
+
+        def free_mib():
+            lib.gb200_trim_memory()
+            torch.cuda.synchronize(dev)
+            return torch.cuda.mem_get_info(dev)[0] / 2**20
+
+        memory = {}
+        f0 = free_mib()
+        cset = gb.ComparatorSet(orig, capacity=cap, device=args.device)
+        memory["set_mib"] = round(f0 - free_mib(), 1)
+        f0 = free_mib()
+        batch = gb.ButteraugliBatch(bh, bw, cap, device=args.device)
+        memory["sizes_batch_mib"] = round(f0 - free_mib(), 1)
+        cmps = None
+        if name == "kodak":
+            f0 = free_mib()
+            cmps = [gb.Comparator(x, device=args.device, capacity=q) for x in orig]
+            memory["comparators_mib"] = round(f0 - free_mib(), 1)
+            stacked = [torch.stack(cands_dev[i * q:(i + 1) * q]) for i in range(k)]
+            torch.cuda.synchronize(dev)
+
+        def in_calls(f, a, b):
+            scores = []
+            for j in range(0, n, cap):
+                scores += f(a[j:j + cap], b[j:j + cap])[1].tolist()
+            return scores
+
+        def set_cuda():
+            return in_calls(cset.diffmap, index, cands_dev)
+
+        def set_host():
+            return in_calls(cset.diffmap, index, cands)
+
+        def sizes_cuda():
+            return in_calls(batch.diffmap_sizes, [orig_dev[i] for i in index], cands_dev)
+
+        def sizes_host():
+            return in_calls(batch.diffmap_sizes, [orig[i] for i in index], cands)
+
+        def comparators_cuda():
+            return [v for i in range(k) for v in cmps[i].diffmap(stacked[i])[1].tolist()]
+
+        modes = {"set_cuda": set_cuda, "set_host": set_host, "sizes_cuda": sizes_cuda, "sizes_host": sizes_host}
+        if cmps is not None:
+            modes["comparators_cuda"] = comparators_cuda
+        scores, h2d = {}, {}
+        for m, f in modes.items():  # also the warm-up
+            before = gb.counters()[1]
+            scores[m] = f()
+            h2d[m] = (gb.counters()[1] - before) / n
+        ms = {m: [] for m in modes}
+        for _ in range(args.rounds):
+            for m, f in modes.items():
+                torch.cuda.synchronize(dev)
+                t0 = time.perf_counter()
+                f()
+                torch.cuda.synchronize(dev)
+                ms[m].append((time.perf_counter() - t0) * 1e3 / n)
+        cset.close()
+        batch.close()
+        for c in cmps or []:
+            c.close()
+        out[name] = {"originals": k, "candidates_per_original": q, "candidates": n, "calls_of": cap,
+                     "distinct_sizes": len(set(shapes)), "batch": f"{bw}x{bh}",
+                     "ms_per_candidate": {m: {"median": round(statistics.median(v), 4), "min": round(min(v), 4),
+                                              "max": round(max(v), 4)} for m, v in ms.items()},
+                     "h2d_kib_per_candidate": {m: round(h2d[m] / 1024, 1) for m in ("set_host", "sizes_host")},
+                     "scores_identical": all(v == scores["set_cuda"] for v in scores.values()),
+                     "device_memory": memory}
     return out
 
 
