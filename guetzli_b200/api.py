@@ -59,6 +59,16 @@ def load_library(path=None):
                                       C.c_void_p, P(P(C.c_uint8)), P(C.c_size_t), P(_CStats)]
     lib.gb200_process_jpeg.argtypes = [P(_CParams), C.c_void_p, C.c_size_t, C.c_int, _LOG_FN,
                                        C.c_void_p, P(P(C.c_uint8)), P(C.c_size_t), P(_CStats)]
+    process_image = [P(_CParams), C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, _LOG_FN, C.c_void_p,
+                     P(P(C.c_uint8)), P(C.c_size_t), P(_CStats)]
+    lib.gb200_process_image.argtypes = process_image
+    lib.gb200_process_image_device.argtypes = process_image + [C.c_void_p]
+    lib.gb200_image_create_strided.restype = C.c_void_p
+    lib.gb200_image_create_strided.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int]
+    lib.gb200_image_create_device.restype = C.c_void_p
+    lib.gb200_image_create_device.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int,
+                                              C.c_void_p]
+    lib.gb200_image_rgb.argtypes = [C.c_void_p, C.c_void_p]
     lib.gb200_free.argtypes = [C.c_void_p]
     lib.gb200_process_rgb_tiled_threads.argtypes = [P(_CParams), C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                                     P(P(C.c_uint8)), P(C.c_size_t), P(_CStats)]
@@ -253,6 +263,66 @@ def process(params, stats, rgb, w, h, device=0, lib=None):
     data = _take(lib, out, out_len)
     _fill_stats(stats, cs)
     if not ok and not data:
+        _raise_device_error(lib)
+    return bool(ok), data
+
+
+def _image_view(image):
+    """Checks the 8-bit image of process_image and DeviceImage.from_image: a uint8 numpy array or torch tensor
+    (host or CUDA) of shape [h][w] (gray) or [h][w][C] with C = 1 (gray), 2 (gray + alpha), 3 (RGB) or 4 (RGBA),
+    taken as it is laid out, strides and storage offset included -> (pointer, w, h, C, strides int64[3] in
+    bytes, the torch device of a CUDA tensor or None, the object that owns the memory)."""
+    if _is_torch_tensor(image):
+        import torch
+        if image.dtype != torch.uint8:
+            raise ValueError(f"image must be uint8, got {image.dtype}")
+        shape, strides, ptr = tuple(image.shape), tuple(image.stride()), image.data_ptr()
+        dev = image.device if image.is_cuda else None
+    else:
+        image = np.asarray(image)
+        if image.dtype != np.uint8:
+            raise ValueError(f"image must be uint8, got {image.dtype}")
+        shape, strides, ptr, dev = image.shape, image.strides, image.ctypes.data, None
+    if len(shape) not in (2, 3):
+        raise ValueError(f"image must have 2 or 3 axes ([h][w] or [h][w][C]), got shape {shape}")
+    if len(shape) == 2:
+        shape, strides = shape + (1,), strides + (0,)
+    if shape[2] not in (1, 2, 3, 4):
+        raise ValueError("image must have 1 (gray), 2 (gray + alpha), 3 (RGB) or 4 (RGBA) channels in its last "
+                         f"axis, got shape {shape}")
+    if min(strides) < 0:
+        raise ValueError(f"image must have non-negative strides, got {strides}")
+    h, w, ch = shape
+    return ptr, w, h, ch, np.array(strides, dtype=np.int64), dev, image
+
+
+def process_image(params, stats, image, device=0, lib=None):
+    """guetzli::Process on an 8-bit image of any channel count, converted to RGB as the guetzli tool converts
+    PNG layouts (guetzli.cc:43-145): gray replicated, gray + alpha and RGBA blended on black with
+    (v * a + 128) // 255, RGB as it is.  Returns (ok, jpeg_bytes) like process().
+
+    image: uint8 [h][w] or [h][w][C], C = 1..4, a numpy array or a torch tensor, read with its strides and
+    storage offset as they are (no contiguous copy).  Host memory is uploaded (the span the view covers) and
+    encoded on `device`; a CUDA tensor is read in place on its own device, after the work queued on that
+    device's current torch stream, and nothing of it crosses to the host.  Malformed images raise ValueError;
+    the encoder's own refusals return (False, b"") as process() does, with the message in last_error()."""
+    lib = lib or load_library()
+    ptr, w, h, ch, strides, dev, _owner = _image_view(image)
+    cp, cs = _cparams(params), _CStats()
+    cb = _log_sink(stats)
+    out, out_len = C.POINTER(C.c_uint8)(), C.c_size_t()
+    args = (C.byref(cp), ptr, w, h, ch, strides.ctypes.data)
+    tail = (cb, None, C.byref(out), C.byref(out_len), C.byref(cs))
+    if dev is not None:
+        import torch
+        ok = lib.gb200_process_image_device(*args, dev.index, *tail, torch.cuda.current_stream(dev).cuda_stream)
+    else:
+        ok = lib.gb200_process_image(*args, device, *tail)
+    data = _take(lib, out, out_len)
+    _fill_stats(stats, cs)
+    if not ok and not data:
+        if "device memory" in _err(lib):  # a pointer the device entry refused
+            raise RuntimeError(_err(lib))
         _raise_device_error(lib)
     return bool(ok), data
 
@@ -922,6 +992,32 @@ class DeviceImage(_Handle):
             raise RuntimeError("gb200_image_create failed: " + _err(self.lib))
         self.nblocks = self.lib.gb200_image_num_blocks(self._h)
 
+    @classmethod
+    def from_image(cls, image, device=0, prepare=True, lib=None):
+        """A resident image made from an 8-bit image of any channel count and layout, converted to RGB on the
+        device as process_image converts it.  A CUDA tensor is read in place on its own device after the work
+        queued on that device's current torch stream; host memory goes to `device`.  The image has been read
+        when this returns, so the caller may overwrite it right away."""
+        self = cls.__new__(cls)
+        self.lib = lib or load_library()
+        ptr, self.w, self.h, ch, strides, dev, _owner = _image_view(image)
+        if dev is not None:
+            import torch
+            self._h = self.lib.gb200_image_create_device(ptr, self.w, self.h, ch, strides.ctypes.data, dev.index,
+                                                         int(prepare), torch.cuda.current_stream(dev).cuda_stream)
+        else:
+            self._h = self.lib.gb200_image_create_strided(ptr, self.w, self.h, ch, strides.ctypes.data, device,
+                                                          int(prepare))
+        if not self._h:
+            raise RuntimeError("gb200_image_create failed: " + _err(self.lib))
+        self.nblocks = self.lib.gb200_image_num_blocks(self._h)
+        return self
+
+    def rgb(self):
+        """The resident image's RGB as the encoder sees it, uint8 [h][w][3]."""
+        out = np.empty((self.h, self.w, 3), dtype=np.uint8)
+        self._ck(self.lib.gb200_image_rgb(self._h, out.ctypes.data))
+        return out
 
     def reset(self):
         """Forget the one-time results: the next process() repeats the whole job."""

@@ -271,6 +271,56 @@ int gb200_process_rgb(const gb200_params* params, const uint8_t* rgb, int w, int
   return (guarded_ok && ok) ? 1 : 0;
 }
 
+namespace {
+// the encoder's result and counters into the C outputs
+void take_jpeg(const std::string& jpeg, const gb200::SearchStats& st, uint8_t** out, size_t* out_len,
+               gb200_stats* stats) {
+  if (!jpeg.empty()) {
+    *out = static_cast<uint8_t*>(malloc(jpeg.size()));
+    memcpy(*out, jpeg.data(), jpeg.size());
+    *out_len = jpeg.size();
+  }
+  fill_stats(st, stats);
+}
+}  // namespace
+
+int gb200_process_image(const gb200_params* params, const uint8_t* img, int w, int h, int channels,
+                        const int64_t* strides, int device, gb200_log_fn log, void* log_user, uint8_t** out,
+                        size_t* out_len, gb200_stats* stats) {
+  *out = nullptr;
+  *out_len = 0;
+  bool ok = false;
+  int guarded_ok = guarded([&]() {
+    gb200::SearchStats st;
+    std::string jpeg, err;
+    ok = gb200::process_image(to_search_params(params), img, w, h, channels, strides, device, log, log_user, &jpeg,
+                              &st, &err);
+    if (!ok) g_err = err;
+    take_jpeg(jpeg, st, out, out_len, stats);
+  });
+  return (guarded_ok && ok) ? 1 : 0;
+}
+
+int gb200_process_image_device(const gb200_params* params, const uint8_t* img_dev, int w, int h, int channels,
+                               const int64_t* strides, int device, gb200_log_fn log, void* log_user, uint8_t** out,
+                               size_t* out_len, gb200_stats* stats, void* stream) {
+  *out = nullptr;
+  *out_len = 0;
+  bool ok = false;
+  int guarded_ok = guarded([&]() {
+    const void* ptrs[1] = {img_dev};
+    const char* what[1] = {"img"};
+    check_device_pointers("process_image_device", device, ptrs, what, 1);
+    gb200::SearchStats st;
+    std::string jpeg, err;
+    ok = gb200::process_image_device(to_search_params(params), img_dev, w, h, channels, strides, device,
+                                     caller_stream(stream), log, log_user, &jpeg, &st, &err);
+    if (!ok) g_err = err;
+    take_jpeg(jpeg, st, out, out_len, stats);
+  });
+  return (guarded_ok && ok) ? 1 : 0;
+}
+
 int gb200_process_jpeg(const gb200_params* params, const uint8_t* jpeg_in, size_t jpeg_len, int device,
                        gb200_log_fn log, void* log_user, uint8_t** out, size_t* out_len, gb200_stats* stats) {
   *out = nullptr;
@@ -979,6 +1029,46 @@ gb200_image* gb200_image_create2(const uint8_t* rgb, int w, int h, int device, i
     img->ctx = ctx;
   });
   return img;
+}
+
+namespace {
+// a resident image from an 8-bit view: create2's checks and messages, then the view's
+gb200_image* image_from_view(const uint8_t* data, int w, int h, int channels, const int64_t* strides, int device,
+                             int prepare, bool on_device, void* stream) {
+  gb200_image* img = nullptr;
+  guarded([&]() {
+    if (on_device) {
+      const void* ptrs[1] = {data};
+      const char* what[1] = {"img"};
+      check_device_pointers("image_create_device", device, ptrs, what, 1);
+    }
+    if (!data || w <= 0 || h <= 0 || w >= 65536 || h >= 65536) throw std::runtime_error("bad image size");
+    std::string why;
+    gb200::ImageView view;
+    if (!gb200::image_view(data, w, channels, strides, &view, &why)) throw std::runtime_error(why);
+    if (!gb200::image_size_supported(w, h, &why)) throw std::runtime_error(why);
+    view.device = on_device;
+    view.stream = caller_stream(stream);
+    gb200::ImageContext* ctx = new gb200::ImageContext(view, w, h, device, prepare != 0);
+    img = new gb200_image;
+    img->ctx = ctx;
+  });
+  return img;
+}
+}  // namespace
+
+gb200_image* gb200_image_create_strided(const uint8_t* img, int w, int h, int channels, const int64_t* strides,
+                                        int device, int prepare) {
+  return image_from_view(img, w, h, channels, strides, device, prepare, false, nullptr);
+}
+
+gb200_image* gb200_image_create_device(const uint8_t* img_dev, int w, int h, int channels, const int64_t* strides,
+                                       int device, int prepare, void* stream) {
+  return image_from_view(img_dev, w, h, channels, strides, device, prepare, true, stream);
+}
+
+int gb200_image_rgb(gb200_image* img, uint8_t* out) {
+  return guarded([&]() { img->ctx->download_rgb(out); });
 }
 
 void gb200_image_destroy(gb200_image* img) {

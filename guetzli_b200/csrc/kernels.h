@@ -58,6 +58,46 @@ struct FdctBlocks {
   }
 };
 
+// BlendOnBlack of the guetzli tool (g/guetzli.cc:43-45): an 8-bit sample under 8-bit alpha, laid over
+// black in integers.  Not the butteraugli tool's rule (srgb_over_linear rounds with + 127, not + 128).
+GB_HD int blend_on_black(int v, int a) { return (v * a + 128) / 255; }
+
+// An 8-bit image of C = 1..4 channels in any strided layout -> packed sRGB [h][w][3], converted as the
+// guetzli tool converts the PNG layouts before Process (ReadPNG, g/guetzli.cc:43-145): gray replicated
+// (C = 1), gray + alpha blended on black and replicated (C = 2), RGB copied (C = 3), RGBA with each of
+// R, G, B blended on black under the pixel's alpha (C = 4).  Sample (y, x, c) is at byte
+// y rs + x ps + c cs of src; strides may be 0 (a broadcast view).  Launched over w x h.
+struct IngestU8 {
+  const uint8_t* src;
+  long long rs, ps, cs;  // row, pixel and channel strides in bytes
+  int C;
+  uint8_t* rgb;  // [h][w][3]
+  int w;
+  GB_HD void operator()(int x, int y) const {
+    const uint8_t* p = src + y * rs + x * ps;
+    int r, g, b;
+    if (C <= 2) {
+      r = p[0];
+      if (C == 2) r = blend_on_black(r, p[cs]);
+      g = b = r;
+    } else {
+      r = p[0];
+      g = p[cs];
+      b = p[2 * cs];
+      if (C == 4) {
+        const int a = p[3 * cs];
+        r = blend_on_black(r, a);
+        g = blend_on_black(g, a);
+        b = blend_on_black(b, a);
+      }
+    }
+    uint8_t* o = rgb + 3 * (static_cast<size_t>(y) * w + x);
+    o[0] = static_cast<uint8_t>(r);
+    o[1] = static_cast<uint8_t>(g);
+    o[2] = static_cast<uint8_t>(b);
+  }
+};
+
 // Original image u8 sRGB -> linear float planes (g/butteraugli_comparator.cc:33).
 struct LinearizeRgb {
   const uint8_t* rgb;

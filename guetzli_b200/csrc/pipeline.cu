@@ -1085,12 +1085,18 @@ ImageContext::ImageContext(const int16_t* dq_coeffs, int w, int h, int device, b
   guarded_init(nullptr, dq_coeffs, prepare_now);
 }
 
+ImageContext::ImageContext(const ImageView& view, int w, int h, int device, bool prepare_now)
+    : ba_(w, h, device, nullptr) {
+  guarded_init(nullptr, nullptr, prepare_now, &view);
+}
+
 // A constructor that throws never reaches the destructor: the encoder's buffers acquired so far are
 // handed back here, and the metric, a member constructed by then, hands back its own and the
 // stream, so that an out-of-memory condition does not become permanent for the process.
-void ImageContext::guarded_init(const uint8_t* rgb, const int16_t* dq_coeffs, bool prepare_now) {
+void ImageContext::guarded_init(const uint8_t* rgb, const int16_t* dq_coeffs, bool prepare_now,
+                                const ImageView* view) {
   try {
-    init(rgb, dq_coeffs, prepare_now);
+    init(rgb, dq_coeffs, prepare_now, view);
   } catch (...) {
     release();
     throw;
@@ -1102,7 +1108,29 @@ void ImageContext::download_rgb(uint8_t* rgb) {
   d2h(rgb, d_rgb_, static_cast<size_t>(3) * g_.w * g_.h, s_);
 }
 
-void ImageContext::init(const uint8_t* rgb, const int16_t* dq_coeffs, bool prepare_now) {
+// The view's pixels into d_rgb_ (IngestU8), read before this returns.  A host view's span goes through
+// a staging buffer, the last one owned: if anything throws, release() waits for the stream and frees it
+// with the rest; otherwise it is freed here once the kernel has read it.
+void ImageContext::ingest(const ImageView& view) {
+  const uint8_t* src = view.data;
+  if (view.device) {
+    stream_wait(s_, view.stream);
+  } else {
+    const size_t span = view.span(g_.w, g_.h);
+    void* staged = own(span);
+    h2d(staged, view.data, span, s_);
+    src = static_cast<const uint8_t*>(staged);
+  }
+  launch_2d(s_, IngestU8{src, view.stride[0], view.stride[1], view.stride[2], view.channels, d_rgb_, g_.w}, g_.w, g_.h,
+            "ingest_u8");
+  stream_sync(s_);
+  if (!view.device) {
+    dev_free(owned_.back());
+    owned_.pop_back();
+  }
+}
+
+void ImageContext::init(const uint8_t* rgb, const int16_t* dq_coeffs, bool prepare_now, const ImageView* view) {
   const int w = g_.w, h = g_.h;
   const size_t ncoef = static_cast<size_t>(3) * g_.nblocks * 64;
   d_rgb_ = static_cast<uint8_t*>(own(static_cast<size_t>(3) * w * h));
@@ -1134,6 +1162,8 @@ void ImageContext::init(const uint8_t* rgb, const int16_t* dq_coeffs, bool prepa
   d_dirty_ = static_cast<int*>(own(sizeof(int) * g_.nblocks));
   if (from_coeffs_) {
     h2d(d_orig_, dq_coeffs, static_cast<size_t>(3) * g_.nblocks * 64 * sizeof(int16_t), s_);
+  } else if (view != nullptr) {
+    ingest(*view);
   } else {
     h2d(d_rgb_, rgb, static_cast<size_t>(3) * w * h, s_);
   }

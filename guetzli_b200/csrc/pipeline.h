@@ -16,6 +16,22 @@ namespace gb200 {
 struct OrderItem;
 struct OrderSelectState;
 
+// An 8-bit image of 1 (gray), 2 (gray + alpha), 3 (RGB) or 4 (RGBA) channels in any layout with
+// non-negative strides: sample (y, x, c) is at byte y * stride[0] + x * stride[1] + c * stride[2] of data.
+struct ImageView {
+  const uint8_t* data = nullptr;
+  int channels = 3;
+  int64_t stride[3] = {0, 0, 0};  // bytes: row, pixel, channel
+  // data is memory of the context's device, read in place once the work queued on `stream` so far is
+  // done; otherwise host memory
+  bool device = false;
+  Stream stream = 0;
+  // bytes from data to the last sample of a w x h image, inclusive: the span a host view uploads
+  size_t span(int w, int h) const {
+    return static_cast<size_t>((h - 1) * stride[0] + (w - 1) * stride[1] + (channels - 1) * stride[2] + 1);
+  }
+};
+
 class ImageContext {
  public:
   // Uploads the image, runs the one-time kernels (a2 FDCT, a3 PsychoImage of the
@@ -26,6 +42,11 @@ class ImageContext {
   // JPEG input (4:4:4): the original is given as dequantised DCT coefficients
   // [3][nblocks][64]; its pixels (DecodeJpegToRGB) are rendered on the device.
   ImageContext(const int16_t* dq_coeffs, int w, int h, int device, bool prepare_now, Comm* comm);
+  // An 8-bit view (ImageView) turned into the packed RGB of the first constructor on the device, as the
+  // guetzli tool turns PNG layouts into RGB (IngestU8, kernels.h); everything after that is the RGB path.
+  // A device view is read in place after the work queued on its stream; a host view's span is uploaded
+  // into a staging buffer.  Either way the view has been read when the constructor returns.
+  ImageContext(const ImageView& view, int w, int h, int device, bool prepare_now);
   // EXPERIMENTAL (order_exact.h, GB200_DEVICE_ORDER=1): the reference-ordered candidate list
   // and the introsort partition passes over large ranges on the device.  Returns k_end and the
   // first k_end entries exactly as std::sort would leave them (exact_sort.h semantics).
@@ -251,8 +272,9 @@ class ImageContext {
   void gather_reserve(size_t n);
   void gather_fetch(size_t n, std::vector<int16_t>* coeffs, std::vector<int>* cursor, std::vector<int>* in_bulk);
   bool from_coeffs_ = false;  // original given as coefficients (JPEG input)
-  void guarded_init(const uint8_t* rgb, const int16_t* dq_coeffs, bool prepare_now);
-  void init(const uint8_t* rgb, const int16_t* dq_coeffs, bool prepare_now);
+  void guarded_init(const uint8_t* rgb, const int16_t* dq_coeffs, bool prepare_now, const ImageView* view = nullptr);
+  void init(const uint8_t* rgb, const int16_t* dq_coeffs, bool prepare_now, const ImageView* view);
+  void ingest(const ImageView& view);
   void release();
   float* weights_ = nullptr;    // [nblocks]
   float* zero_block_max_ = nullptr;

@@ -1513,4 +1513,77 @@ bool process_rgb_tiled(const SearchParams& params, const uint8_t* rgb, int w, in
   return ok;
 }
 
+bool image_view(const uint8_t* img, int w, int channels, const int64_t* strides, ImageView* view, std::string* err) {
+  char buf[192];
+  if (channels < 1 || channels > 4) {
+    snprintf(buf, sizeof(buf),
+             "guetzli_b200: an image has 1 (gray), 2 (gray + alpha), 3 (RGB) or 4 (RGBA) channels, got %d\n",
+             channels);
+    *err = buf;
+    fputs(buf, stderr);
+    return false;
+  }
+  if (strides != nullptr && (strides[0] < 0 || strides[1] < 0 || strides[2] < 0)) {
+    snprintf(buf, sizeof(buf), "guetzli_b200: image strides must not be negative, got row %lld, pixel %lld, channel %lld\n",
+             static_cast<long long>(strides[0]), static_cast<long long>(strides[1]), static_cast<long long>(strides[2]));
+    *err = buf;
+    fputs(buf, stderr);
+    return false;
+  }
+  view->data = img;
+  view->channels = channels;
+  view->stride[0] = strides ? strides[0] : static_cast<int64_t>(w) * channels;
+  view->stride[1] = strides ? strides[1] : channels;
+  view->stride[2] = strides ? strides[2] : 1;
+  return true;
+}
+
+namespace {
+// process_rgb_tiled's checks, messages and accounting (one GPU) on an image view
+bool process_view(const SearchParams& params, const uint8_t* img, int w, int h, int channels, const int64_t* strides,
+                  int device, bool on_device, Stream stream, LogSink log, void* log_user, std::string* jpeg_out,
+                  SearchStats* stats, std::string* err) {
+  SearchStats local;
+  SearchStats* st = stats ? stats : &local;
+  *st = SearchStats();
+  jpeg_out->clear();
+  if (img == nullptr || w < 0 || w >= 1 << 16 || h < 0 || h >= 1 << 16) {
+    *err = "Could not create jpg data from rgb pixels\n";
+    fputs(err->c_str(), stderr);
+    return false;
+  }
+  ImageView view;
+  if (!image_view(img, w, channels, strides, &view, err)) return false;
+  view.device = on_device;
+  view.stream = stream;
+  if (!check_params(params, err)) return false;
+  if (w == 0 || h == 0) {
+    *err = "guetzli_b200: empty image\n";
+    fputs(err->c_str(), stderr);
+    return false;
+  }
+  if (!image_size_supported(w, h, err)) return false;
+  Clock::time_point t0 = Clock::now();
+  const long long h2d0 = h2d_bytes_total();
+  ImageContext ctx(view, w, h, device, false);
+  st->ms_device_setup = ms_since(t0);
+  const bool ok = process_resident(params, &ctx, log, log_user, jpeg_out, st, err);
+  st->h2d_bytes = h2d_bytes_total() - h2d0;
+  st->ms_total = ms_since(t0);
+  return ok;
+}
+}  // namespace
+
+bool process_image(const SearchParams& params, const uint8_t* img, int w, int h, int channels, const int64_t* strides,
+                   int device, LogSink log, void* log_user, std::string* jpeg_out, SearchStats* stats,
+                   std::string* err) {
+  return process_view(params, img, w, h, channels, strides, device, false, 0, log, log_user, jpeg_out, stats, err);
+}
+
+bool process_image_device(const SearchParams& params, const uint8_t* img, int w, int h, int channels,
+                          const int64_t* strides, int device, Stream stream, LogSink log, void* log_user,
+                          std::string* jpeg_out, SearchStats* stats, std::string* err) {
+  return process_view(params, img, w, h, channels, strides, device, true, stream, log, log_user, jpeg_out, stats, err);
+}
+
 }  // namespace gb200

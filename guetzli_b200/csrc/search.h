@@ -7,7 +7,11 @@
 
 #include <string>
 
+#include "backend.h"
+
 namespace gb200 {
+
+struct ImageView;
 
 // Mirrors guetzli::Params (g/processor.h:29-37).
 struct SearchParams {
@@ -57,6 +61,22 @@ bool process_jpeg(const SearchParams& params, const uint8_t* data, size_t len, i
 
 bool process_rgb(const SearchParams& params, const uint8_t* rgb, int w, int h, int device, LogSink log,
                  void* log_user, std::string* jpeg_out, SearchStats* stats, std::string* err);
+
+// Process(RGB) on an 8-bit image of 1 (gray), 2 (gray + alpha), 3 (RGB) or 4 (RGBA) channels, turned into
+// RGB on the device as the guetzli tool turns PNG layouts into RGB (g/guetzli.cc:43-145; ImageContext's
+// ImageView source).  strides: bytes per row, pixel and channel, or null for contiguous [h][w][channels].
+// process_image reads img from host memory; process_image_device reads it in place from memory of `device`
+// once the work queued on `stream` so far is done.  The checks and messages of process_rgb, plus refusals
+// of channels outside 1..4 and of negative strides; then the RGB path.
+bool process_image(const SearchParams& params, const uint8_t* img, int w, int h, int channels, const int64_t* strides,
+                   int device, LogSink log, void* log_user, std::string* jpeg_out, SearchStats* stats,
+                   std::string* err);
+bool process_image_device(const SearchParams& params, const uint8_t* img, int w, int h, int channels,
+                          const int64_t* strides, int device, Stream stream, LogSink log, void* log_user,
+                          std::string* jpeg_out, SearchStats* stats, std::string* err);
+// The view of such an image (on the host; the caller sets device and stream), or false + message when
+// channels is outside 1..4 or a stride is negative.
+bool image_view(const uint8_t* img, int w, int channels, const int64_t* strides, ImageView* view, std::string* err);
 
 // a11 as a call of its own (SaveToJpegData + WriteJpeg, g/output_image.cc:348, g/jpeg_data_writer.cc:540):
 // the JPEG file of the context's current candidate, whose coefficients are multiples of q[3][64];

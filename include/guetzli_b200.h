@@ -69,6 +69,28 @@ int gb200_process_rgb(const gb200_params* params, const uint8_t* rgb, int w, int
                       gb200_log_fn log, void* log_user, uint8_t** out, size_t* out_len,
                       gb200_stats* stats);
 
+/* ---- 8-bit images of any channel count and layout, from host or device memory ----
+ * img holds w x h pixels of `channels` 8-bit samples: 1 (gray), 2 (gray + alpha), 3 (RGB) or 4 (RGBA).
+ * Sample (y, x, c) is at byte y * strides[0] + x * strides[1] + c * strides[2] of img; strides (int64[3]:
+ * row, pixel, channel bytes, each >= 0, 0 allowed for a broadcast view) may be NULL for contiguous
+ * [h][w][channels].  The image is turned into RGB on the device as the guetzli tool turns PNG layouts into
+ * RGB before guetzli::Process (guetzli/guetzli.cc:43-145): gray is replicated, gray + alpha and RGBA are
+ * blended on black per sample with (v * a + 128) / 255 in integers (BlendOnBlack; not the butteraugli
+ * tool's rule, which rounds with + 127), RGB is copied.  The encoder then runs as gb200_process_rgb runs on
+ * that RGB, with its checks and messages; channels outside 1..4 and negative strides are refused as well.
+ *
+ * gb200_process_image: img in host memory; the smallest span of bytes that covers the view is uploaded. */
+int gb200_process_image(const gb200_params* params, const uint8_t* img, int w, int h, int channels,
+                        const int64_t* strides, int device, gb200_log_fn log, void* log_user, uint8_t** out,
+                        size_t* out_len, gb200_stats* stats);
+/* The same with img in device memory of `device`, read in place once the work queued on `stream` so far is
+ * done (a cudaStream_t, NULL = the legacy default stream); nothing of the image crosses to the host.  The
+ * image has been read when the call returns.  A host, managed or other device's pointer is refused, nothing
+ * runs. */
+int gb200_process_image_device(const gb200_params* params, const uint8_t* img_dev, int w, int h, int channels,
+                               const int64_t* strides, int device, gb200_log_fn log, void* log_user, uint8_t** out,
+                               size_t* out_len, gb200_stats* stats, void* stream);
+
 /* guetzli::Process(params, stats, jpeg_in, &out) (guetzli/processor.h:39-41,
  * guetzli/processor.cc:890): JPEG input.  The file is parsed on the host
  * (ReadJpeg, guetzli/jpeg_data_reader.cc:931); its coefficients and quant tables
@@ -309,6 +331,16 @@ typedef struct gb200_image gb200_image;
 gb200_image* gb200_image_create(const uint8_t* rgb, int w, int h, int device);
 /* prepare=0: upload only; the one-time kernels then run inside gb200_image_process */
 gb200_image* gb200_image_create2(const uint8_t* rgb, int w, int h, int device, int prepare);
+/* A resident image from an 8-bit view (channels, strides and conversion as in gb200_process_image), img
+ * in host memory.  The image has been read and converted when the call returns, whatever `prepare`. */
+gb200_image* gb200_image_create_strided(const uint8_t* img, int w, int h, int channels, const int64_t* strides,
+                                        int device, int prepare);
+/* The same with img in device memory of `device`, read in place after the work queued on `stream` (as in
+ * gb200_process_image_device); the caller may overwrite or free it once the call returns. */
+gb200_image* gb200_image_create_device(const uint8_t* img_dev, int w, int h, int channels, const int64_t* strides,
+                                       int device, int prepare, void* stream);
+/* test hook: the resident image's RGB as the encoder sees it, [h][w][3] into out */
+int gb200_image_rgb(gb200_image* img, uint8_t* out);
 void gb200_image_destroy(gb200_image* img);
 /* guetzli::Process on an image that is already resident in HBM (same result as
  * gb200_process_rgb; used to time the job without the host->device upload) */
