@@ -101,6 +101,9 @@ def load_library(path=None):
     lib.gb200_profile_enable.argtypes = [C.c_int]
     lib.gb200_profile_get.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
     lib.gb200_debug_read_jpeg.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t]
+    lib.gb200_jpeg_dimensions.argtypes = [C.c_void_p, C.c_size_t, P(C.c_int), P(C.c_int)]
+    lib.gb200_jpeg_decode_rgb.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]
+    lib.gb200_jpeg_decode_rgb_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
     lib.gb200_butteraugli_diffmap.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                               P(C.c_double)]
     lib.gb200_butteraugli_comparator_create.restype = C.c_void_p
@@ -342,6 +345,50 @@ def process_jpeg(params, stats, jpeg_in, device=0, lib=None):
     if not ok and not data:
         _raise_device_error(lib)
     return bool(ok), data
+
+
+def decode_jpeg(data, device=0, cuda=True, lib=None):
+    """The pixels libjpeg-turbo gives for JPEG files, as the butteraugli tool reads them (ReadJPEG,
+    butteraugli_main.cc:157: JDCT_ISLOW, fancy upsampling, RGB, gray replicated), decoded on the GPU.
+
+    data: one bytes-like object, or a list of them (decoded together in one pass whatever their sizes).
+    Returns a uint8 [h][w][3] CUDA tensor on cuda:`device` per file, written after the work queued on that
+    device's current torch stream, or a numpy array where cuda is False; a list for a list.  They go as
+    they are into the 8-bit butteraugli entries (butteraugli_srgb, diffmap_sizes_srgb, from_srgb).
+    A file the decoder does not reproduce libjpeg on raises ValueError naming its index and the reason:
+    what ReadJpeg rejects, CMYK / YCCK, samplings other than 4:4:4, 4:2:2 and 4:2:0, and progressive files
+    that libjpeg would block-smooth."""
+    lib = lib or load_library()
+    single = isinstance(data, (bytes, bytearray, memoryview))
+    files = [bytes(d) for d in ([data] if single else data)]
+    if not files:
+        raise ValueError("decode_jpeg: no files")
+    bufs = [np.frombuffer(f, dtype=np.uint8) for f in files]
+    shapes = []
+    for b in bufs:
+        w, h = C.c_int(), C.c_int()
+        ok = b.size and lib.gb200_jpeg_dimensions(b.ctypes.data, b.size, C.byref(w), C.byref(h))
+        # a file without a readable frame size gets a 1x1 output; the decoder then refuses it with its reason
+        shapes.append((h.value, w.value, 3) if ok else (1, 1, 3))
+    n = len(files)
+    ptrs = (C.c_void_p * n)(*[b.ctypes.data if b.size else None for b in bufs])
+    lens = (C.c_size_t * n)(*[b.size for b in bufs])
+    if cuda:
+        import torch
+        dev = torch.device("cuda", device)
+        out = [torch.empty(s, dtype=torch.uint8, device=dev) for s in shapes]
+        outp = (C.c_void_p * n)(*[o.data_ptr() for o in out])
+        ok = lib.gb200_jpeg_decode_rgb_device(ptrs, lens, n, device, outp, torch.cuda.current_stream(dev).cuda_stream)
+    else:
+        out = [np.empty(s, dtype=np.uint8) for s in shapes]
+        outp = (C.c_void_p * n)(*[o.ctypes.data for o in out])
+        ok = lib.gb200_jpeg_decode_rgb(ptrs, lens, n, device, outp)
+    if not ok:
+        msg = _err(lib)
+        if ": file " in msg:
+            raise ValueError(msg)
+        raise RuntimeError(msg)
+    return out[0] if single else out
 
 
 def read_jpeg(jpeg_in, lib=None):

@@ -4,8 +4,9 @@
 // third_party/butteraugli/butteraugli/butteraugli_main.cc:362-455; the distance map
 // comes from gb200_butteraugli_diffmap_srgb (the tool's sRGB conversion and alpha rule in front of
 // ButteraugliInterface, butteraugli.cc:1858).
-// PNG input only: the reference decodes JPEG with libjpeg, whose IDCT this repo does
-// not reproduce, so JPEG arguments are refused instead of scored differently.
+// A JPEG argument (FF D8, as the tool sniffs it, butteraugli_main.cc:282-307) is decoded on the device by
+// gb200_jpeg_decode_rgb into the pixels the tool's ReadJPEG gets from libjpeg-turbo (RGB, gray replicated);
+// a file that decoder refuses is reported as the tool reports a JPEG it cannot read.
 #include <math.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -49,8 +50,27 @@ Picture ReadImageOrDie(const char* name) {
   }
   Picture p;
   if (static_cast<uint8_t>(data[0]) == 0xff && static_cast<uint8_t>(data[1]) == 0xd8) {
-    fprintf(stderr, "File %s is a JPEG; this build scores PNG input only (no libjpeg decoder).\n", name);
-    exit(1);
+    const uint8_t* bytes = reinterpret_cast<const uint8_t*>(data.data());
+    const size_t len = data.size();
+    std::vector<uint8_t> rgb;
+    bool ok = gb200_jpeg_dimensions(bytes, len, &p.w, &p.h) != 0;
+    if (ok) {
+      rgb.resize(static_cast<size_t>(3) * p.w * p.h);
+      uint8_t* out = rgb.data();
+      int device = 0;
+      if (const char* e = getenv("GUETZLI_B200_DEVICE")) device = atoi(e);
+      ok = gb200_jpeg_decode_rgb(&bytes, &len, 1, device, &out) != 0;
+    }
+    if (!ok) {
+      fprintf(stderr, "File %s is a malformed JPEG.\n", name);
+      exit(1);
+    }
+    p.rgba.resize(static_cast<size_t>(4) * p.w * p.h);
+    for (size_t i = 0; i < static_cast<size_t>(p.w) * p.h; ++i) {
+      for (int c = 0; c < 3; ++c) p.rgba[4 * i + c] = rgb[3 * i + c];
+      p.rgba[4 * i + 3] = 255;
+    }
+    return p;
   }
   if (!gb200_cli::ReadPNGRGBA(data, &p.w, &p.h, &p.rgba, &p.has_alpha)) {
     fprintf(stderr, "File %s is neither a valid JPEG nor a valid PNG.\n", name);

@@ -852,6 +852,52 @@ int gb200_jpeg_dimensions(const uint8_t* jpeg_in, size_t jpeg_len, int* width, i
   return gb200::read_jpeg_dimensions(jpeg_in, jpeg_len, width, height) ? 1 : 0;
 }
 
+namespace {
+// gb200_jpeg_decode_rgb[_device]: every file parsed and checked, and every output pointer, before anything
+// runs; a refusal names the file
+int jpeg_decode(const char* who, const uint8_t* const* jpeg, const size_t* len, int n, int device,
+                uint8_t* const* out, bool on_device, void* stream) {
+  return guarded([&]() {
+    if (n < 1) throw std::runtime_error(std::string(who) + ": n must be at least 1");
+    if (jpeg == nullptr || len == nullptr || out == nullptr)
+      throw std::runtime_error(std::string(who) + ": jpeg, len and out must not be null");
+    for (int i = 0; i < n; ++i) {
+      const std::string k = "[" + std::to_string(i) + "]";
+      if (jpeg[i] == nullptr) throw std::runtime_error(std::string(who) + ": jpeg" + k + " is null");
+      if (out[i] == nullptr) throw std::runtime_error(std::string(who) + ": out" + k + " is null");
+      if (on_device) {
+        const std::string name = "out" + k;
+        const void* ptrs[1] = {out[i]};
+        const char* what[1] = {name.c_str()};
+        check_device_pointers(who, device, ptrs, what, 1);
+      }
+    }
+    std::vector<gb200::JpegInput> files(n);
+    std::vector<const gb200::JpegInput*> ptrs(n);
+    for (int i = 0; i < n; ++i) {
+      const std::string file = std::string(who) + ": file " + std::to_string(i) + ": ";
+      std::string why;
+      if (!gb200::read_jpeg(jpeg[i], len[i], &files[i], &why)) throw std::runtime_error(file + why);
+      int w = 0, h = 0;
+      if (!gb200::read_jpeg_dimensions(jpeg[i], len[i], &w, &h) || w != files[i].width || h != files[i].height)
+        throw std::runtime_error(file + "the frame size differs from what gb200_jpeg_dimensions reads");
+      if (!gb200::libjpeg_decodable(files[i], &why)) throw std::runtime_error(file + why);
+      ptrs[i] = &files[i];
+    }
+    gb200::jpeg_decode_rgb(ptrs.data(), n, device, out, on_device, caller_stream(stream));
+  });
+}
+}  // namespace
+
+int gb200_jpeg_decode_rgb(const uint8_t* const* jpeg, const size_t* len, int n, int device, uint8_t* const* out) {
+  return jpeg_decode("jpeg_decode_rgb", jpeg, len, n, device, out, false, nullptr);
+}
+
+int gb200_jpeg_decode_rgb_device(const uint8_t* const* jpeg, const size_t* len, int n, int device,
+                                 uint8_t* const* out_dev, void* stream) {
+  return jpeg_decode("jpeg_decode_rgb_device", jpeg, len, n, device, out_dev, true, stream);
+}
+
 int gb200_debug_read_jpeg(const uint8_t* jpeg_in, size_t jpeg_len, int* dims, int16_t* out, size_t out_cap) {
   gb200::JpegInput jpg;
   std::string err;

@@ -8,6 +8,7 @@
 
 #include <algorithm>
 
+#include "jpeg_math.h"
 #include "tables.h"
 
 namespace gb200 {
@@ -38,6 +39,81 @@ bool has_ycbcr_color_space(const JpegInput& jpg) {
   }
   if (adobe) return transform != 0;
   return !(jpg.components[0].id == 'R' && jpg.components[1].id == 'G' && jpg.components[2].id == 'B');
+}
+
+bool libjpeg_ycbcr(const JpegInput& jpg) {
+  bool adobe = false;
+  uint8_t transform = 0;
+  for (const std::string& app : jpg.app_data) {
+    // app: marker byte, two length bytes, payload
+    const uint8_t marker = static_cast<uint8_t>(app[0]);
+    const size_t payload = app.size() - 3;
+    if (marker == 0xe0 && payload >= 14 && app.compare(3, 5, std::string("JFIF\0", 5)) == 0) return true;
+    if (marker == 0xee && payload >= 12 && app.compare(3, 5, "Adobe") == 0) {
+      adobe = true;
+      transform = static_cast<uint8_t>(app[3 + 11]);
+    }
+  }
+  if (adobe) return transform != 0;
+  return !(jpg.components[0].id == 'R' && jpg.components[1].id == 'G' && jpg.components[2].id == 'B');
+}
+
+bool libjpeg_decodable(const JpegInput& jpg, std::string* why) {
+  const int n = static_cast<int>(jpg.components.size());
+  if (n == 4) {
+    *why = "4 components (CMYK or YCCK): libjpeg gives no RGB or gray output for them";
+    return false;
+  }
+  if (n != 1 && n != 3) {
+    *why = std::to_string(n) + " components: libjpeg gives no RGB or gray output for them";
+    return false;
+  }
+  if (n == 3) {
+    const JpegComponent* c = jpg.components.data();
+    const bool layout = c[0].h_samp == jpg.max_h && c[0].v_samp == jpg.max_v && c[1].h_samp == 1 &&
+                        c[1].v_samp == 1 && c[2].h_samp == 1 && c[2].v_samp == 1 &&
+                        ((jpg.max_h == 1 && jpg.max_v == 1) || (jpg.max_h == 2 && jpg.max_v == 1) ||
+                         (jpg.max_h == 2 && jpg.max_v == 2));
+    if (!layout) {
+      *why = "sampling factors " + std::to_string(c[0].h_samp) + "x" + std::to_string(c[0].v_samp) + ", " +
+             std::to_string(c[1].h_samp) + "x" + std::to_string(c[1].v_samp) + ", " + std::to_string(c[2].h_samp) +
+             "x" + std::to_string(c[2].v_samp) + ": only 4:4:4, 4:2:2 and 4:2:0 are decoded";
+      return false;
+    }
+  }
+  // smoothing_ok (libjpeg-turbo 2.1 and later, jdcoefct.c): a progressive file is block-smoothed unless
+  // some component's DC was never coded, when a coefficient of zig-zag positions 1..9 of some component
+  // lacks its last bit (coef_bits != 0: never coded, or coded only down to a bit above 0)
+  if (jpg.progressive) {
+    bool dc_all = true, useful = false;
+    for (int c = 0; c < n && dc_all; ++c) {
+      dc_all = jpg.coded_bits[c][0] != 0;
+      for (int k = 1; k <= 9; ++k) useful |= (jpg.coded_bits[c][k] & 1) == 0;
+    }
+    if (dc_all && useful) {
+      *why = "progressive file with coefficients not refined to their last bit: libjpeg block-smooths it";
+      return false;
+    }
+  }
+  // libjpeg-turbo decodes through its SIMD IDCT where the CPU has one, and that computes libjpeg's
+  // integers only within its 16-bit ranges (jpeg_islow).  The exact test runs only on blocks of
+  // sum |coef q| > 2040: below that every pass-1 value and sum of them is under 5.66 x 2040 and the
+  // output under 2040 / 4 + 1 in magnitude, inside every range.
+  for (int c = 0; c < n; ++c) {
+    const JpegComponent& comp = jpg.components[c];
+    const int* q = jpg.quant[comp.quant_idx].values;
+    for (size_t b = 0; b < comp.coeffs.size(); b += 64) {
+      const int16_t* blk = &comp.coeffs[b];
+      long long t = 0;
+      for (int k = 0; k < 64; ++k) t += static_cast<long long>(blk[k] < 0 ? -blk[k] : blk[k]) * q[k];
+      if (t > 2040 && !jpeg_islow<true>(blk, q, nullptr, 0)) {
+        *why = "coefficients beyond the range in which libjpeg-turbo's SIMD IDCT computes its C IDCT's samples "
+               "(component " + std::to_string(c) + ", block " + std::to_string(b / 64) + ")";
+        return false;
+      }
+    }
+  }
+  return true;
 }
 
 bool check_jpeg_sanity(const JpegInput& jpg) {
@@ -215,6 +291,8 @@ class Reader {
     }
     if (num_dht_ == 0) return fail_("Need at least one Huffman code table.");
     if (num_dht_ >= 512) return fail_("Too many Huffman tables.");
+    jpg_->progressive = progressive_;
+    memcpy(jpg_->coded_bits, progression_, sizeof(progression_));
     return true;
   }
 

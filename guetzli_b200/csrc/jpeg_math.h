@@ -154,4 +154,147 @@ GB_HD int16_t fdct_descale(int16_t v) {
   return static_cast<int16_t>((v * 65537 + (0x80 << 12)) >> 20);
 }
 
+// ---------------------------------------------------------------------------
+// libjpeg's post-IDCT range limit: range_limit[x & RANGE_MASK] of the table of prepare_range_limit_table
+// (jdmaster.c), x the descaled output without its +128 centring.  The mask keeps 10 bits, so sums out of
+// [-512, 511] wrap before the clamp, as in libjpeg.
+GB_HD int jpeg_idct_limit(long long x) {
+  int v = static_cast<int>(x) & 1023;
+  if (v >= 512) v -= 1024;
+  v += 128;
+  return v < 0 ? 0 : (v > 255 ? 255 : v);
+}
+
+GB_HD bool jpeg_fits16(long long v) { return v >= -32768 && v <= 32767; }
+GB_HD bool jpeg_fits32(long long v) { return v >= -2147483647LL - 1 && v <= 2147483647LL; }
+
+// One 8-point pass of jpeg_islow: inputs in[0], in[s], .. in[7 s] (already dequantised), outputs
+// DESCALE(., sh) into out[0], out[s], ..; CHECK: *ok is cleared where a quantity leaves the range of
+// libjpeg-turbo's SIMD version (sums of inputs to 16 bits, products and sums to 32 bits).
+template <bool CHECK>
+GB_HD void jpeg_islow_pass(const long long* in, int s, int sh, long long* out, bool* ok) {
+  const long long F0298 = 2446, F0390 = 3196, F0541 = 4433, F0765 = 6270, F0899 = 7373, F1175 = 9633,
+                  F1501 = 12299, F1847 = 15137, F1961 = 16069, F2053 = 16819, F2562 = 20995, F3072 = 25172;
+  // even part
+  long long z2 = in[2 * s], z3 = in[6 * s];
+  long long z1 = (z2 + z3) * F0541;
+  long long tmp2 = z1 + z3 * -F1847, tmp3 = z1 + z2 * F0765;
+  const long long e0 = in[0] + in[4 * s], e1 = in[0] - in[4 * s];
+  long long tmp0 = static_cast<long long>(static_cast<unsigned long long>(e0) << 13);
+  long long tmp1 = static_cast<long long>(static_cast<unsigned long long>(e1) << 13);
+  const long long t10 = tmp0 + tmp3, t13 = tmp0 - tmp3, t11 = tmp1 + tmp2, t12 = tmp1 - tmp2;
+  if (CHECK)
+    *ok = *ok && jpeg_fits16(z2 + z3) && jpeg_fits16(e0) && jpeg_fits16(e1) && jpeg_fits32(t10) &&
+          jpeg_fits32(t11) && jpeg_fits32(t12) && jpeg_fits32(t13) && jpeg_fits32(z1);
+  // odd part: y7, y5, y3, y1
+  tmp0 = in[7 * s];
+  tmp1 = in[5 * s];
+  tmp2 = in[3 * s];
+  tmp3 = in[s];
+  z1 = tmp0 + tmp3;
+  z2 = tmp1 + tmp2;
+  z3 = tmp0 + tmp2;
+  long long z4 = tmp1 + tmp3;
+  const long long z5 = (z3 + z4) * F1175;
+  if (CHECK)
+    *ok = *ok && jpeg_fits16(z1) && jpeg_fits16(z2) && jpeg_fits16(z3) && jpeg_fits16(z4) && jpeg_fits16(z3 + z4);
+  tmp0 *= F0298;
+  tmp1 *= F2053;
+  tmp2 *= F3072;
+  tmp3 *= F1501;
+  z1 *= -F0899;
+  z2 *= -F2562;
+  z3 *= -F1961;
+  z4 *= -F0390;
+  z3 += z5;
+  z4 += z5;
+  tmp0 += z1 + z3;
+  tmp1 += z2 + z4;
+  tmp2 += z2 + z3;
+  tmp3 += z1 + z4;
+  const long long r = 1LL << (sh - 1);
+  out[0] = (t10 + tmp3 + r) >> sh;
+  out[7 * s] = (t10 - tmp3 + r) >> sh;
+  out[s] = (t11 + tmp2 + r) >> sh;
+  out[6 * s] = (t11 - tmp2 + r) >> sh;
+  out[2 * s] = (t12 + tmp1 + r) >> sh;
+  out[5 * s] = (t12 - tmp1 + r) >> sh;
+  out[3 * s] = (t13 + tmp0 + r) >> sh;
+  out[4 * s] = (t13 - tmp0 + r) >> sh;
+  if (CHECK)
+    *ok = *ok && jpeg_fits32(t10 + tmp3 + r) && jpeg_fits32(t10 - tmp3 + r) && jpeg_fits32(t11 + tmp2 + r) &&
+          jpeg_fits32(t11 - tmp2 + r) && jpeg_fits32(t12 + tmp1 + r) && jpeg_fits32(t12 - tmp1 + r) &&
+          jpeg_fits32(t13 + tmp0 + r) && jpeg_fits32(t13 - tmp0 + r);
+}
+
+// libjpeg's jpeg_idct_islow (jidctint.c) of one block: coefficients in natural order dequantised by q
+// (the product an int), the two-pass LL&M with its constants, PASS1_BITS = 2, DESCALE rounding, an int
+// workspace and 64-bit JLONG, its shortcuts for columns and rows whose AC terms are all zero, and
+// jpeg_idct_limit; 8 rows of 8 samples at out, pitch bytes apart.
+//
+// libjpeg-turbo's SIMD IDCTs compute the same integers as long as its 16-bit lanes hold every
+// dequantised value, pass-1 output and sum of them, and the output stays in [-512, 511] before the
+// range limit; past that they saturate or wrap differently.  CHECK: nothing is written, and the result
+// tells whether the block stays inside those ranges (on every quantity that could be 16 bits there).
+template <bool CHECK>
+GB_HD bool jpeg_islow(const int16_t* in, const int* q, uint8_t* out, int pitch) {
+  bool ok = true;
+  if (CHECK) {
+    // a DC-only block takes both shortcuts here and the 16-bit DC shortcut there, which wraps 4 x DC to
+    // 16 bits: the same output modulo 1024, so the same sample where that 16-bit output is in range
+    bool ac = false;
+    for (int k = 1; k < 64; ++k) ac = ac || in[k] != 0;
+    if (!ac) {
+      const long long dq = in[0] * q[0];
+      const long long x = (static_cast<long long>(static_cast<int16_t>(static_cast<uint16_t>(4 * dq))) + 16) >> 5;
+      return jpeg_fits16(dq) && x >= -512 && x <= 511;
+    }
+  }
+  long long col[64], ws[64];
+  int wsi[64];
+#if defined(__CUDA_ARCH__)
+#pragma unroll
+#endif
+  for (int x = 0; x < 8; ++x) {
+    for (int y = 0; y < 8; ++y) {
+      col[8 * y + x] = in[8 * y + x] * q[8 * y + x];
+      if (CHECK) ok = ok && jpeg_fits16(col[8 * y + x]);
+    }
+    if (in[8 + x] == 0 && in[16 + x] == 0 && in[24 + x] == 0 && in[32 + x] == 0 && in[40 + x] == 0 &&
+        in[48 + x] == 0 && in[56 + x] == 0) {
+      const int dc = static_cast<int>(static_cast<unsigned int>(in[x] * q[x]) << 2);
+      if (CHECK) ok = ok && jpeg_fits16(4LL * col[x]);
+      for (int y = 0; y < 8; ++y) wsi[8 * y + x] = dc;
+      continue;
+    }
+    jpeg_islow_pass<CHECK>(col + x, 8, 11, ws + x, &ok);  // CONST_BITS - PASS1_BITS
+    for (int y = 0; y < 8; ++y) {
+      wsi[8 * y + x] = static_cast<int>(ws[8 * y + x]);
+      if (CHECK) ok = ok && jpeg_fits16(ws[8 * y + x]);
+    }
+  }
+#if defined(__CUDA_ARCH__)
+#pragma unroll
+#endif
+  for (int y = 0; y < 8; ++y) {
+    const int* w = wsi + 8 * y;
+    long long row[8], o[8];
+    if (w[1] == 0 && w[2] == 0 && w[3] == 0 && w[4] == 0 && w[5] == 0 && w[6] == 0 && w[7] == 0) {
+      const long long v = (static_cast<long long>(w[0]) + 16) >> 5;  // PASS1_BITS + 3
+      for (int x = 0; x < 8; ++x) o[x] = v;
+    } else {
+      for (int x = 0; x < 8; ++x) row[x] = w[x];
+      jpeg_islow_pass<CHECK>(row, 1, 18, o, &ok);  // CONST_BITS + PASS1_BITS + 3
+    }
+    for (int x = 0; x < 8; ++x) {
+      if (CHECK) {
+        ok = ok && o[x] >= -512 && o[x] <= 511;
+      } else {
+        out[static_cast<size_t>(y) * pitch + x] = static_cast<uint8_t>(jpeg_idct_limit(o[x]));
+      }
+    }
+  }
+  return ok;
+}
+
 }  // namespace gb200

@@ -98,6 +98,126 @@ struct IngestU8 {
   }
 };
 
+// ---------------------------------------------------------------------------
+// JPEG decode as libjpeg-turbo decodes (jpeg_start_decompress with JDCT_ISLOW, fancy upsampling, RGB or
+// gray output), N files of different sizes and samplings per launch.  Host side: jpeg_decode_rgb
+// (pipeline.cu), which also lays out the buffers below.
+//
+// Every component of every file is one run of blocks of the call: coefficients [block][64] in natural
+// order, and samples in a plane of 8 bw x 8 bh bytes (pitch 8 bw) that starts at byte 64 x its first block.
+struct JpegDecFile {
+  int w, h;          // image size
+  int ncomp;         // 1 (gray) or 3
+  int ycc;           // 3 components: 1 YCbCr, converted to RGB; 0 RGB, copied
+  int hs, vs;        // the frame's maximum sampling (the first component's): 1x1, 2x1 or 2x2
+  int blk0[4];       // first block of each component in the call; blk0[ncomp] ends the file's run
+  int bw[3];         // blocks per row of each component
+  int cw, ch;        // the chroma components' real size: ceil(w / hs) x ceil(h / vs)
+  int row0;          // first output row of the file in the call's rows
+  uint8_t* out;      // [h][w][3]
+};
+
+// the j with t0[j] <= v < t0[j + 1], for a non-decreasing t0[0 .. m] with t0[0] <= v < t0[m]
+GB_HD int jpeg_find(const int* t0, int m, int v) {
+  int lo = 0, hi = m;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (t0[mid] <= v) {
+      lo = mid;
+    } else {
+      hi = mid;
+    }
+  }
+  return lo;
+}
+
+// One 8x8 block per invocation, over all blocks of the call: jpeg_islow (jpeg_math.h) with the
+// component's table (quant[3 f + c][64], natural order), into the component's plane.
+struct JpegIdctIslow {
+  const int16_t* coeffs;      // [blocks][64]
+  const int* quant;           // [3 n][64]
+  const JpegDecFile* files;   // [n]
+  const int* file_blk0;       // [n + 1]: first block of each file, then the total
+  int n;
+  uint8_t* samples;           // 64 bytes per block
+  GB_HD void operator()(int b) const {
+    const int f = jpeg_find(file_blk0, n, b);
+    const JpegDecFile& d = files[f];
+    const int c = b >= d.blk0[1] ? (b >= d.blk0[2] ? 2 : 1) : 0;
+    const int local = b - d.blk0[c], bw = d.bw[c];
+    const int bx = local % bw, by = local / bw;
+    uint8_t* out = samples + static_cast<size_t>(d.blk0[c]) * 64 + static_cast<size_t>(8 * by) * (8 * bw) + 8 * bx;
+    jpeg_islow<false>(coeffs + static_cast<size_t>(b) * 64, quant + (3 * f + c) * 64, out, 8 * bw);
+  }
+};
+
+// libjpeg's YCbCr -> RGB (jdcolor.c, build_ycc_rgb_table: SCALEBITS 16, ONE_HALF, FIX() of 1.40200,
+// 1.77200, 0.71414 and 0.34414), clamped by the simple range-limit table.
+GB_HD void jpeg_ycc_rgb(int y, int cb, int cr, uint8_t* o) {
+  const int x_cb = cb - 128, x_cr = cr - 128, half = 1 << 15;
+  const int r = y + ((91881 * x_cr + half) >> 16);
+  const int g = y + ((-22554 * x_cb + half + -46802 * x_cr) >> 16);
+  const int b = y + ((116130 * x_cb + half) >> 16);
+  o[0] = static_cast<uint8_t>(r < 0 ? 0 : (r > 255 ? 255 : r));
+  o[1] = static_cast<uint8_t>(g < 0 ? 0 : (g > 255 ? 255 : g));
+  o[2] = static_cast<uint8_t>(b < 0 ? 0 : (b > 255 ? 255 : b));
+}
+
+// Output pixels of the call's rows: row yy of the call is row yy - row0 of file jpeg_find(file_row0, n,
+// yy).  Invocation (lane, yy) writes pixels x = lane, lane + lanes, ... of that row.  Chroma is upsampled
+// as jdsample.c does with do_fancy_upsampling: 2x1 by h2v1_fancy_upsample (3:1 weights, biases 1 and 2),
+// 2x2 by h2v2_fancy_upsample (the 3:1 vertical sum, then 3:1 across with biases 8 and 7); the neighbour
+// columns and rows beyond the chroma's real size cw x ch repeat its last one, and the row above the first
+// is the first (jdmainct.c's context rows).  A chroma width of 1 or 2 is replicated instead
+// (h2v1_upsample, h2v2_upsample), as libjpeg-turbo does at those widths.  Then jpeg_ycc_rgb, a copy for
+// RGB files, or gray replicated.
+struct JpegUpsampleYccRgb {
+  const JpegDecFile* files;
+  const int* file_row0;  // [n + 1]
+  int n;
+  const uint8_t* samples;
+  int lanes;
+  GB_HD int chroma(const JpegDecFile& d, const uint8_t* p, int x, int y) const {
+    const int pitch = 8 * d.bw[1];
+    const int j = x >> (d.hs - 1);
+    if (d.hs == 1) return p[static_cast<size_t>(y) * pitch + x];
+    if (d.cw <= 2) return p[static_cast<size_t>(y >> (d.vs - 1)) * pitch + j];
+    const int jn = (x & 1) ? hd_min(j + 1, d.cw - 1) : hd_max(j - 1, 0);
+    if (d.vs == 1) {
+      const uint8_t* r = p + static_cast<size_t>(y) * pitch;
+      return (3 * r[j] + r[jn] + 1 + (x & 1)) >> 2;
+    }
+    const int i = y >> 1, in = (y & 1) ? hd_min(i + 1, d.ch - 1) : hd_max(i - 1, 0);
+    const uint8_t* r0 = p + static_cast<size_t>(i) * pitch;
+    const uint8_t* r1 = p + static_cast<size_t>(in) * pitch;
+    const int s = 3 * r0[j] + r1[j], sn = 3 * r0[jn] + r1[jn];
+    return (3 * s + sn + ((x & 1) ? 7 : 8)) >> 4;
+  }
+  GB_HD void operator()(int lane, int yy) const {
+    const int f = jpeg_find(file_row0, n, yy);
+    const JpegDecFile& d = files[f];
+    const int y = yy - d.row0;
+    const uint8_t* yp = samples + static_cast<size_t>(d.blk0[0]) * 64 + static_cast<size_t>(y) * (8 * d.bw[0]);
+    uint8_t* o = d.out + static_cast<size_t>(y) * d.w * 3;
+    for (int x = lane; x < d.w; x += lanes) {
+      const int v0 = yp[x];
+      if (d.ncomp == 1) {
+        o[3 * x] = o[3 * x + 1] = o[3 * x + 2] = static_cast<uint8_t>(v0);
+        continue;
+      }
+      const int v1 = chroma(d, samples + static_cast<size_t>(d.blk0[1]) * 64, x, y);
+      const int v2 = chroma(d, samples + static_cast<size_t>(d.blk0[2]) * 64, x, y);
+      if (d.ycc) {
+        jpeg_ycc_rgb(v0, v1, v2, o + 3 * x);
+      } else {
+        o[3 * x] = static_cast<uint8_t>(v0);
+        o[3 * x + 1] = static_cast<uint8_t>(v1);
+        o[3 * x + 2] = static_cast<uint8_t>(v2);
+      }
+    }
+  }
+};
+
 // Original image u8 sRGB -> linear float planes (g/butteraugli_comparator.cc:33).
 struct LinearizeRgb {
   const uint8_t* rgb;

@@ -15,6 +15,7 @@
 
 #include "block_math.h"
 #include "jpeg_dev.h"
+#include "jpeg_in.h"
 #include "walk_dev.h"
 #if !defined(GB200_HOSTSIM)
 #include <deque>
@@ -3000,5 +3001,124 @@ long ImageContext::launches() const { return total_launches(); }
 void ImageContext::set_profiling(bool on) { profiling_enable(on); }
 std::vector<KernelStat> ImageContext::kernel_stats() const { return profiling_snapshot(); }
 void ImageContext::reset_stats() { profiling_reset(); }
+
+// ---------------------------------------------------------------------------
+// JPEG decode (JpegIdctIslow, JpegUpsampleYccRgb in kernels.h)
+#if !defined(GB200_HOSTSIM)
+namespace {
+// JpegUpsampleYccRgb over the call's rows: a warp per row, 8 rows per block (as k_mix_rows)
+template <class F>
+__global__ void __launch_bounds__(256) k_jpeg_rows(F f, int rows) {
+  const int row = blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (row < rows) f(threadIdx.x & 31, row);
+}
+}  // namespace
+#endif
+
+void jpeg_decode_rgb(const JpegInput* const* files, int n, int device, uint8_t* const* out, bool out_on_device,
+                     Stream stream) {
+  std::vector<JpegDecFile> tab(n);
+  std::vector<int> blk0(n + 1), row0(n + 1), quant(static_cast<size_t>(n) * 3 * 64, 1);
+  long long blocks = 0, rows = 0, out_bytes = 0, pixels = 0;
+  for (int i = 0; i < n; ++i) {
+    const JpegInput& j = *files[i];
+    JpegDecFile& d = tab[i];
+    d.w = j.width;
+    d.h = j.height;
+    d.ncomp = static_cast<int>(j.components.size());
+    d.ycc = d.ncomp == 3 && libjpeg_ycbcr(j);
+    d.hs = j.max_h;
+    d.vs = j.max_v;
+    d.cw = (d.w + d.hs - 1) / d.hs;
+    d.ch = (d.h + d.vs - 1) / d.vs;
+    blk0[i] = static_cast<int>(blocks);
+    for (int c = 0; c < 4; ++c) {
+      d.blk0[c] = static_cast<int>(blocks);
+      if (c >= d.ncomp) continue;
+      const JpegComponent& comp = j.components[c];
+      d.bw[c] = comp.width_in_blocks;
+      memcpy(&quant[(3 * i + c) * 64], j.quant[comp.quant_idx].values, 64 * sizeof(int));
+      blocks += static_cast<long long>(comp.width_in_blocks) * comp.height_in_blocks;
+    }
+    d.row0 = static_cast<int>(rows);
+    rows += d.h;
+    d.out = nullptr;
+    pixels += static_cast<long long>(d.w) * d.h;
+    if (blocks > (1LL << 30) || rows > (1LL << 30))
+      throw std::runtime_error("jpeg_decode_rgb: more than 2^30 blocks or rows in one call");
+  }
+  blk0[n] = static_cast<int>(blocks);
+  row0[n] = static_cast<int>(rows);
+  for (int i = 0; i < n; ++i) row0[i] = tab[i].row0;
+  out_bytes = 3 * pixels;
+  std::vector<int16_t> coeffs(static_cast<size_t>(blocks) * 64);
+  for (int i = 0; i < n; ++i)
+    for (int c = 0; c < tab[i].ncomp; ++c) {
+      const std::vector<int16_t>& v = files[i]->components[c].coeffs;
+      memcpy(&coeffs[static_cast<size_t>(tab[i].blk0[c]) * 64], v.data(), v.size() * sizeof(int16_t));
+    }
+
+  // everything acquired is handed back on every path; buffers only once the stream is idle
+  struct Scope {
+    Stream s = 0;
+    bool have = false;
+    std::vector<void*> bufs;
+    void* alloc(size_t bytes) {
+      bufs.push_back(dev_alloc(bytes));
+      return bufs.back();
+    }
+    ~Scope() {
+      if (have) {
+        try {
+          stream_sync(s);
+        } catch (...) {
+        }
+        destroy_stream(s);
+      }
+      for (void* p : bufs) dev_free(p);
+    }
+  } sc;
+  select_device(device);
+  sc.s = make_stream();
+  sc.have = true;
+  const Stream s = sc.s;
+  uint8_t* staged = nullptr;
+  if (out_on_device) {
+    for (int i = 0; i < n; ++i) tab[i].out = out[i];
+  } else {
+    staged = static_cast<uint8_t*>(sc.alloc(static_cast<size_t>(out_bytes)));
+    size_t o = 0;
+    for (int i = 0; i < n; ++i) {
+      tab[i].out = staged + o;
+      o += static_cast<size_t>(3) * tab[i].w * tab[i].h;
+    }
+  }
+  JpegDecFile* d_tab = static_cast<JpegDecFile*>(sc.alloc(sizeof(JpegDecFile) * n));
+  int* d_blk0 = static_cast<int*>(sc.alloc(sizeof(int) * (n + 1)));
+  int* d_row0 = static_cast<int*>(sc.alloc(sizeof(int) * (n + 1)));
+  int* d_quant = static_cast<int*>(sc.alloc(sizeof(int) * quant.size()));
+  int16_t* d_coeffs = static_cast<int16_t*>(sc.alloc(sizeof(int16_t) * coeffs.size()));
+  uint8_t* d_samples = static_cast<uint8_t*>(sc.alloc(static_cast<size_t>(blocks) * 64));
+  h2d(d_tab, tab.data(), sizeof(JpegDecFile) * n, s);
+  h2d(d_blk0, blk0.data(), sizeof(int) * (n + 1), s);
+  h2d(d_row0, row0.data(), sizeof(int) * (n + 1), s);
+  h2d(d_quant, quant.data(), sizeof(int) * quant.size(), s);
+  h2d(d_coeffs, coeffs.data(), sizeof(int16_t) * coeffs.size(), s);
+  if (out_on_device) stream_wait(s, stream);
+  launch_1d(s, JpegIdctIslow{d_coeffs, d_quant, d_tab, d_blk0, n, d_samples}, static_cast<int>(blocks),
+            "jpeg_idct_islow");
+  JpegUpsampleYccRgb up{d_tab, d_row0, n, d_samples, 1};
+#if defined(GB200_HOSTSIM)
+  launch_2d(s, up, 1, static_cast<int>(rows));
+#else
+  up.lanes = 32;
+  note_launch("jpeg_upsample_ycc_rgb", s, static_cast<double>(pixels));
+  k_jpeg_rows<<<cdiv(static_cast<int>(rows), 8), 256, 0, s>>>(up, static_cast<int>(rows));
+  note_launch_end("jpeg_upsample_ycc_rgb", s);
+#endif
+  if (!out_on_device)
+    for (int i = 0; i < n; ++i) d2h(out[i], tab[i].out, static_cast<size_t>(3) * tab[i].w * tab[i].h, s);
+  stream_sync(s);
+}
 
 }  // namespace gb200

@@ -15,6 +15,15 @@ namespace gb200 {
 
 struct OrderItem;
 struct OrderSelectState;
+struct JpegInput;
+
+// libjpeg-turbo's pixels of n parsed files that libjpeg_decodable (jpeg_in.h) accepted, decoded on `device`
+// with one launch of JpegIdctIslow and one of JpegUpsampleYccRgb (kernels.h) for all of them: out[i]
+// receives file i as [h][w][3] bytes.  The coefficients of all files go up in one staging buffer, beside
+// one per-file table.  Host outputs come back per file; with out_on_device, out[i] is memory of `device`,
+// written after the work queued on `stream` so far.  Either way the outputs are written when this returns.
+void jpeg_decode_rgb(const JpegInput* const* files, int n, int device, uint8_t* const* out, bool out_on_device,
+                     Stream stream);
 
 // An 8-bit image of 1 (gray), 2 (gray + alpha), 3 (RGB) or 4 (RGBA) channels in any layout with
 // non-negative strides: sample (y, x, c) is at byte y * stride[0] + x * stride[1] + c * stride[2] of data.

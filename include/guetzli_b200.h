@@ -297,6 +297,22 @@ int gb200_butteraugli_adaptive_quantization(const float* rgb, int w, int h, int 
 /* ReadJpeg(JPEG_READ_HEADER) as the CLI uses it (guetzli/guetzli.cc:306): frame size only. */
 int gb200_jpeg_dimensions(const uint8_t* jpeg_in, size_t jpeg_len, int* width, int* height);
 
+/* The pixels libjpeg-turbo gives for n JPEG files (jpeg_start_decompress with the defaults the butteraugli
+ * tool's ReadJPEG keeps: JDCT_ISLOW, fancy upsampling, RGB output, gray replicated into R, G and B), decoded
+ * on `device` in one pass for files of any sizes: out[i] receives file i as [h][w][3] bytes in host memory,
+ * w x h as gb200_jpeg_dimensions gives them.  Accepted: baseline, extended and progressive Huffman files
+ * that are gray or have 3 components sampled 4:4:4, 4:2:2 or 4:2:0.  Refused, with the file's index and the
+ * reason in gb200_last_error() and nothing run: what ReadJpeg rejects, 4 components (CMYK, YCCK), other
+ * samplings, progressive files that libjpeg would block-smooth (some low-frequency coefficient not
+ * refined to its last bit), and files with coefficients so large that libjpeg-turbo's SIMD and C IDCTs
+ * give different samples.  Returns 1 on success. */
+int gb200_jpeg_decode_rgb(const uint8_t* const* jpeg, const size_t* len, int n, int device, uint8_t* const* out);
+/* The same with out_dev[i] in device memory of `device`, written after the work queued on `stream` so far
+ * (a cudaStream_t, NULL = the legacy default stream) and written when the call returns.  A host, managed
+ * or other device's pointer is refused, nothing runs. */
+int gb200_jpeg_decode_rgb_device(const uint8_t* const* jpeg, const size_t* len, int n, int device,
+                                 uint8_t* const* out_dev, void* stream);
+
 /* test hook: ReadJpeg(JPEG_READ_ALL) alone.  dims = {w, h, ncomp, wb0, hb0, wb1, hb1, ...} (11 ints);
  * out receives the quantised coefficients of all components, concatenated. */
 int gb200_debug_read_jpeg(const uint8_t* jpeg_in, size_t jpeg_len, int* dims, int16_t* out, size_t out_cap);
