@@ -65,16 +65,6 @@ Butteraugli::Butteraugli(int w, int h, int capacity, int device, Slots slots) : 
 // A constructor that throws never reaches the destructor: everything acquired so far (device
 // buffers of owned_, the stream) is handed back here, so that an out-of-memory condition does not
 // become permanent for the process.
-namespace {
-// GB200_COMPARE=staged keeps the round-1 kernel sequence (one kernel per stage) for A/B
-// measurements and for the cross-check in tests; default is the fused chain.
-bool fused_enabled() {
-  const char* e = getenv("GB200_COMPARE");  // read per metric: tests switch it between images
-  return !(e != nullptr && e[0] == 's');
-}
-
-}  // namespace
-
 void Butteraugli::init(int w, int h, Comm* comm) {
   r_.g = make_geom(w, h);
   r_.comm = comm;
@@ -88,21 +78,18 @@ void Butteraugli::init(int w, int h, Comm* comm) {
     select_device(device_);
     r_.s = make_stream();
     have_stream_ = true;
-#if !defined(GB200_HOSTSIM)
-    use_fused_ = fused_enabled();
+#if defined(GB200_HOSTSIM)
+    // the CPU port has no batched launches: compare_many scores the candidates one by one on a
+    // single-image layout, compare_batch the pairs through metrics of their own
+    if (one_original_) kslot_ = 0;
+    if (kslot_ != 0) return;
 #endif
-    // the staged chain and the CPU port have no batched launches: compare_many scores the candidates
-    // one by one on a single-image layout, compare_batch the pairs through metrics of their own
-    if (one_original_ && !use_fused_) kslot_ = 0;
-    if (kslot_ != 0 && !use_fused_) return;
     t_ = build_tables(w, h, s_, &owned_, &ht_);
     malta_call_params(malta_);
     l2_asym_weights(&asym_w0_, &asym_w1_);
 #if !defined(GB200_HOSTSIM)
-    if (use_fused_) {
-      fused_ = new Fused();
-      fused_->capacity = capacity_;
-    }
+    fused_ = new Fused();
+    fused_->capacity = capacity_;
 #endif
     alloc_planes();
     stream_sync(s_);
@@ -121,22 +108,29 @@ float* Butteraugli::planes(size_t n) {
 
 // The plane groups of all three shapes.  They lie in one arena of `slots` slots, each group at the
 // same offset in every slot, so that slot n's copy of a group is the group plus n slots.  A batch
-// slot holds only what the analysis of an original and the fused chain touch (DESIGN.md §4).  With
-// one original for all slots, the original's groups lie once after the slots, with the planes of
-// its mask activity (mask()), and a slot holds the rest.
+// slot holds only what the analysis of an original and the fused chain touch (DESIGN.md §4); the
+// slot of one image adds the mask activity and, in the CPU port, the planes its chain blurs into.
+// With one original for all slots, the original's groups lie once after the slots, with the planes
+// of its mask activity (mask()), and a slot holds the rest.
 void Butteraugli::alloc_planes() {
   struct Group {
     float** p;
     int single, batch;  // planes in the slot of one image / of a batch
     bool orig;          // the original's: outside the slots when they share one original
   };
+#if defined(GB200_HOSTSIM)
+  constexpr int kPort = 1;
+#else
+  constexpr int kPort = 0;
+#endif
   const Group groups[] = {
       {&lin_, 3, 3, false},    {&xyb_, 3, 3, false},  {&lf_, 3, 3, false},  {&mf_in_, 3, 3, false},
       {&hf_raw_, 2, 2, false}, {&ps0_, kPsychoPlanes, kPsychoPlanes, true}, {&ps1_, kPsychoPlanes, kPsychoPlanes, false},
-      {&sup0_, 2, 2, true},    {&diffs6_, 6, 6, false}, {&noise_, 2, 1, false}, {&mpre_, 2, 2, false},
-      {&tmp_, 3, 3, false},    {&blr_, 3, 1, false},  {&ac_, 2, 2, false},  {&dm_, 2, 2, false},
-      // the staged chain's own planes and the mask activity
-      {&mf_blr_, 3, 0, false}, {&hf_blr_, 2, 0, false}, {&diffs_, 1, 0, false}, {&sact_, 3, 0, true}};
+      {&sup0_, 2, 2, true},    {&diffs6_, 6, 6, false}, {&noise_, 1 + kPort, 1, false}, {&mpre_, 2, 2, false},
+      {&tmp_, 3, 3, false},    {&blr_, 1 + 2 * kPort, 1, false}, {&ac_, 2, 2, false},  {&dm_, 2, 2, false},
+      // the CPU port's blurred planes and the mask activity
+      {&mf_blr_, 3 * kPort, 0, false}, {&hf_blr_, 2 * kPort, 0, false}, {&diffs_, kPort, 0, false},
+      {&sact_, 3, 0, true}};
   const bool shared = one_original_ && kslot_ != 0;
   const int slots = kslot_ ? capacity_ : 1;
   int slot = 0, once = 0;
@@ -217,13 +211,10 @@ void Butteraugli::compare_batch(const float* rgb0, const float* rgb1, int n, flo
   if (n < 1 || n > capacity_) throw std::runtime_error("butteraugli batch: n must be in 1..capacity");
   bind();
 #if !defined(GB200_HOSTSIM)
-  if (use_fused_) {
-    if (device) stream_wait(s_, caller);
-    fused_compare_batch(rgb0, rgb1, n, diffmap, maxima);
-    return;
-  }
-#endif
-  // the staged chain and the CPU port: compare_batch_sizes with every pair at this batch's size
+  if (device) stream_wait(s_, caller);
+  fused_compare_batch(rgb0, rgb1, n, diffmap, maxima);
+#else
+  // the CPU port: compare_batch_sizes with every pair at this batch's size
   const size_t img = static_cast<size_t>(3) * g_.w * g_.h, px = static_cast<size_t>(g_.w) * g_.h;
   const std::vector<int> w(n, g_.w), h(n, g_.h);
   std::vector<const float*> p0(n), p1(n);
@@ -234,6 +225,7 @@ void Butteraugli::compare_batch(const float* rgb0, const float* rgb1, int n, flo
     dm[i] = diffmap != nullptr ? diffmap + i * px : nullptr;
   }
   compare_batch_sizes(w.data(), h.data(), p0.data(), p1.data(), n, dm.data(), maxima, device, caller);
+#endif
 }
 
 void Butteraugli::check_sizes(const int* w, const int* h, int n) const {
@@ -247,46 +239,31 @@ void Butteraugli::compare_batch_sizes(const int* w, const int* h, const float* c
   check_sizes(w, h, n);
   bind();
 #if !defined(GB200_HOSTSIM)
-  if (use_fused_) {
-    if (device) stream_wait(s_, caller);
-    const std::vector<const void*> in0(rgb0, rgb0 + n), in1(rgb1, rgb1 + n);
-    fused_compare_sizes(w, h, nullptr, in0.data(), in1.data(), n, diffmap, maxima, device);
-    return;
+  if (device) stream_wait(s_, caller);
+  const std::vector<const void*> in0(rgb0, rgb0 + n), in1(rgb1, rgb1 + n);
+  fused_compare_sizes(w, h, nullptr, in0.data(), in1.data(), n, diffmap, maxima, device);
+#else
+  // the CPU port (host memory only): one single-image metric per pair, of the pair's size
+  for (int i = 0; i < n; ++i) {
+    Butteraugli pair(w[i], h[i], device_, nullptr);
+    pair.analyse_original(rgb0[i]);
+    maxima[i] = pair.compare_linear(rgb1[i]);
+    if (diffmap != nullptr && diffmap[i] != nullptr) pair.download_distmap(diffmap[i]);
   }
 #endif
-  // the staged chain and the CPU port: one single-image metric per pair, of the pair's size
-  for (int i = 0; i < n; ++i) {
-    const size_t img = static_cast<size_t>(3) * w[i] * h[i];
-    const float* p0 = rgb0[i];
-    std::vector<float> host0;
-    if (device) {  // the pair's original goes through host memory, after the caller's work
-      host0.resize(img);
-      d2h(host0.data(), p0, img * sizeof(float), caller);
-      p0 = host0.data();
-    }
-    Butteraugli pair(w[i], h[i], device_, nullptr);
-    pair.analyse_original(p0);
-    float* dm = diffmap != nullptr ? diffmap[i] : nullptr;
-    if (device) {
-      maxima[i] = pair.compare_linear_device(rgb1[i], dm, caller);
-    } else {
-      maxima[i] = pair.compare_linear(rgb1[i]);
-      if (dm != nullptr) pair.download_distmap(dm);
-    }
-  }
 }
 
 void Butteraugli::compare_many(const float* rgb1, int n, float* diffmap, float* maxima, bool device, Stream caller) {
   if (n < 1 || n > capacity_) throw std::runtime_error("butteraugli comparator: n must be in 1..capacity");
   bind();
 #if !defined(GB200_HOSTSIM)
-  if (use_fused_ && kslot_ != 0) {
+  if (kslot_ != 0) {
     if (device) stream_wait(s_, caller);
     fused_compare_batch(nullptr, rgb1, n, diffmap, maxima);
     return;
   }
 #endif
-  // capacity 1, the staged chain and the CPU port: one candidate at a time in slot 0
+  // capacity 1 and the CPU port: one candidate at a time in slot 0
   const size_t img = static_cast<size_t>(3) * g_.w * g_.h, px = static_cast<size_t>(g_.w) * g_.h;
   for (int i = 0; i < n; ++i) {
     float* dm = diffmap != nullptr ? diffmap + i * px : nullptr;
@@ -319,8 +296,8 @@ void check_channels(int channels) {
 
 void Butteraugli::srgb_alloc(int per_slot) {
   if (srgb_lin_ != nullptr) return;
-  // the pair batch builds no tables of its own where its pairs go through metrics of their own; the
-  // conversion needs only the sRGB table
+  // the CPU port's pair batch builds no tables of its own (its pairs go through metrics of their own);
+  // the conversion needs only the sRGB table
   if (t_.srgb_lin == nullptr) t_.srgb_lin = upload_srgb_lin(s_, &owned_, nullptr);
   const size_t px = static_cast<size_t>(g_.w) * g_.h, imgs = static_cast<size_t>(per_slot) * capacity_;
   srgb_u8_ = static_cast<uint8_t*>(dev_alloc(4 * px * imgs));
@@ -429,19 +406,17 @@ void Butteraugli::compare_batch_sizes_srgb(const int* w, const int* h, const int
   for (int i = 0; i < n; ++i) check_channels(channels[i]);
   bind();
 #if !defined(GB200_HOSTSIM)
-  if (use_fused_) {
-    if (device) stream_wait(s_, caller);
-    const std::vector<const void*> in0(img0, img0 + n), in1(img1, img1 + n);
-    fused_compare_sizes(w, h, channels, in0.data(), in1.data(), n, diffmap, maxima, device);
-    return;
-  }
-#endif
-  // the staged chain and the CPU port: one pair batch per pair, of the pair's size
+  if (device) stream_wait(s_, caller);
+  const std::vector<const void*> in0(img0, img0 + n), in1(img1, img1 + n);
+  fused_compare_sizes(w, h, channels, in0.data(), in1.data(), n, diffmap, maxima, device);
+#else
+  // the CPU port: one pair batch per pair, of the pair's size
   for (int i = 0; i < n; ++i) {
     Butteraugli pair(w[i], h[i], 1, device_, Slots::kPairs);
     pair.compare_batch_srgb(img0[i], img1[i], 1, channels[i], diffmap != nullptr ? diffmap[i] : nullptr, &maxima[i],
                             device, caller);
   }
+#endif
 }
 
 // ---- comparator sets (butteraugli.h) ----
@@ -454,8 +429,14 @@ ComparatorSet::ComparatorSet(const int* w, const int* h, const int* channels, co
   }
   ba_.reset(new Butteraugli(*std::max_element(w_.begin(), w_.end()), *std::max_element(h_.begin(), h_.end()),
                             capacity, device, Butteraugli::Slots::kPairs));
-  const bool fused = ba_->fused();
-  // the store: each original's analyses (fused chain) or its input, 16-byte aligned
+#if defined(GB200_HOSTSIM)
+  for (int i = 0; i < count; ++i) {
+    const size_t in = static_cast<size_t>(w[i]) * h[i] * (srgb() ? channels[i] : 3 * sizeof(float));
+    const unsigned char* p = static_cast<const unsigned char*>(img0[i]);
+    host_.emplace_back(p, p + in);
+  }
+#else
+  // the store: each original's analyses, 16-byte aligned
   size_t bytes = 0;
   const auto take = [&](size_t n) {
     const size_t at = bytes;
@@ -465,54 +446,40 @@ ComparatorSet::ComparatorSet(const int* w, const int* h, const int* channels, co
   for (size_t b = 0; b < 2; ++b) at_[b].assign(count, kNone);
   for (int i = 0; i < count; ++i) {
     const size_t px = static_cast<size_t>(w[i]) * h[i];
-    if (fused) {
-      at_[0][i] = take(sizeof(float) * kStoredPlanes * px);
-      if (srgb() && channels[i] == 4) at_[1][i] = take(sizeof(float) * kStoredPlanes * px);
-    } else {
-      const size_t in = px * (srgb() ? channels[i] : 3 * sizeof(float));
-      at_[0][i] = take(in);
-      const unsigned char* p = static_cast<const unsigned char*>(img0[i]);
-      host_.emplace_back(p, p + in);
-    }
+    at_[0][i] = take(sizeof(float) * kStoredPlanes * px);
+    if (srgb() && channels[i] == 4) at_[1][i] = take(sizeof(float) * kStoredPlanes * px);
   }
   ba_->bind();
   store_ = dev_alloc(bytes);
   try {
     unsigned char* base = static_cast<unsigned char*>(store_);
-#if !defined(GB200_HOSTSIM)
-    if (fused) {
-      // mixed passes of up to `capacity` originals: every original over black, then the RGBA ones over white
-      for (int bg = 0; bg < 2; ++bg) {
-        std::vector<int> all;
-        for (int i = 0; i < count; ++i)
-          if (at_[bg][i] != kNone) all.push_back(i);
-        for (size_t k = 0; k < all.size(); k += capacity) {
-          const size_t m = std::min(all.size() - k, static_cast<size_t>(capacity));
-          std::vector<int> cw(m), ch(m), cc(m);
-          std::vector<const void*> in(m);
-          std::vector<float*> to(m);
-          for (size_t j = 0; j < m; ++j) {
-            const int i = all[k + j];
-            cw[j] = w_[i];
-            ch[j] = h_[i];
-            cc[j] = srgb() ? channels_[i] : 3;
-            in[j] = img0[i];
-            to[j] = reinterpret_cast<float*>(base + at_[bg][i]);
-          }
-          ba_->analyse_originals(cw.data(), ch.data(), srgb() ? cc.data() : nullptr, in.data(), static_cast<int>(m),
-                                 bg == 0 ? 0 : 255, to.data());
+    // mixed passes of up to `capacity` originals: every original over black, then the RGBA ones over white
+    for (int bg = 0; bg < 2; ++bg) {
+      std::vector<int> all;
+      for (int i = 0; i < count; ++i)
+        if (at_[bg][i] != kNone) all.push_back(i);
+      for (size_t k = 0; k < all.size(); k += capacity) {
+        const size_t m = std::min(all.size() - k, static_cast<size_t>(capacity));
+        std::vector<int> cw(m), ch(m), cc(m);
+        std::vector<const void*> in(m);
+        std::vector<float*> to(m);
+        for (size_t j = 0; j < m; ++j) {
+          const int i = all[k + j];
+          cw[j] = w_[i];
+          ch[j] = h_[i];
+          cc[j] = srgb() ? channels_[i] : 3;
+          in[j] = img0[i];
+          to[j] = reinterpret_cast<float*>(base + at_[bg][i]);
         }
+        ba_->analyse_originals(cw.data(), ch.data(), srgb() ? cc.data() : nullptr, in.data(), static_cast<int>(m),
+                               bg == 0 ? 0 : 255, to.data());
       }
-      return;
     }
-#endif
-    // a copy of the inputs in device memory, for candidates in device memory
-    for (int i = 0; i < count; ++i) h2d(base + at_[0][i], host_[i].data(), host_[i].size(), ba_->region().s);
-    stream_sync(ba_->region().s);
   } catch (...) {
     dev_free(store_);
     throw;
   }
+#endif
 }
 
 ComparatorSet::~ComparatorSet() {
@@ -528,7 +495,6 @@ ComparatorSet::~ComparatorSet() {
 void ComparatorSet::compare(const int* original, const void* const* img1, int n, float* const* diffmap, float* maxima,
                             bool device, Stream caller) {
   std::vector<int> w(n), h(n), ch(n, 3);
-  unsigned char* base = static_cast<unsigned char*>(store_);
   for (int i = 0; i < n; ++i) {
     const int o = original[i];
     w[i] = w_[o];
@@ -537,23 +503,20 @@ void ComparatorSet::compare(const int* original, const void* const* img1, int n,
   }
   const int* channels = srgb() ? ch.data() : nullptr;
 #if !defined(GB200_HOSTSIM)
-  if (ba_->fused()) {
-    std::vector<float*> stored[2];
-    for (int b = 0; b < 2; ++b)
-      for (int i = 0; i < n; ++i) {
-        const size_t at = at_[b][original[i]];
-        stored[b].push_back(at == kNone ? nullptr : reinterpret_cast<float*>(base + at));
-      }
-    float* const* const st[2] = {stored[0].data(), stored[1].data()};
-    ba_->compare_originals(w.data(), h.data(), channels, st, img1, n, diffmap, maxima, device, caller);
-    return;
-  }
-#endif
-  // the staged chain and the CPU port: the pairs (original, candidate), from the inputs' copy on the
-  // candidates' side
+  unsigned char* base = static_cast<unsigned char*>(store_);
+  std::vector<float*> stored[2];
+  for (int b = 0; b < 2; ++b)
+    for (int i = 0; i < n; ++i) {
+      const size_t at = at_[b][original[i]];
+      stored[b].push_back(at == kNone ? nullptr : reinterpret_cast<float*>(base + at));
+    }
+  float* const* const st[2] = {stored[0].data(), stored[1].data()};
+  ba_->compare_originals(w.data(), h.data(), channels, st, img1, n, diffmap, maxima, device, caller);
+#else
+  // the CPU port: the pairs (original, candidate)
   std::vector<const unsigned char*> in0(n), in1(n);
   for (int i = 0; i < n; ++i) {
-    in0[i] = device ? base + at_[0][original[i]] : host_[original[i]].data();
+    in0[i] = host_[original[i]].data();
     in1[i] = static_cast<const unsigned char*>(img1[i]);
   }
   if (srgb()) {
@@ -567,6 +530,7 @@ void ComparatorSet::compare(const int* original, const void* const* img1, int n,
     }
     ba_->compare_batch_sizes(w.data(), h.data(), f0.data(), f1.data(), n, diffmap, maxima, device, caller);
   }
+#endif
 }
 
 void Butteraugli::adaptive_quantization(const float* linear_rgb, float* quant) {
@@ -577,8 +541,8 @@ void Butteraugli::adaptive_quantization(const float* linear_rgb, float* quant) {
 }
 
 void Butteraugli::compare_begin() {
-  compare_pending_ = use_fused_ && !r_.strips();
 #if !defined(GB200_HOSTSIM)
+  compare_pending_ = !r_.strips();
   if (compare_pending_) return fused_compare_submit();
 #endif
   compare_stash_ = compare();

@@ -1,5 +1,5 @@
-// The butteraugli metric on the device: the Compare chain (the TMA-staged fused chain, and the staged
-// chain it is checked against), the float planes it works on, and the analysis of the original.
+// The butteraugli metric on the device: the Compare chain (the TMA-staged fused chain; the CPU port
+// runs one launch per stage instead), the float planes it works on, and the analysis of the original.
 // One Butteraugli scores one image -- the encoder's candidate (ImageContext holds one) or a
 // stand-alone comparator's -- or a batch of same-size pairs, or a batch of same-size candidates
 // against one original (ComparatorSet: against resident originals of sizes of their own).  It owns the
@@ -164,7 +164,7 @@ class Butteraugli {
   // maxima on the device and returns the distance.
   float compare();
   // the same in two halves: compare_begin() queues the kernels, compare_end() waits for the
-  // distance (where the launches need a host round trip -- strip mode, the staged chain --
+  // distance (where the launches need a host round trip -- strip mode, the CPU port --
   // compare_begin() does it all)
   void compare_begin();
   float compare_end();
@@ -186,13 +186,13 @@ class Butteraugli {
                      Stream caller);
   // ButteraugliComparator::Diffmap against the original for each of n <= capacity candidates,
   // rgb1 packed [n][3][h][w]; outputs, device and caller as in compare_batch.  Slots kCandidates;
-  // with capacity 1, the staged chain or the CPU port the candidates go one by one through slot 0.
+  // with capacity 1 or in the CPU port the candidates go one by one through slot 0.
   void compare_many(const float* rgb1, int n, float* diffmap, float* maxima, bool device, Stream caller);
   // compare_batch on n <= capacity pairs of different sizes: pair i is w[i] x h[i], each at least 8x8 and
   // at most this batch's size, rgb0[i] / rgb1[i] packed [3][h[i]][w[i]], diffmap[i] [h[i]][w[i]] (diffmap
   // itself may be null).  Outputs, device and caller as in compare_batch.  The fused chain scores all pairs
   // in one pass of launches over (image, tile) work items, with tensor maps of each distinct size; the
-  // staged chain and the CPU port score each pair through a metric of its own size.
+  // CPU port scores each pair through a metric of its own size.
   void compare_batch_sizes(const int* w, const int* h, const float* const* rgb0, const float* const* rgb1, int n,
                            float* const* diffmap, float* maxima, bool device, Stream caller);
 
@@ -217,8 +217,8 @@ class Butteraugli {
   // compare_batch_sizes on 8-bit pairs: img0[i] / img1[i] interleaved [h[i]][w[i]][channels[i]], channels 3
   // or 4 per pair; diffmap itself and its entries may be null.  The fused chain converts while it packs
   // the images into the arena (k_mix_srgb): one run over all pairs laid over black, then one over the RGBA
-  // pairs alone laid over white, with passes of their own sizes.  The staged chain and the CPU port score
-  // each pair through compare_batch_srgb of a pair batch of its own size.
+  // pairs alone laid over white, with passes of their own sizes.  The CPU port scores each pair through
+  // compare_batch_srgb of a pair batch of its own size.
   void compare_batch_sizes_srgb(const int* w, const int* h, const int* channels, const uint8_t* const* img0,
                                 const uint8_t* const* img1, int n, float* const* diffmap, float* maxima, bool device,
                                 Stream caller);
@@ -233,7 +233,6 @@ class Butteraugli {
   void compare_originals(const int* w, const int* h, const int* channels, float* const* const* stored,
                          const void* const* img1, int n, float* const* diffmap, float* maxima, bool device,
                          Stream caller);
-  bool fused() const { return use_fused_; }
   // ButteraugliComparator::Mask (b/butteraugli.cc:793) of the original at every pixel, on the
   // host: mask, mask_dc [3][h][w].  Leaves the resident PsychoImage as it is.
   void mask(float* mask, float* mask_dc);
@@ -274,7 +273,6 @@ class Butteraugli {
   // TMA-staged fused Compare chain (fused_kernels.cuh; CUDA build only)
   struct Fused;
   Fused* fused_ = nullptr;
-  bool use_fused_ = false;
   // nimg images in arena slots kslot planes apart, the original's planes kslot0 apart (kslot0 =
   // kslot: an original per image, 0: one for all; a single image passes 1, 0, 0)
   void fused_opsin(const float* lin, float* xyb, int nimg, int kslot);
@@ -321,7 +319,7 @@ class Butteraugli {
   int capacity_ = 1;
   int kslot_ = 0;
   bool one_original_ = false;  // Slots::kCandidates with capacity > 1
-  Tables t_ = Tables();  // null until built: the pair batch's staged chain builds none
+  Tables t_ = Tables();  // null until built: the CPU port's pair batch builds none
   HostTables ht_;
   MaltaParams malta_[6];
   double asym_w0_, asym_w1_;
@@ -337,15 +335,15 @@ class Butteraugli {
   float* ps1_ = nullptr;     // [10]
   float* sup0_ = nullptr;    // [2] DiffPrecompute neighbour sums of the original (X, Y)
   float* diffs6_ = nullptr;  // [6] Malta pre-pass planes: X uhf, hf, mf; Y uhf, hf, mf
-  float* noise_ = nullptr;   // [2] pre, blurred
+  float* noise_ = nullptr;   // [1] pre (CPU port: [2] pre, blurred)
   float* mpre_ = nullptr;    // [2]
   float* tmp_ = nullptr;     // [3] blur x-pass output
-  float* blr_ = nullptr;     // [3]
+  float* blr_ = nullptr;     // [1] noise blur x-pass output (CPU port: [3] opsin's blurs)
   float* ac_ = nullptr;      // [2]
   float* dm_ = nullptr;      // [2] diffmap, blurred
-  float* mf_blr_ = nullptr;  // [3]
-  float* hf_blr_ = nullptr;  // [2]
-  float* diffs_ = nullptr;   // [1]
+  float* mf_blr_ = nullptr;  // CPU port only: [3]
+  float* hf_blr_ = nullptr;  // CPU port only: [2]
+  float* diffs_ = nullptr;   // CPU port only: [1]
   float* sact_ = nullptr;    // [3] sx, sy1, sy2
   float* mask_ = nullptr;
   float* block_max_ = nullptr;      // [capacity][nblocks]
@@ -359,11 +357,11 @@ class Butteraugli {
 };
 
 // A comparator set: `count` originals of sizes of their own, each analysed once when the set is made, and
-// candidates scored against the original each names (DESIGN.md §4).  On the fused chain the analyses stay in
-// one device buffer, the store: kStoredPlanes planes [h][w] per original, an RGBA original of an 8-bit set
-// twice (over black, then over white).  A call gathers them into the slots of one pair batch of the largest
-// width x largest height.  The staged chain and the CPU port keep the originals' inputs instead and score a
-// call through that batch's compare_batch_sizes*.
+// candidates scored against the original each names (DESIGN.md §4).  The analyses stay in one device buffer,
+// the store: kStoredPlanes planes [h][w] per original, an RGBA original of an 8-bit set twice (over black,
+// then over white).  A call gathers them into the slots of one pair batch of the largest width x largest
+// height.  The CPU port keeps the originals' inputs instead and scores a call through that batch's
+// compare_batch_sizes*.
 class ComparatorSet {
  public:
   // w, h [count], each at least 8x8; channels null: img0[i] float planes [3][h][w], else 8-bit
@@ -384,12 +382,11 @@ class ComparatorSet {
  private:
   std::vector<int> w_, h_, channels_;
   std::unique_ptr<Butteraugli> ba_;
-  void* store_ = nullptr;
-  // byte offsets in store_ of each original's analysis over black and over white (kNone: none); staged chain
-  // and CPU port: of its input, at_[0] only
+  void* store_ = nullptr;  // null in the CPU port
+  // byte offsets in store_ of each original's analysis over black and over white (kNone: none)
   static constexpr size_t kNone = ~static_cast<size_t>(0);
   std::vector<size_t> at_[2];
-  std::vector<std::vector<unsigned char> > host_;  // staged chain and CPU port: the inputs
+  std::vector<std::vector<unsigned char> > host_;  // CPU port: the inputs
 };
 
 #if defined(__CUDACC__) && !defined(GB200_HOSTSIM)

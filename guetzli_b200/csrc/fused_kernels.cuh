@@ -24,13 +24,14 @@
 // per-position scale of ConvolveBorderColumn (b/butteraugli.cc:156-181); tiles that
 // contain such outputs run a second streaming pass with the raw taps.
 // All results are bit-identical to the generic functors in kernels.h (same products, same
-// order of additions), which remain the CPU port's version and the reference for
-// tests/test_gpu_parity.py::test_fused_matches_staged.
+// order of additions), which remain the CPU port's version and, through it, the reference for
+// tests/test_gpu_parity.py::test_fused_matches_port.
 #pragma once
 #include <cuda_runtime.h>
 
 #include "ba_math.h"
 #include "kernels.h"
+#include "malta_unrolled.inc"
 #include "tma.cuh"
 
 namespace gb200 {
@@ -1118,8 +1119,63 @@ __global__ void __launch_bounds__(256) k_tma_mask_y(const __grid_constant__ type
 // S7 Malta line sums of both colour channels in one launch (b/butteraugli.cc:1429-1568;
 // MaltaUnit :914, :1146).  The "diffs" planes (pre-pass, written by EpiMf / EpiHf) are
 // copied as 72 x 40 boxes by the TMA unit, double-buffered over the three bands; the zero
-// fill outside the image is PaddedMaltaUnit's padding.  Line sums as in k_malta_sums
-// (tiled_kernels.cuh): a thread evaluates 2 x 4 pixels from a 9 x 12 register window.
+// fill outside the image is PaddedMaltaUnit's padding.
+//
+// Tile 64 x 32 outputs per CTA (256 threads = 16 column groups x 16
+// rows); a thread makes 4 ADJACENT pixels of a row, for rows ty and ty + 16.  Its 9 x 12
+// sample window comes from shared memory as 27 float4 loads and then lives in registers:
+// every sample is loaded once per 4 pixels instead of once per line-sum term.
+#define GB_MALTA_TILE_W 64
+#define GB_MALTA_TILE_H 32
+#define GB_MALTA_SW (GB_MALTA_TILE_W + 8)
+#define GB_MALTA_SH (GB_MALTA_TILE_H + 8)
+
+// Line sums of the thread's 2 x 4 pixels for one band from the diffs tile; r += sums.
+__device__ __forceinline__ void malta_window_sums(const float* tile, int tx, int ty, bool hf, float r[2][4]) {
+#pragma unroll
+  for (int k = 0; k < 2; ++k) {
+    // window rows ty + 16k .. +8, columns 4tx .. 4tx + 11 of the tile (pixel p of the
+    // thread is at window column 4 + p, window row 4)
+    float win[9][12];
+    const float4* src = reinterpret_cast<const float4*>(tile + (ty + 16 * k) * GB_MALTA_SW + 4 * tx);
+#pragma unroll
+    for (int wy = 0; wy < 9; ++wy) {
+#pragma unroll
+      for (int q = 0; q < 3; ++q) {
+        const float4 v = src[wy * (GB_MALTA_SW / 4) + q];
+        win[wy][4 * q + 0] = v.x;
+        win[wy][4 * q + 1] = v.y;
+        win[wy][4 * q + 2] = v.z;
+        win[wy][4 * q + 3] = v.w;
+      }
+    }
+    float u0 = 0.0f, u1 = 0.0f, u2 = 0.0f, u3 = 0.0f;
+#define GB_T0(dx, dy) win[(dy) + 4][(dx) + 4]
+#define GB_T1(dx, dy) win[(dy) + 4][(dx) + 5]
+#define GB_T2(dx, dy) win[(dy) + 4][(dx) + 6]
+#define GB_T3(dx, dy) win[(dy) + 4][(dx) + 7]
+    if (hf) {
+      GB_MALTA_HF_SUMS(GB_T0, u0)
+      GB_MALTA_HF_SUMS(GB_T1, u1)
+      GB_MALTA_HF_SUMS(GB_T2, u2)
+      GB_MALTA_HF_SUMS(GB_T3, u3)
+    } else {
+      GB_MALTA_LF_SUMS(GB_T0, u0)
+      GB_MALTA_LF_SUMS(GB_T1, u1)
+      GB_MALTA_LF_SUMS(GB_T2, u2)
+      GB_MALTA_LF_SUMS(GB_T3, u3)
+    }
+#undef GB_T0
+#undef GB_T1
+#undef GB_T2
+#undef GB_T3
+    r[k][0] = r[k][0] + u0;
+    r[k][1] = r[k][1] + u1;
+    r[k][2] = r[k][2] + u2;
+    r[k][3] = r[k][3] + u3;
+  }
+}
+
 // grid (ceil(w / 64), ceil(rows / 32), 2 channels), times the images of a batched launch; 256 threads.
 template <int B>
 __global__ void __launch_bounds__(256, 2) k_tma_malta_sums(const __grid_constant__ typename MapArg<B>::type diffs_map_arg,

@@ -292,7 +292,6 @@ void Butteraugli::fused_separate(const float* xyb, float* ps, bool with_diffs, i
 
 // Neighbour sums of DiffPrecompute for the original's PsychoImage (constant during the search).
 void Butteraugli::fused_sup0(int nimg, int kslot) {
-  if (!use_fused_) return;
   const PlaneGeom pg = fused_geom(g_, r_.cr_lo, r_.cr_hi, kslot, kslot);
   const int rows = r_.cr_hi - r_.cr_lo;
   dim3 block(32, 8), grid = grid_of(dim3(cdiv(g_.w, 32), cdiv(rows, 8), nimg), mix_, kMixPx);
@@ -405,8 +404,7 @@ void Butteraugli::fused_compare_launches(int nimg, int kslot, int kslot0) {
     note_launch_end("mask_pre", s_);
   }
   // x passes of the noise blur (S8) and of the three mask blurs in one launch:
-  //   noise_ -> blr_[0] (r 23);  mpre[X] -> tmp_[0] (r 20);  mpre[Y] -> tmp_[1] (r 20);  mpre[Y] -> tmp_[2] (r 5)
-  // (blr_ is a plane group of the staged chain, free here)
+  //   noise_ -> blr_ (r 23);  mpre[X] -> tmp_[0] (r 20);  mpre[Y] -> tmp_[1] (r 20);  mpre[Y] -> tmp_[2] (r 5)
   {
     BlurX4Args<GB_R_NOISE, GB_R_MASKX, GB_R_MASKY1, GB_R_MASKY0> xa;
     xa.out[0] = blr_;
@@ -934,9 +932,20 @@ void Butteraugli::compare_originals(const int* w, const int* h, const int* chann
   fused_compare_sizes(w, h, channels, nullptr, img1, n, diffmap, maxima, device, stored);
 }
 
+// The stage entries on the fused chain.
+void Butteraugli::blur(const float* in, float* out, int nplanes, int id) { fused_blur(in, out, nplanes, id); }
+void Butteraugli::opsin(const float* lin, float* xyb) { fused_opsin(lin, xyb, 1, 0); }
+void Butteraugli::separate(const float* xyb, float* ps) { fused_separate(xyb, ps, false, 1, 0, 0); }
+
+float Butteraugli::compare() {
+  bind();
+  fused_compare_submit();
+  return fused_compare_result();
+}
+
 #endif  // !GB200_HOSTSIM
 
-// The staged chain (the CPU port's only chain) and the mask (Butteraugli members).
+// The mask (Butteraugli members).
 void Butteraugli::mask_activity(const float* xy) {
   r_.px(MaskDiffPreSelf{xy, mpre_, g_}, "mask_diff_pre_self");
   blur(mpre_, sact_, 1, kBlurMaskX);
@@ -972,29 +981,19 @@ void Butteraugli::srgb_to_linear(const uint8_t* src, int n, int channels, int ba
   }
 }
 
-void Butteraugli::blur(const float* in, float* out, int nplanes, int id) {
 #if defined(GB200_HOSTSIM)
+// The CPU port's Compare chain: one launch per stage of the functors of kernels.h.
+void Butteraugli::blur(const float* in, float* out, int nplanes, int id) {
   r_.px(BlurX{in, tmp_, t_.blur[id], g_}, "blur_x", nplanes);
   r_.px(BlurY{tmp_, out, t_.blur[id], g_}, "blur_y", nplanes);
-#else
-  if (use_fused_) return fused_blur(in, out, nplanes, id);
-  launch_blur_tiled(s_, in, tmp_, out, nplanes, t_.blur[id], ht_.blur_taps_n[id].data(), g_, r_.cr_lo,
-                    r_.cr_hi - r_.cr_lo);
-#endif
 }
 
 void Butteraugli::opsin(const float* lin, float* xyb) {
-#if !defined(GB200_HOSTSIM)
-  if (use_fused_) return fused_opsin(lin, xyb, 1, 0);
-#endif
   blur(lin, blr_, 3, kBlurOpsin);
   r_.px(OpsinPx{lin, blr_, xyb, g_}, "opsin_px");
 }
 
 void Butteraugli::separate(const float* xyb, float* ps) {
-#if !defined(GB200_HOSTSIM)
-  if (use_fused_) return fused_separate(xyb, ps, false, 1, 0, 0);
-#endif
   blur(xyb, lf_, 3, kBlurLf);
   r_.px(SubPlanes{xyb, lf_, mf_in_, g_}, "sub_planes", 3);
   blur(mf_in_, mf_blr_, 3, kBlurMf);
@@ -1005,18 +1004,10 @@ void Butteraugli::separate(const float* xyb, float* ps) {
 
 // S1..S13 on the linear RGB planes in lin_ (butteraugli::ButteraugliComparator::Diffmap).
 float Butteraugli::compare() {
-  bind();
-#if !defined(GB200_HOSTSIM)
-  if (use_fused_) {
-    fused_compare_submit();
-    return fused_compare_result();
-  }
-#endif
   const size_t P = g_.plane;
   opsin(lin_, xyb_);
   separate(xyb_, ps1_);
   // S7 Malta: uhf[Y], uhf[X] with 9-tap lines; hf[Y], hf[X], mf[Y], mf[X] with 5-tap lines
-#if defined(GB200_HOSTSIM)
   static const int kMaltaPlane[6] = {kUhfY, kUhfX, kHfY, kHfX, kMfY, kMfX};
   static const int kMaltaAcc[6] = {1, 0, 1, 0, 1, 0};
   for (int i = 0; i < 6; ++i) {
@@ -1032,23 +1023,6 @@ float Butteraugli::compare() {
     acc.g = g_;
     r_.px(acc, i < 2 ? "malta_acc_hf" : "malta_acc_lf");
   }
-#else
-  for (int ch = 0; ch < 2; ++ch) {  // 0 = X, 1 = Y
-    MaltaChannelArgs a;
-    const int planes[3] = {kUhfX + ch, kHfX + ch, kMfX + ch};
-    const int calls[3] = {ch == 1 ? 0 : 1, ch == 1 ? 2 : 3, ch == 1 ? 4 : 5};  // call order, tables.h
-    for (int k = 0; k < 3; ++k) {
-      a.lum0[k] = ps0_ + planes[k] * P;
-      a.lum1[k] = ps1_ + planes[k] * P;
-      a.mp[k] = malta_[calls[k]];
-    }
-    a.acc = ac_ + ch * P;
-    a.g = g_;
-    a.y0 = r_.cr_lo;
-    a.nrows = r_.cr_hi - r_.cr_lo;
-    launch_malta_channel(s_, a, tmp_);  // tmp_ (blur x-pass scratch) is free here
-  }
-#endif
   // S8 + S9 on block_diff_ac[Y]
   r_.px(NoisePre{ps0_ + kHfY * P, ps1_ + kHfY * P, noise_, g_}, "noise_pre");
   blur(noise_, noise_ + P, 1, kBlurNoise);
@@ -1074,6 +1048,8 @@ float Butteraugli::compare() {
   for (int i = 0; i < lanes; ++i) m = std::max(m, part[i]);
   return m;
 }
+
+#endif  // GB200_HOSTSIM
 
 ImageContext::ImageContext(const uint8_t* rgb, int w, int h, int device, bool prepare_now, Comm* comm)
     : ba_(w, h, device, comm) {

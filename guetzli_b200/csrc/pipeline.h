@@ -102,7 +102,7 @@ class ImageContext {
   }
   // the same in two halves: compare_begin() queues the kernels, compare_end() waits for the
   // distance; stream work queued in between runs behind the metric's kernels (where the
-  // launches need a host round trip -- strip mode, the staged chain -- compare_begin() does it all)
+  // launches need a host round trip -- strip mode, the CPU port -- compare_begin() does it all)
   void compare_begin() {
     compare_render();
     ba_.compare_begin();

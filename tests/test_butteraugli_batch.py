@@ -140,25 +140,6 @@ def test_cuda_batch_matches_reference(cuda_lib, ref, h, w, n):
     check_against_reference(cuda_lib, ref, h, w, n, comparator=True)
 
 
-@pytest.mark.gpu
-def test_cuda_batch_matches_reference_staged(cuda_lib, ref, monkeypatch):
-    """GB200_COMPARE=staged: the batch scores pair by pair through the staged chain, host and device entry."""
-    torch = pytest.importorskip("torch")
-    monkeypatch.setenv("GB200_COMPARE", "staged")
-    h, w, n = PAIR[0]
-    a, b = pairs(h, w, n)
-    batch = gb.ButteraugliBatch(h, w, n, lib=cuda_lib)
-    try:
-        dm, score = batch.diffmap(a, b)
-        dm_t, score_t = batch.diffmap(torch.from_numpy(a).cuda(), torch.from_numpy(b).cuda())
-    finally:
-        batch.close()
-    for i in range(n):
-        dm0, score0 = ref.butteraugli_interface(a[i], b[i])
-        assert score[i] == score0 and parity.bits_equal(dm[i], dm0), f"pair {i}"
-    assert (score_t == score).all() and parity.bits_equal(dm_t.cpu().numpy(), dm)
-
-
 def isolation_pairs(h, w, n):
     """Slots alternate a high-contrast noise pair with an identical flat-gray pair."""
     a, b = [], []

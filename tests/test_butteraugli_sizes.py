@@ -322,26 +322,6 @@ def test_cuda_sizes_device_path(cuda_lib):
 
 
 @pytest.mark.gpu
-def test_cuda_sizes_staged(cuda_lib, ref, monkeypatch):
-    """GB200_COMPARE=staged: pair by pair through metrics of each pair's size, host and device entry."""
-    torch = pytest.importorskip("torch")
-    monkeypatch.setenv("GB200_COMPARE", "staged")
-    bh, bw, shapes = SETS["repeated"]
-    a, b = pairs_of(shapes)
-    batch = gb.ButteraugliBatch(bh, bw, len(shapes), lib=cuda_lib)
-    try:
-        dm, score = batch.diffmap_sizes(a, b)
-        dm_t, score_t = batch.diffmap_sizes([torch.from_numpy(x).cuda() for x in a],
-                                            [torch.from_numpy(x).cuda() for x in b])
-    finally:
-        batch.close()
-    for i in range(len(a)):
-        dm0, score0 = ref.butteraugli_interface(a[i], b[i])
-        assert score[i] == score0 and parity.bits_equal(dm[i], dm0), f"pair {i}"
-        assert score_t[i] == score[i] and parity.bits_equal(dm_t[i].cpu().numpy(), dm[i]), f"pair {i} (device)"
-
-
-@pytest.mark.gpu
 def test_cuda_refusals_launch_nothing(cuda_lib):
     torch = pytest.importorskip("torch")
     launches = gb.counters(lib=cuda_lib)[0]

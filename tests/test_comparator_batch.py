@@ -168,26 +168,6 @@ def test_cuda_comparator_batch_matches_reference(cuda_lib, ref, h, w, n):
 
 
 @pytest.mark.gpu
-def test_cuda_comparator_batch_staged(cuda_lib, ref, monkeypatch):
-    """GB200_COMPARE=staged: the comparator scores candidate by candidate through the staged chain, from
-    the host and the device entry."""
-    torch = pytest.importorskip("torch")
-    monkeypatch.setenv("GB200_COMPARE", "staged")
-    h, w, n = PAIR[0]
-    a, b = candidates(h, w, n)
-    cmp = gb.Comparator(a, capacity=n, lib=cuda_lib)
-    try:
-        dm, score = cmp.diffmap(b)
-        dm_t, score_t = cmp.diffmap(torch.from_numpy(b).cuda())
-    finally:
-        cmp.close()
-    for i in range(n):
-        dm0, score0 = ref.butteraugli_interface(a, b[i])
-        assert score[i] == score0 and parity.bits_equal(dm[i], dm0), f"candidate {i}"
-    assert (score_t == score).all() and parity.bits_equal(dm_t.cpu().numpy(), dm)
-
-
-@pytest.mark.gpu
 @pytest.mark.parametrize("h,w,n", [(40, 56, 6), (300, 411, 5)])
 def test_cuda_slots_are_isolated(cuda_lib, h, w, n):
     """Candidates alternate noise with exact copies of the original: the copies score 0 with an all-zero

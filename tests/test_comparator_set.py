@@ -429,24 +429,6 @@ def test_cuda_srgb_set_matches_pairs(cuda_lib, ref):
 
 
 @pytest.mark.gpu
-def test_cuda_set_staged(cuda_lib, monkeypatch):
-    """GB200_COMPARE=staged gives the fused chain's bits, host and device memory."""
-    torch = pytest.importorskip("torch")
-    shapes = [(40, 56), (17, 9), (64, 64), (8, 8), (33, 20)]
-    index = [2, 0, 4, 1, 2, 3]
-    origs, cands = float_set(shapes, index)
-    fused = scored(cuda_lib, origs, index, cands)
-    monkeypatch.setenv("GB200_COMPARE", "staged")
-    s = make_set(cuda_lib, origs, len(index))
-    try:
-        assert_same(s.diffmap(index, cands), fused, "staged, host")
-        dm, score = s.diffmap(index, [torch.from_numpy(x).cuda() for x in cands])
-        assert_same(([d.cpu().numpy() for d in dm], score), fused, "staged, device")
-    finally:
-        s.close()
-
-
-@pytest.mark.gpu
 def test_cuda_set_refusals(cuda_lib):
     """Every refusal launches nothing; the device entries refuse a host pointer and a CPU tensor."""
     torch = pytest.importorskip("torch")

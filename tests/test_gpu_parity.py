@@ -177,23 +177,18 @@ AB_IMAGES = [("noise", 40, 33, 2), ("gradnoise", 70, 51, 3), ("noise", 136, 200,
 
 
 @pytest.mark.parametrize("gen,h,w,seed", AB_IMAGES)
-def test_fused_matches_staged(cuda_lib, gen, h, w, seed):
-    """The TMA-staged fused Compare chain (fused_kernels.cuh, default) against the staged
-    round-1 sequence of the same library (GB200_COMPARE=staged): every intermediate that both
-    expose must have identical bits.  Localises a defect to a stage."""
-    import os
+def test_fused_matches_port(cuda_lib, port_lib, gen, h, w, seed):
+    """The TMA-staged fused Compare chain (fused_kernels.cuh) against the CPU port's chain of one
+    launch per stage (the functors of kernels.h, pinned to the reference): every intermediate
+    that both expose must have identical bits.  Localises a defect to a stage."""
     import guetzli_b200 as gb
     rgb = getattr(synth, gen)(h, w, seed)
     rng = np.random.default_rng(seed)
     plane = (rng.random((h, w), dtype=np.float32) * 255).astype(np.float32)
     q = parity.test_quant(seed)
     out = {}
-    for mode in ("staged", "fused"):
-        os.environ["GB200_COMPARE"] = mode
-        try:
-            img = gb.DeviceImage(rgb, lib=cuda_lib)
-        finally:
-            del os.environ["GB200_COMPARE"]
+    for name, lib in (("port", port_lib), ("fused", cuda_lib)):
+        img = gb.DeviceImage(rgb, lib=lib)
         r = {}
         for i in range(len(parity.BLUR_SPECS)):
             r["blur%d" % i] = img.debug_blur(plane, i)
@@ -212,13 +207,13 @@ def test_fused_matches_staged(cuda_lib, gen, h, w, seed):
         r["distance2"] = np.float32(img.compare())
         r["distmap2"] = img.distmap()
         img.close()
-        out[mode] = r
-    for key in out["staged"]:
-        a, b = np.asarray(out["staged"][key]), np.asarray(out["fused"][key])
+        out[name] = r
+    for key in out["port"]:
+        a, b = np.asarray(out["port"][key]), np.asarray(out["fused"][key])
         if not parity.bits_equal(a, b):
             bad = np.argwhere(a.view(np.uint32) != b.view(np.uint32))
             raise AssertionError(f"{key}: {len(bad)} of {a.size} values differ, first at {bad[0].tolist()}: "
-                                 f"staged {a[tuple(bad[0])]!r} fused {b[tuple(bad[0])]!r}; "
+                                 f"port {a[tuple(bad[0])]!r} fused {b[tuple(bad[0])]!r}; "
                                  f"last at {bad[-1].tolist()}")
 
 

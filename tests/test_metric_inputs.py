@@ -509,17 +509,6 @@ def test_cuda_slots(cuda_lib, port_lib, ref, h, w):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("h,w", [(40, 56), (1080, 100)], ids=lambda v: str(v))
-def test_cuda_staged(cuda_lib, port_lib, ref, monkeypatch, h, w):
-    """GB200_COMPARE=staged: the one-kernel-per-stage chain on the same cases, single and batched."""
-    monkeypatch.setenv("GB200_COMPARE", "staged")
-    for c in CASES:
-        if c[1:] == (h, w):
-            check_case(cuda_lib, port_lib, ref, *c, device=True)
-    check_slots(cuda_lib, port_lib, ref, h, w, device=True)
-
-
-@pytest.mark.gpu
 @pytest.mark.parametrize("name,h,w", STAGE_CASES, ids=[case_id(c) for c in STAGE_CASES])
 def test_cuda_stages(cuda_lib, ref, name, h, w):
     check_stages(cuda_lib, ref, name, h, w)

@@ -486,35 +486,6 @@ def test_cuda_batch_and_comparator(cuda_lib, ref, h, w, n, channels):
 
 
 @pytest.mark.gpu
-def test_cuda_staged_chain(cuda_lib, monkeypatch):
-    """GB200_COMPARE=staged: the pairs go through metrics of their own and the candidates one by one,
-    from host and device memory, with the same results as the fused chain."""
-    torch = pytest.importorskip("torch")
-    h, w, n = 40, 56, 3
-    a, b = batch_pairs(h, w, n, 4)
-    o, c = candidates(h, w, n, 4)
-
-    def run():
-        batch = gb.ButteraugliBatch(h, w, n, lib=cuda_lib)
-        cmp = gb.Comparator.from_srgb(o, capacity=n, lib=cuda_lib)
-        try:
-            out = [batch.diffmap_srgb(a, b), cmp.diffmap(c)]
-            dm, s = batch.diffmap_srgb(torch.from_numpy(a).cuda(), torch.from_numpy(b).cuda())
-            dmc, sc = cmp.diffmap(torch.from_numpy(c).cuda())
-            return out + [(dm.cpu().numpy(), s), (dmc.cpu().numpy(), sc)]
-        finally:
-            batch.close()
-            cmp.close()
-
-    fused = run()
-    monkeypatch.setenv("GB200_COMPARE", "staged")
-    staged = run()
-    for k, ((dm0, s0), (dm1, s1)) in enumerate(zip(fused, staged)):
-        assert (s0 == s1).all() and parity.bits_equal(dm1, dm0), f"result {k}"
-    assert (fused[0][1] == fused[2][1]).all() and (fused[1][1] == fused[3][1]).all()
-
-
-@pytest.mark.gpu
 def test_cuda_refusals_launch_nothing(cuda_lib):
     refusals(cuda_lib, "{} is not device memory of device 0")
 

@@ -397,28 +397,6 @@ def test_cuda_device_path(cuda_lib):
 
 
 @pytest.mark.gpu
-def test_cuda_staged(cuda_lib, monkeypatch):
-    """GB200_COMPARE=staged: pair by pair through pair batches of each pair's size, from host and device
-    memory, with the fused chain's bits."""
-    torch = pytest.importorskip("torch")
-    a, b, bh, bw = choice_pairs()
-
-    def run():
-        dm, s = score_set(cuda_lib, bh, bw, a, b)
-        dmt, st = score_set(cuda_lib, bh, bw, [torch.from_numpy(x).cuda() for x in a],
-                            [torch.from_numpy(x).cuda() for x in b])
-        return [(dm, s), ([x.cpu().numpy() for x in dmt], st)]
-
-    fused = run()
-    monkeypatch.setenv("GB200_COMPARE", "staged")
-    staged = run()
-    for k in range(2):
-        assert (staged[k][1] == fused[0][1]).all(), k
-        assert all(parity.bits_equal(x, y) for x, y in zip(staged[k][0], fused[0][0])), k
-    assert (fused[1][1] == fused[0][1]).all() and all(parity.bits_equal(x, y) for x, y in zip(fused[1][0], fused[0][0]))
-
-
-@pytest.mark.gpu
 def test_cuda_refusals_launch_nothing(cuda_lib):
     torch = pytest.importorskip("torch")
     refusals(cuda_lib, "img0[0] is not device memory of device 0")
