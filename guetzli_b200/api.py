@@ -104,6 +104,12 @@ def load_library(path=None):
     lib.gb200_jpeg_dimensions.argtypes = [C.c_void_p, C.c_size_t, P(C.c_int), P(C.c_int)]
     lib.gb200_jpeg_decode_rgb.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]
     lib.gb200_jpeg_decode_rgb_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
+    lib.gb200_jpeg_dimensions_from_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
+                                                      C.c_void_p, C.c_void_p]
+    lib.gb200_jpeg_decode_rgb_from_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
+                                                      C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.gb200_debug_entropy_decode.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_size_t,
+                                               P(C.c_int)]
     lib.gb200_butteraugli_diffmap.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                               P(C.c_double)]
     lib.gb200_butteraugli_comparator_create.restype = C.c_void_p
@@ -351,18 +357,30 @@ def decode_jpeg(data, device=0, cuda=True, lib=None):
     """The pixels libjpeg-turbo gives for JPEG files, as the butteraugli tool reads them (ReadJPEG,
     butteraugli_main.cc:157: JDCT_ISLOW, fancy upsampling, RGB, gray replicated), decoded on the GPU.
 
-    data: one bytes-like object, or a list of them (decoded together in one pass whatever their sizes).
-    Returns a uint8 [h][w][3] CUDA tensor on cuda:`device` per file, written after the work queued on that
-    device's current torch stream, or a numpy array where cuda is False; a list for a list.  They go as
-    they are into the 8-bit butteraugli entries (butteraugli_srgb, diffmap_sizes_srgb, from_srgb).
-    A file the decoder does not reproduce libjpeg on raises ValueError naming its index and the reason:
-    what ReadJpeg rejects, CMYK / YCCK, samplings other than 4:4:4, 4:2:2 and 4:2:0, and progressive files
-    that libjpeg would block-smooth."""
+    data: one file or a list of files (decoded together in one pass whatever their sizes), each a bytes-like
+    object in host memory or a contiguous 1-D torch.uint8 CUDA tensor holding the file's bytes.  A list is
+    all host bytes or all CUDA tensors, the tensors on one device.
+    Returns a uint8 [h][w][3] CUDA tensor per file, written after the work queued on the device's current
+    torch stream, or a numpy array where cuda is False; a list for a list.  Host bytes are decoded on
+    cuda:`device`; CUDA tensors on their own device, where the Huffman decoding of sequential files runs
+    too (the headers are read from prefixes copied to the host, and other files are copied back whole).
+    The outputs go as they are into the 8-bit butteraugli entries (butteraugli_srgb, diffmap_sizes_srgb,
+    from_srgb).  A file the decoder does not reproduce libjpeg on raises ValueError naming its index and
+    the reason: what ReadJpeg rejects, CMYK / YCCK, samplings other than 4:4:4, 4:2:2 and 4:2:0, and
+    progressive files that libjpeg would block-smooth.  Mixing host bytes and tensors, tensors on several
+    devices or not contiguous 1-D uint8, and cuda=False with tensors raise ValueError as well."""
     lib = lib or load_library()
-    single = isinstance(data, (bytes, bytearray, memoryview))
-    files = [bytes(d) for d in ([data] if single else data)]
-    if not files:
+    single = isinstance(data, (bytes, bytearray, memoryview)) or _is_torch_tensor(data)
+    items = [data] if single else list(data)
+    if not items:
         raise ValueError("decode_jpeg: no files")
+    tensors = [_is_torch_tensor(d) for d in items]
+    if any(tensors):
+        if not all(tensors):
+            raise ValueError("decode_jpeg: a list mixes host bytes and torch tensors")
+        out = _decode_jpeg_tensors(items, cuda, lib)
+        return out[0] if single else out
+    files = [bytes(d) for d in items]
     bufs = [np.frombuffer(f, dtype=np.uint8) for f in files]
     shapes = []
     for b in bufs:
@@ -384,19 +402,68 @@ def decode_jpeg(data, device=0, cuda=True, lib=None):
         outp = (C.c_void_p * n)(*[o.ctypes.data for o in out])
         ok = lib.gb200_jpeg_decode_rgb(ptrs, lens, n, device, outp)
     if not ok:
-        msg = _err(lib)
-        if ": file " in msg:
-            raise ValueError(msg)
-        raise RuntimeError(msg)
+        _raise_decode_error(lib)
     return out[0] if single else out
 
 
-def read_jpeg(jpeg_in, lib=None):
-    """ReadJpeg alone (test hook) -> (ok, dims, quantised coefficients concatenated over components)."""
+def _raise_decode_error(lib):
+    msg = _err(lib)
+    if ": file " in msg:
+        raise ValueError(msg)
+    raise RuntimeError(msg)
+
+
+def _decode_jpeg_tensors(items, cuda, lib):
+    """decode_jpeg on files held in CUDA tensors (gb200_jpeg_decode_rgb_from_device)."""
+    import torch
+    if not cuda:
+        raise ValueError("decode_jpeg: files in torch tensors are decoded into CUDA tensors; cuda=False takes "
+                         "host bytes only")
+    for i, t in enumerate(items):
+        if not t.is_cuda or t.dtype != torch.uint8 or t.dim() != 1 or not t.is_contiguous():
+            raise ValueError(f"decode_jpeg: file {i} must be a contiguous 1-D torch.uint8 CUDA tensor, got "
+                             f"{t.dtype} {tuple(t.shape)} on {t.device}")
+    dev = items[0].device
+    if any(t.device != dev for t in items):
+        raise ValueError("decode_jpeg: the tensors are on more than one device")
+    n = len(items)
+    ptrs = (C.c_void_p * n)(*[t.data_ptr() if t.numel() else None for t in items])
+    lens = (C.c_size_t * n)(*[t.numel() for t in items])
+    stream = torch.cuda.current_stream(dev).cuda_stream
+    w, h = (C.c_int * n)(), (C.c_int * n)()
+    if not lib.gb200_jpeg_dimensions_from_device(ptrs, lens, n, dev.index, stream, w, h):
+        raise RuntimeError(_err(lib))
+    # a file without a readable frame size gets a 1x1 output; the decoder then refuses it with its reason
+    shapes = [(h[i], w[i], 3) if w[i] > 0 else (1, 1, 3) for i in range(n)]
+    out = [torch.empty(s, dtype=torch.uint8, device=dev) for s in shapes]
+    outp = (C.c_void_p * n)(*[o.data_ptr() for o in out])
+    ws = (C.c_int * n)(*[s[1] for s in shapes])
+    hs = (C.c_int * n)(*[s[0] for s in shapes])
+    if not lib.gb200_jpeg_decode_rgb_from_device(ptrs, lens, n, dev.index, ws, hs, outp, stream):
+        _raise_decode_error(lib)
+    return out
+
+
+def entropy_decode(jpeg_in, S, lib=None, cap=1 << 24):
+    """The device path's entropy decoding of one file with subsequences of S bits (test hook) -> (taken,
+    coefficients): where the device path takes the file, its quantised coefficients concatenated over the
+    components as read_jpeg gives them, at the start of a buffer of cap values whose rest stays zero."""
+    lib = lib or load_library()
+    buf = np.frombuffer(bytes(jpeg_in), dtype=np.uint8)
+    out = np.zeros(cap, dtype=np.int16)
+    status = C.c_int()
+    if not lib.gb200_debug_entropy_decode(buf.ctypes.data if buf.size else None, buf.size, S, out.ctypes.data, cap,
+                                          C.byref(status)):
+        raise RuntimeError(_err(lib))
+    return bool(status.value), (out if status.value else None)
+
+
+def read_jpeg(jpeg_in, lib=None, cap=1 << 24):
+    """ReadJpeg alone (test hook) -> (ok, dims, quantised coefficients concatenated over components); ok is
+    False as well where there are more than cap coefficients."""
     lib = lib or load_library()
     buf = np.frombuffer(bytes(jpeg_in), dtype=np.uint8)
     dims = (C.c_int * 11)()
-    cap = 1 << 24
     out = np.zeros(cap, dtype=np.int16)
     ok = lib.gb200_debug_read_jpeg(buf.ctypes.data, buf.size, dims, out.ctypes.data, cap)
     d = list(dims)

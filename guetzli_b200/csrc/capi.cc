@@ -898,6 +898,60 @@ int gb200_jpeg_decode_rgb_device(const uint8_t* const* jpeg, const size_t* len, 
   return jpeg_decode("jpeg_decode_rgb_device", jpeg, len, n, device, out_dev, true, stream);
 }
 
+namespace {
+// the pointer checks of the *_from_device entries: every input and output pointer, before anything runs
+void check_jpeg_device_args(const char* who, const uint8_t* const* jpeg, const size_t* len, int n, int device,
+                            uint8_t* const* out) {
+  if (n < 1) throw std::runtime_error(std::string(who) + ": n must be at least 1");
+  if (jpeg == nullptr || len == nullptr) throw std::runtime_error(std::string(who) + ": jpeg and len must not be null");
+  for (int i = 0; i < n; ++i) {
+    const std::string k = "[" + std::to_string(i) + "]";
+    // an empty file may have no bytes at all; the decode then refuses it with read_jpeg's reason
+    if (jpeg[i] == nullptr && len[i] != 0) throw std::runtime_error(std::string(who) + ": jpeg" + k + " is null");
+    if (out && out[i] == nullptr) throw std::runtime_error(std::string(who) + ": out" + k + " is null");
+    const std::string nj = "jpeg" + k, no = "out" + k;
+    const void* ptrs[2] = {len[i] ? jpeg[i] : nullptr, out ? out[i] : nullptr};
+    const char* what[2] = {nj.c_str(), no.c_str()};
+    check_device_pointers(who, device, ptrs, what, out ? 2 : 1);
+  }
+}
+}  // namespace
+
+int gb200_jpeg_dimensions_from_device(const uint8_t* const* jpeg_dev, const size_t* len, int n, int device,
+                                      void* stream, int* width, int* height) {
+  return guarded([&]() {
+    const char* who = "jpeg_dimensions_from_device";
+    if (width == nullptr || height == nullptr)
+      throw std::runtime_error(std::string(who) + ": width and height must not be null");
+    check_jpeg_device_args(who, jpeg_dev, len, n, device, nullptr);
+    gb200::jpeg_dimensions_from_device(jpeg_dev, len, n, device, caller_stream(stream), width, height);
+  });
+}
+
+int gb200_jpeg_decode_rgb_from_device(const uint8_t* const* jpeg_dev, const size_t* len, int n, int device,
+                                      const int* width, const int* height, uint8_t* const* out_dev, void* stream) {
+  return guarded([&]() {
+    const char* who = "jpeg_decode_rgb_from_device";
+    if (width == nullptr || height == nullptr || out_dev == nullptr)
+      throw std::runtime_error(std::string(who) + ": width, height and out must not be null");
+    check_jpeg_device_args(who, jpeg_dev, len, n, device, out_dev);
+    gb200::jpeg_decode_rgb_from_device(who, jpeg_dev, len, n, device, width, height, out_dev, caller_stream(stream));
+  });
+}
+
+int gb200_debug_entropy_decode(const uint8_t* jpeg_in, size_t jpeg_len, int S, int16_t* out, size_t out_cap,
+                               int* status) {
+  return guarded([&]() {
+    if (jpeg_in == nullptr || status == nullptr) throw std::runtime_error("debug_entropy_decode: null argument");
+    std::vector<int16_t> c;
+    *status = gb200::jpeg_debug_entropy_decode(jpeg_in, jpeg_len, S, &c) ? 1 : 0;
+    if (*status) {
+      if (c.size() > out_cap) throw std::runtime_error("debug_entropy_decode: out is too small");
+      memcpy(out, c.data(), c.size() * sizeof(int16_t));
+    }
+  });
+}
+
 int gb200_debug_read_jpeg(const uint8_t* jpeg_in, size_t jpeg_len, int* dims, int16_t* out, size_t out_cap) {
   gb200::JpegInput jpg;
   std::string err;

@@ -48,6 +48,16 @@ GB_HD unsigned int hd_atomic_or(unsigned int* p, unsigned int v) {
   return __atomic_fetch_or(p, v, __ATOMIC_RELAXED);
 #endif
 }
+GB_HD unsigned int hd_atomic_min(unsigned int* p, unsigned int v) {
+#if defined(__CUDA_ARCH__)
+  return atomicMin(p, v);
+#else
+  unsigned int old = __atomic_load_n(p, __ATOMIC_RELAXED);
+  while (v < old && !__atomic_compare_exchange_n(p, &old, v, true, __ATOMIC_RELAXED, __ATOMIC_RELAXED)) {
+  }
+  return old;
+#endif
+}
 GB_HD unsigned int hd_float_bits(float f) {
 #if defined(__CUDA_ARCH__)
   return __float_as_uint(f);

@@ -131,21 +131,15 @@ namespace {
 
 struct Fail {
   std::string* err;
+  bool quiet = false;
   bool operator()(const char* msg) const {
     if (err) *err = msg;
-    fprintf(stderr, "%s\n", msg);
+    if (!quiet) fprintf(stderr, "%s\n", msg);
     return false;
   }
 };
 
-// Canonical Huffman code of one DHT table: decode by code length.
-struct HuffTable {
-  bool defined = false;
-  int max_code[18];   // largest code of each length, -1 if none
-  int val_offset[18]; // index of the first symbol of each length minus its first code
-  uint8_t symbols[256];
-  int num_symbols = 0;
-};
+typedef JpegHuffTable HuffTable;
 
 // Segment cursor with bounds checks.
 struct Cursor {
@@ -233,15 +227,16 @@ int decode_symbol(const HuffTable& t, ScanBits* br) {
 
 inline int extend(int v, int s) { return v < (1 << (s - 1)) ? v - (1 << s) + 1 : v; }
 
-struct ScanSpec {
-  int ncomp;
-  int comp[4], dc_tbl[4], ac_tbl[4];
-  int ss, se, ah, al;
-};
+typedef JpegScanSpec ScanSpec;
 
 class Reader {
  public:
   Reader(const uint8_t* data, size_t len, JpegInput* jpg, std::string* err) : c_{data, len, 0}, jpg_(jpg), fail_{err} {
+    memset(progression_, 0, sizeof(progression_));
+  }
+  // header only: stop after the first SOS header, quietly, and allocate no coefficients
+  explicit Reader(const uint8_t* data, size_t len, JpegScanHeader* hdr)
+      : c_{data, len, 0}, jpg_(&hdr->jpg), fail_{nullptr, true}, hdr_(hdr) {
     memset(progression_, 0, sizeof(progression_));
   }
 
@@ -265,6 +260,7 @@ class Reader {
       } else if (marker == 0xd9) {
         // end of image
       } else if (marker == 0xda) {
+        if (hdr_) return first_scan_header();
         ok = scan();
       } else if (marker == 0xdb) {
         ok = quant_tables();
@@ -279,8 +275,15 @@ class Reader {
       }
       if (!ok) return false;
     } while (marker != 0xd9);
+    if (hdr_) return false;  // no scan
     if (!have_frame_) return fail_("Missing SOF marker.");
     if (c_.pos < c_.len) jpg_->tail_data.assign(reinterpret_cast<const char*>(c_.data + c_.pos), c_.len - c_.pos);
+    return finish_tables();
+  }
+
+ private:
+  // what run() checks once the last segment is read
+  bool finish_tables() {
     // component Tq -> position of that table in the list (first match)
     for (JpegComponent& comp : jpg_->components) {
       int found = -1;
@@ -296,7 +299,19 @@ class Reader {
     return true;
   }
 
- private:
+  // header-only read: the first SOS header ends it, with the tables and position as they stand there
+  bool first_scan_header() {
+    if (!scan_header(&hdr_->scan)) return false;
+    if (!finish_tables()) return false;
+    for (int i = 0; i < 4; ++i) {
+      hdr_->dc[i] = dc_[i];
+      hdr_->ac[i] = ac_[i];
+    }
+    hdr_->restart_interval = restart_interval_;
+    hdr_->scan_start = c_.pos;
+    return true;
+  }
+
   // Bytes between segments that are not a marker the format knows are skipped.
   void skip_to_marker() {
     static const uint8_t kKnown[64] = {
@@ -350,7 +365,7 @@ class Reader {
       comp.height_in_blocks = jpg_->mcu_rows * comp.v_samp;
       const uint64_t nb = static_cast<uint64_t>(comp.width_in_blocks) * comp.height_in_blocks;
       if (nb > (1ull << 21)) return fail_("Image too large.");
-      comp.coeffs.assign(static_cast<size_t>(nb) * 64, 0);
+      if (!hdr_) comp.coeffs.assign(static_cast<size_t>(nb) * 64, 0);
     }
     return segment_end(start, marker_len);
   }
@@ -674,6 +689,7 @@ class Reader {
   uint16_t progression_[4][64];
   bool progressive_ = false, have_frame_ = false;
   int restart_interval_ = 0, num_dht_ = 0, eobrun_ = -1;
+  JpegScanHeader* hdr_ = nullptr;
 };
 
 }  // namespace
@@ -708,6 +724,12 @@ bool read_jpeg_dimensions(const uint8_t* data, size_t len, int* width, int* heig
 bool read_jpeg(const uint8_t* data, size_t len, JpegInput* jpg, std::string* err) {
   *jpg = JpegInput();
   Reader r(data, len, jpg, err);
+  return r.run();
+}
+
+bool read_jpeg_header(const uint8_t* data, size_t len, JpegScanHeader* hdr) {
+  *hdr = JpegScanHeader();
+  Reader r(data, len, hdr);
   return r.run();
 }
 

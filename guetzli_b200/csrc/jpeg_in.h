@@ -41,8 +41,38 @@ struct JpegInput {
   bool is_420() const;                // g/jpeg_data.cc:24
 };
 
+// Canonical Huffman code of one DHT table, decoded by code length (decode_symbol in jpeg_in.cc).
+struct JpegHuffTable {
+  bool defined = false;
+  int max_code[18];    // largest code of each length, -1 if none
+  int val_offset[18];  // index of the first symbol of each length minus its first code
+  uint8_t symbols[256];
+  int num_symbols = 0;
+};
+
+// One SOS header: the frame's components it carries and their tables, spectral selection, approximation.
+struct JpegScanSpec {
+  int ncomp;
+  int comp[4], dc_tbl[4], ac_tbl[4];
+  int ss, se, ah, al;
+};
+
+// A file read up to and including its first SOS header (read_jpeg_header).
+struct JpegScanHeader {
+  JpegInput jpg;  // frame, quant tables (Tq fixed up as read_jpeg does), APPn / COM; no coefficients
+  JpegHuffTable dc[4], ac[4];
+  JpegScanSpec scan;
+  int restart_interval = 0;
+  size_t scan_start = 0;  // offset of the first byte of entropy-coded data
+};
+
 // Returns false (message in *err) for streams the reference rejects.
 bool read_jpeg(const uint8_t* data, size_t len, JpegInput* jpg, std::string* err);
+
+// read_jpeg up to the end of the first SOS header, with the same checks on what it reads and the ones
+// read_jpeg makes after the last segment (quant tables found, DHT count); it prints nothing.  False if
+// read_jpeg would refuse what was read, or if the bytes end first (data may be a prefix of the file).
+bool read_jpeg_header(const uint8_t* data, size_t len, JpegScanHeader* hdr);
 
 // ReadJpeg(JPEG_READ_HEADER): only the frame size (the CLI's memory-limit check,
 // g/guetzli.cc:306-312).

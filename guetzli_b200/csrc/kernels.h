@@ -218,6 +218,467 @@ struct JpegUpsampleYccRgb {
   }
 };
 
+// ---------------------------------------------------------------------------
+// Entropy decoding of sequential scans on the device (jpeg_entropy_decode, pipeline.cu), for files whose
+// first scan carries every component with Ss = 0, Se = 63, Ah = Al = 0.  Each functor restates a part of
+// read_jpeg's scan() / first_pass() / ScanBits (jpeg_in.cc), so that a file decodes to read_jpeg's
+// coefficients or is flagged in its status word and decoded on the host instead.
+//
+// Bytes: the call's scan bytes are one flat range, file f's readable ones (before len - 2, where
+// ScanBits stops) at [byte0[f], byte0[f + 1]).  The segment pass compacts them, stuffed zeros and RSTn
+// dropped, into one stream; restart interval I is bytes [cbyte, cbyte + nbytes) of it.
+
+constexpr unsigned kJpegBadSegment = 1u;  // scan data does not end in EOI, or RSTn missing / out of order
+constexpr unsigned kJpegBadCode = 2u;     // an error first_pass() / scan() raises, in the synchronised pass
+constexpr unsigned kJpegBadRange = 4u;    // a block fails libjpeg_decodable's SIMD-range test
+constexpr unsigned kJpegBadSync = 8u;     // the speculative decode did not converge within its rounds
+constexpr int kJpegMaxSlots = 10;         // blocks per MCU
+
+struct JpegScanFile {
+  const uint8_t* data;  // the file
+  long long len;
+  int s0;               // first byte of entropy-coded data
+  int int0, nint;       // the file's restart intervals in the call
+  int R;                // restart interval in MCUs; 0 none
+  int mcus, mcus_per_row;
+  int nslot;            // blocks per MCU, in scan order
+  int period;           // smallest p dividing nslot with slot s using slot s % p's tables: the decoder's states
+                        // count slots modulo p, since the bits cannot tell slots with the same tables apart
+  int slot_comp[kJpegMaxSlots], slot_ix[kJpegMaxSlots], slot_iy[kJpegMaxSlots];
+  int slot_dc[kJpegMaxSlots], slot_ac[kJpegMaxSlots];  // lookup tables of the call
+  int comp_h[3], comp_v[3], bw[3];  // MCU blocks per component (1 x 1 non-interleaved), blocks per row
+  int blk0[3];                      // first block of each component in the coefficients
+};
+
+struct JpegInterval {
+  long long cbyte;  // first compacted byte
+  int nbytes;
+  int file, mcu0, nmcu;
+};
+
+GB_HD bool jpeg_is_rst(int b) { return b >= 0xd0 && b <= 0xd7; }
+
+// 4.1a: per scan byte, the first 0xFF followed by neither 0x00 nor RSTn ends the file's data (end[f] starts
+// at len - 2, the file's last two bytes)
+struct JpegSegEnd {
+  const JpegScanFile* files;
+  const int* byte0;  // [n + 1]
+  int n;
+  unsigned* end;
+  GB_HD void operator()(int i) const {
+    const int f = jpeg_find(byte0, n, i);
+    const JpegScanFile& d = files[f];
+    const long long p = d.s0 + (i - byte0[f]);
+    if (d.data[p] != 0xff) return;
+    const int nx = d.data[p + 1];
+    if (nx != 0 && !jpeg_is_rst(nx)) hd_atomic_min(&end[f], static_cast<unsigned>(p));
+  }
+};
+
+// 4.1b: per scan byte before the end: keep[i] = 1 for a data byte, rst[i] = 1 for the 0xFF of an RSTn
+struct JpegSegFlags {
+  const JpegScanFile* files;
+  const int* byte0;
+  int n;
+  const unsigned* end;
+  unsigned* keep;
+  unsigned* rst;
+  GB_HD void operator()(int i) const {
+    const int f = jpeg_find(byte0, n, i);
+    const JpegScanFile& d = files[f];
+    const long long p = d.s0 + (i - byte0[f]);
+    unsigned k = 0, r = 0;
+    if (p < static_cast<long long>(end[f])) {
+      const int b = d.data[p];
+      const bool after_ff = p > d.s0 && d.data[p - 1] == 0xff;
+      if (b == 0xff && jpeg_is_rst(d.data[p + 1])) {
+        r = 1;
+      } else if (!(after_ff && (b == 0 || jpeg_is_rst(b)))) {
+        k = 1;
+      }
+    }
+    keep[i] = k;
+    rst[i] = r;
+  }
+};
+
+// 4.1c: data bytes to their compacted place; RSTn to the start of the next interval, checked in order
+struct JpegSegCompact {
+  const JpegScanFile* files;
+  const int* byte0;
+  int n;
+  const unsigned* keep;
+  const unsigned* cpos;  // exclusive scan of keep
+  const unsigned* rst;
+  const unsigned* ridx;  // exclusive scan of rst
+  uint8_t* comp;
+  long long* istart;     // [intervals]: compacted start of each interval after the first
+  unsigned* status;
+  GB_HD void operator()(int i) const {
+    const int f = jpeg_find(byte0, n, i);
+    const JpegScanFile& d = files[f];
+    const long long p = d.s0 + (i - byte0[f]);
+    if (keep[i]) comp[cpos[i]] = d.data[p];
+    if (rst[i]) {
+      const unsigned r = ridx[i] - ridx[byte0[f]];
+      if (static_cast<int>(r) + 1 < d.nint && d.data[p + 1] == 0xd0 + (r & 7)) {
+        istart[d.int0 + r + 1] = cpos[i];
+      } else {
+        hd_atomic_or(&status[f], kJpegBadSegment);
+      }
+    }
+  }
+};
+
+// 4.1d: per interval, its bytes and MCUs, and its number of subsequences of S bits; the first interval of
+// a file also checks that the data ends in EOI with one RSTn between each two intervals
+struct JpegIntervals {
+  const JpegScanFile* files;
+  const int* byte0;
+  const int* int0;  // [n + 1]
+  int n;
+  const unsigned* end;
+  const unsigned* cpos;
+  const unsigned* ridx;
+  const long long* istart;
+  int S;
+  JpegInterval* ivs;
+  unsigned* nsub;
+  unsigned* status;
+  GB_HD void operator()(int I) const {
+    const int f = jpeg_find(int0, n, I);
+    const JpegScanFile& d = files[f];
+    const int k = I - d.int0, nb = byte0[f + 1] - byte0[f];
+    const long long e = end[f];
+    const int at_end = static_cast<int>(hd_min(hd_max(e - d.s0, 0LL), static_cast<long long>(nb)));
+    const long long fs = cpos[byte0[f]], fe = cpos[byte0[f] + at_end];
+    long long a = k == 0 ? fs : istart[I];
+    long long b = k == d.nint - 1 ? fe : istart[I + 1];
+    a = hd_min(hd_max(a, fs), fe);
+    b = hd_min(hd_max(b, a), fe);
+    JpegInterval iv;
+    iv.cbyte = a;
+    iv.nbytes = static_cast<int>(b - a);
+    iv.file = f;
+    iv.mcu0 = d.R > 0 ? k * d.R : 0;
+    iv.nmcu = d.R > 0 ? hd_min(d.R, d.mcus - k * d.R) : d.mcus;
+    ivs[I] = iv;
+    const long long bits = 8LL * iv.nbytes;
+    nsub[I] = static_cast<unsigned>(hd_max(1LL, (bits + S - 1) / S));
+    if (k == 0) {
+      const bool eoi = nb > 0 && e + 1 < d.len && d.data[e] == 0xff && d.data[e + 1] == 0xd9;
+      const unsigned rsts = ridx[byte0[f + 1]] - ridx[byte0[f]];
+      if (!eoi || static_cast<int>(rsts) != d.nint - 1) hd_atomic_or(&status[f], kJpegBadSegment);
+    }
+  }
+};
+
+// Decoder state at a subsequence boundary: bit offset in the interval, block slot in the MCU modulo the
+// file's period, zig-zag index in the block (0: the DC symbol is next), and an error mark.
+GB_HD unsigned long long jpeg_state(unsigned pos, int slot, int zz) {
+  return pos | (static_cast<unsigned long long>(slot) << 32) | (static_cast<unsigned long long>(zz) << 40);
+}
+constexpr unsigned long long kJpegStateError = 1ull << 48;
+
+// One DHT table for the decoder: decode_symbol (jpeg_in.cc) on the first 9 bits of a window in `fast`, bit 15
+// set for a symbol with its code length in bits 8..12 and the symbol in bits 0..7, bit 14 set where
+// decode_symbol gives -1 within 9 bits, 0 where it reads on; from there on decode_symbol's own walk over
+// lengths 10 to 16.
+struct JpegHuffDev {
+  uint16_t fast[512];
+  int max_code[18], val_offset[18];
+  int num_symbols;
+  uint8_t symbols[256];
+};
+
+// decode_symbol on the 32 bits w (the first at bit 31): false for -1, else the symbol and its code length
+GB_HD bool jpeg_decode_symbol(const JpegHuffDev& t, unsigned w, int* sym, int* len) {
+  const uint16_t e = t.fast[w >> 23];
+  if (e & 0x8000) {
+    *len = (e >> 8) & 31;
+    *sym = e & 255;
+    return true;
+  }
+  if (e & 0x4000) return false;
+  for (int l = 10; l <= 16; ++l) {
+    const int code = static_cast<int>(w >> (32 - l));
+    if (t.max_code[l] >= 0 && code <= t.max_code[l]) {
+      const int idx = t.val_offset[l] + code;
+      if (idx >= t.num_symbols) return false;
+      *len = l;
+      *sym = t.symbols[idx];
+      return true;
+    }
+  }
+  return false;
+}
+
+// Decodes subsequence bits [start, stop) of one interval from state `in`.  first_pass() for Ss = 0,
+// Se = 63, Al = 0, symbol by symbol: with `coeffs`, blocks b0, b0 + 1, ... are written (DC as the
+// difference) until block `total` is reached, and *end_bit is where that happened; without, only the
+// exit state and the number of blocks completed are computed.  Returns the exit state.
+struct JpegSubDecoder {
+  const JpegScanFile& d;
+  const JpegInterval& iv;
+  const JpegHuffDev* luts;
+  const uint8_t* comp;
+  GB_HD unsigned peek32(unsigned pos) const {
+    const uint8_t* p = comp + iv.cbyte;
+    const unsigned nb = static_cast<unsigned>(iv.nbytes);
+    const unsigned byte = pos >> 3;
+    unsigned long long w = 0;
+    for (unsigned k = 0; k < 5; ++k) w = (w << 8) | (byte + k < nb ? p[byte + k] : 0u);
+    return static_cast<unsigned>((w << (24 + (pos & 7))) >> 32);
+  }
+  GB_HD unsigned long long run(unsigned long long in, unsigned stop, unsigned* blocks, int16_t* coeffs,
+                               const uint8_t* zz_nat, int b0, int total, unsigned* end_bit, bool* bad) const {
+    unsigned pos = static_cast<unsigned>(in);
+    int slot = static_cast<int>((in >> 32) & 0xff), zz = static_cast<int>((in >> 40) & 0xff);
+    const unsigned nbits = 8u * static_cast<unsigned>(iv.nbytes);
+    int b = b0;
+    unsigned done = 0;
+    while (pos < stop) {
+      if (coeffs && b >= total) break;
+      const unsigned w = peek32(pos);
+      int l = 0, sym = 0;
+      if (!jpeg_decode_symbol(luts[zz == 0 ? d.slot_dc[slot] : d.slot_ac[slot]], w, &sym, &l)) goto fail;
+      {
+        const int sz = zz == 0 ? sym : (sym & 15);
+        if (zz == 0 ? sz > 11 : (sz >= 12)) goto fail;
+        const unsigned v = sz ? ((w << l) >> (32 - sz)) : 0u;
+        pos += l + sz;
+        if (pos > nbits) goto fail;
+        const int val = sz ? (v < (1u << (sz - 1)) ? static_cast<int>(v) - (1 << sz) + 1 : static_cast<int>(v)) : 0;
+        bool block_end = false;
+        int16_t* blk = nullptr;
+        if (coeffs) {
+          // the block's own slot: b counts from the interval's start, where slot 0 is
+          const int ts = b % d.nslot, m = iv.mcu0 + b / d.nslot, c = d.slot_comp[ts];
+          const int mx = m % d.mcus_per_row, my = m / d.mcus_per_row;
+          const size_t at = static_cast<size_t>(d.blk0[c]) +
+                            static_cast<size_t>(my * d.comp_v[c] + d.slot_iy[ts]) * d.bw[c] + mx * d.comp_h[c] +
+                            d.slot_ix[ts];
+          blk = coeffs + at * 64;
+        }
+        if (zz == 0) {
+          if (blk) blk[0] = static_cast<int16_t>(val);
+          zz = 1;
+        } else {
+          const int run = sym >> 4;
+          if (sz > 0) {
+            const int k = zz + run;
+            if (k > 63) goto fail;
+            if (blk) blk[zz_nat[k]] = static_cast<int16_t>(val);
+            zz = k + 1;
+          } else if (run == 15) {
+            zz += 16;
+          } else if (run > 0) {
+            goto fail;  // an end-of-block run in a sequential scan
+          } else {
+            block_end = true;
+          }
+          if (zz > 63) block_end = true;
+        }
+        if (block_end) {
+          zz = 0;
+          slot = slot + 1 == d.period ? 0 : slot + 1;
+          ++b;
+          ++done;
+          if (coeffs && b == total) *end_bit = pos;
+        }
+      }
+    }
+    *blocks = done;
+    return jpeg_state(pos, slot, zz);
+  fail:
+    *blocks = done;
+    *bad = true;
+    return jpeg_state(pos, slot, zz) | kJpegStateError;
+  }
+};
+
+// The subsequences of the call: interval I has nsub[I] of them, from sub0[I] on; subsequence j of an
+// interval covers bits [j S, (j + 1) S), the last one up to the interval's end.
+struct JpegSubs {
+  const JpegScanFile* files;
+  const JpegInterval* ivs;
+  int nint;
+  const unsigned* sub0;  // [nint + 1]
+  const JpegHuffDev* luts;
+  const uint8_t* comp;
+  int S;
+  GB_HD bool locate(int t, int* I, int* j, unsigned* stop) const {
+    if (static_cast<unsigned>(t) >= sub0[nint]) return false;
+    *I = jpeg_find(reinterpret_cast<const int*>(sub0), nint, t);
+    *j = t - static_cast<int>(sub0[*I]);
+    const unsigned nbits = 8u * static_cast<unsigned>(ivs[*I].nbytes);
+    const bool last = static_cast<unsigned>(t) + 1 == sub0[*I + 1];
+    *stop = last ? nbits : static_cast<unsigned>(*j + 1) * static_cast<unsigned>(S);
+    return true;
+  }
+};
+
+// 4.2, one round of the speculative decode.  Round 0 decodes every subsequence from the interval's start
+// (its first) or from a guess (an AC symbol of slot 0 at its first bit).  Each later round redoes
+// subsequence j from the exit state subsequence j - 1 had in the round before (a guess again after an
+// error), where that differs from what j started from last time.  States are read from one buffer and
+// written to the other, so a round's result does not depend on the order its invocations run in.  Once a
+// round changes no exit state, every subsequence started from the exact state; that holds file by file,
+// so after the last round the pipeline allows (jpeg_max_sync_rounds), the files whose states still changed are flagged in
+// `status` (null before) and decoded on the host.
+struct JpegHuffSync {
+  JpegSubs subs;
+  int round;
+  const unsigned long long* exit_in;
+  unsigned long long* exit_out;
+  unsigned long long* entry;  // the state each subsequence started from
+  unsigned* count;            // blocks completed in each subsequence
+  unsigned* changed;
+  unsigned* status;
+  GB_HD void operator()(int t) const {
+    int I, j;
+    unsigned stop;
+    if (!subs.locate(t, &I, &j, &stop)) return;
+    const JpegInterval& iv = subs.ivs[I];
+    unsigned long long in = jpeg_state(0, 0, 0);
+    if (j > 0) {
+      in = round == 0 ? kJpegStateError : exit_in[t - 1];
+      if (in & kJpegStateError) in = jpeg_state(static_cast<unsigned>(j) * subs.S, 0, 1);
+    }
+    if (round > 0 && in == entry[t]) {
+      exit_out[t] = exit_in[t];
+      return;
+    }
+    entry[t] = in;
+    const JpegSubDecoder dec{subs.files[iv.file], iv, subs.luts, subs.comp};
+    unsigned blocks = 0, end_bit = 0;
+    bool bad = false;
+    const unsigned long long out = dec.run(in, stop, &blocks, nullptr, nullptr, 0, 0, &end_bit, &bad);
+    exit_out[t] = out;
+    count[t] = blocks;
+    if (round > 0 && out != exit_in[t]) {
+      hd_atomic_or(changed, 1u);
+      if (status) hd_atomic_or(&status[iv.file], kJpegBadSync);
+    }
+  }
+};
+
+// 4.2, the write pass: every subsequence from its exact state writes its blocks' coefficients (DC as the
+// difference); an error in a block the interval needs, an interval that ends early, or one whose last
+// block leaves whole bytes before its RSTn flags the file
+struct JpegHuffWrite {
+  JpegSubs subs;
+  const unsigned long long* entry;
+  const unsigned* bscan;  // exclusive scan of the blocks completed per subsequence
+  const uint8_t* zz_nat;
+  int16_t* coeffs;
+  unsigned* status;
+  GB_HD void operator()(int t) const {
+    int I, j;
+    unsigned stop;
+    if (!subs.locate(t, &I, &j, &stop)) return;
+    const JpegInterval& iv = subs.ivs[I];
+    const JpegScanFile& d = subs.files[iv.file];
+    const int total = iv.nmcu * d.nslot;
+    const int b0 = static_cast<int>(bscan[t] - bscan[subs.sub0[I]]);
+    if (b0 >= total) return;
+    const JpegSubDecoder dec{d, iv, subs.luts, subs.comp};
+    unsigned blocks = 0, end_bit = 0xffffffffu;
+    bool bad = false;
+    dec.run(entry[t], stop, &blocks, coeffs, zz_nat, b0, total, &end_bit, &bad);
+    const bool last_sub = static_cast<unsigned>(t) + 1 == subs.sub0[I + 1];
+    const bool last_interval = I == d.int0 + d.nint - 1;
+    if (end_bit != 0xffffffffu) {
+      // bytes consumed: the next RSTn must follow at once (read_jpeg: "Marker byte (0xff) expected")
+      if (!last_interval && (end_bit + 7) / 8 != static_cast<unsigned>(iv.nbytes)) bad = true;
+    } else if (last_sub && !bad) {
+      bad = true;  // the interval's data ran out before its last block
+    }
+    if (bad) hd_atomic_or(&status[iv.file], kJpegBadCode);
+  }
+};
+
+// DC differences -> values by a prefix sum per (interval, component), in chunks of kJpegDcChunk blocks:
+// block k of a task is the k-th block of that component in the interval's MCUs
+constexpr int kJpegDcChunk = 64;
+struct JpegDcTask {
+  int file, interval, c, nblk;
+};
+GB_HD int16_t* jpeg_dc_block(const JpegScanFile& d, const JpegInterval& iv, int c, int k, int16_t* coeffs) {
+  const int per = d.comp_h[c] * d.comp_v[c];
+  const int m = iv.mcu0 + k / per, w = k % per;
+  const int mx = m % d.mcus_per_row, my = m / d.mcus_per_row;
+  const size_t at = static_cast<size_t>(d.blk0[c]) + static_cast<size_t>(my * d.comp_v[c] + w / d.comp_h[c]) * d.bw[c] +
+                    mx * d.comp_h[c] + w % d.comp_h[c];
+  return coeffs + at * 64;
+}
+struct JpegDcChunkSum {
+  const JpegScanFile* files;
+  const JpegInterval* ivs;
+  const JpegDcTask* tasks;
+  const int* chunk0;  // [ntask + 1]
+  int ntask;
+  int16_t* coeffs;
+  unsigned* sums;
+  GB_HD void operator()(int g) const {
+    const int t = jpeg_find(chunk0, ntask, g);
+    const JpegDcTask& task = tasks[t];
+    const int k0 = (g - chunk0[t]) * kJpegDcChunk, k1 = hd_min(k0 + kJpegDcChunk, task.nblk);
+    unsigned s = 0;
+    for (int k = k0; k < k1; ++k)
+      s += static_cast<unsigned>(static_cast<int>(jpeg_dc_block(files[task.file], ivs[task.interval], task.c, k,
+                                                                coeffs)[0]));
+    sums[g] = s;
+  }
+};
+// every running value checked against int16, as first_pass checks it
+struct JpegDcChunkApply {
+  const JpegScanFile* files;
+  const JpegInterval* ivs;
+  const JpegDcTask* tasks;
+  const int* chunk0;
+  int ntask;
+  int16_t* coeffs;
+  const unsigned* scan;  // exclusive scan of the chunk sums
+  unsigned* status;
+  GB_HD void operator()(int g) const {
+    const int t = jpeg_find(chunk0, ntask, g);
+    const JpegDcTask& task = tasks[t];
+    const int k0 = (g - chunk0[t]) * kJpegDcChunk, k1 = hd_min(k0 + kJpegDcChunk, task.nblk);
+    int v = static_cast<int>(scan[g] - scan[chunk0[t]]);
+    bool bad = false;
+    for (int k = k0; k < k1; ++k) {
+      int16_t* blk = jpeg_dc_block(files[task.file], ivs[task.interval], task.c, k, coeffs);
+      v += blk[0];
+      if (!jpeg_fits16(v)) bad = true;
+      blk[0] = static_cast<int16_t>(v);
+    }
+    if (bad) hd_atomic_or(&status[task.file], kJpegBadCode);
+  }
+};
+
+// 3: libjpeg_decodable's SIMD-range test (jpeg_in.cc) on every block of the files marked in `check`
+struct JpegRangeCheck {
+  const int16_t* coeffs;
+  const int* quant;          // [3 n][64]
+  const JpegDecFile* files;
+  const int* file_blk0;      // [n + 1]
+  int n;
+  const int* check;          // [n]
+  unsigned* status;
+  GB_HD void operator()(int b) const {
+    const int f = jpeg_find(file_blk0, n, b);
+    if (!check[f]) return;
+    const JpegDecFile& d = files[f];
+    const int c = b >= d.blk0[1] ? (b >= d.blk0[2] ? 2 : 1) : 0;
+    const int16_t* blk = coeffs + static_cast<size_t>(b) * 64;
+    const int* q = quant + (3 * f + c) * 64;
+    long long t = 0;
+    for (int k = 0; k < 64; ++k) t += static_cast<long long>(blk[k] < 0 ? -blk[k] : blk[k]) * q[k];
+    if (t > 2040 && !jpeg_islow<true>(blk, q, nullptr, 0)) hd_atomic_or(&status[f], kJpegBadRange);
+  }
+};
+
 // Original image u8 sRGB -> linear float planes (g/butteraugli_comparator.cc:33).
 struct LinearizeRgb {
   const uint8_t* rgb;

@@ -11,6 +11,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <map>
 #include <stdexcept>
 
 #include "block_math.h"
@@ -2672,6 +2673,15 @@ void ImageContext::exclusive_scan_with(const unsigned int* in, unsigned int* out
   }
   *total = acc;
 }
+void exclusive_scan_device(Stream, const unsigned int* in, unsigned int* out, int n, unsigned int*,
+                           unsigned long long* d_total) {
+  unsigned long long acc = 0;
+  for (int i = 0; i < n; ++i) {
+    out[i] = static_cast<unsigned int>(acc);
+    acc += in[i];
+  }
+  *d_total = acc;
+}
 #else
 namespace {
 // 1024 elements per CTA (256 threads x 4): local exclusive scan + CTA total.
@@ -2741,18 +2751,22 @@ __global__ void __launch_bounds__(256) k_scan_add(unsigned int* out, const unsig
 void ImageContext::exclusive_scan(const unsigned int* in, unsigned int* out, int n, unsigned long long* total) {
   exclusive_scan_with(in, out, n, total, j_sums_);
 }
+void exclusive_scan_device(Stream s, const unsigned int* in, unsigned int* out, int n, unsigned int* sums,
+                           unsigned long long* d_total) {
+  const int ctas = (n + 1023) / 1024;
+  note_launch("scan_local", s, n);
+  k_scan_local<<<ctas, 256, 0, s>>>(in, out, sums, n);
+  note_launch_end("scan_local", s);
+  note_launch("scan_sums", s, ctas);
+  k_scan_sums<<<1, 1024, 0, s>>>(sums, ctas, d_total);
+  note_launch_end("scan_sums", s);
+  note_launch("scan_add", s, n);
+  k_scan_add<<<ctas, 256, 0, s>>>(out, sums, n);
+  note_launch_end("scan_add", s);
+}
 // the same without the round trip: the total goes to device memory (8-byte aligned)
 void ImageContext::exclusive_scan_to(const unsigned int* in, unsigned int* out, int n, unsigned long long* d_total) {
-  const int ctas = (n + 1023) / 1024;
-  note_launch("scan_local", s_, n);
-  k_scan_local<<<ctas, 256, 0, s_>>>(in, out, j_sums_, n);
-  note_launch_end("scan_local", s_);
-  note_launch("scan_sums", s_, ctas);
-  k_scan_sums<<<1, 1024, 0, s_>>>(j_sums_, ctas, d_total);
-  note_launch_end("scan_sums", s_);
-  note_launch("scan_add", s_, n);
-  k_scan_add<<<ctas, 256, 0, s_>>>(out, j_sums_, n);
-  note_launch_end("scan_add", s_);
+  exclusive_scan_device(s_, in, out, n, j_sums_, d_total);
 }
 void ImageContext::exclusive_scan_with(const unsigned int* in, unsigned int* out, int n, unsigned long long* total,
                                        unsigned int* j_sums_) {
@@ -2760,15 +2774,7 @@ void ImageContext::exclusive_scan_with(const unsigned int* in, unsigned int* out
   unsigned long long* d_total = reinterpret_cast<unsigned long long*>(j_sums_ + ((ctas + 3) & ~1) + 2);
   // keep the 64-bit total 8-byte aligned inside the scratch buffer
   d_total = reinterpret_cast<unsigned long long*>((reinterpret_cast<uintptr_t>(d_total) + 7) & ~static_cast<uintptr_t>(7));
-  note_launch("scan_local", s_, n);
-  k_scan_local<<<ctas, 256, 0, s_>>>(in, out, j_sums_, n);
-  note_launch_end("scan_local", s_);
-  note_launch("scan_sums", s_, ctas);
-  k_scan_sums<<<1, 1024, 0, s_>>>(j_sums_, ctas, d_total);
-  note_launch_end("scan_sums", s_);
-  note_launch("scan_add", s_, n);
-  k_scan_add<<<ctas, 256, 0, s_>>>(out, j_sums_, n);
-  note_launch_end("scan_add", s_);
+  exclusive_scan_device(s_, in, out, n, j_sums_, d_total);
   d2h(total, d_total, sizeof(unsigned long long), s_);
 }
 #endif
@@ -2980,25 +2986,62 @@ void ImageContext::reset_stats() { profiling_reset(); }
 
 // ---------------------------------------------------------------------------
 // JPEG decode (JpegIdctIslow, JpegUpsampleYccRgb in kernels.h)
-#if !defined(GB200_HOSTSIM)
 namespace {
+#if !defined(GB200_HOSTSIM)
 // JpegUpsampleYccRgb over the call's rows: a warp per row, 8 rows per block (as k_mix_rows)
 template <class F>
 __global__ void __launch_bounds__(256) k_jpeg_rows(F f, int rows) {
   const int row = blockIdx.x * 8 + (threadIdx.x >> 5);
   if (row < rows) f(threadIdx.x & 31, row);
 }
-}  // namespace
 #endif
 
-void jpeg_decode_rgb(const JpegInput* const* files, int n, int device, uint8_t* const* out, bool out_on_device,
-                     Stream stream) {
-  std::vector<JpegDecFile> tab(n);
-  std::vector<int> blk0(n + 1), row0(n + 1), quant(static_cast<size_t>(n) * 3 * 64, 1);
-  long long blocks = 0, rows = 0, out_bytes = 0, pixels = 0;
+// everything a decode acquires is handed back on every path; buffers only once the stream is idle
+struct JpegScope {
+  Stream s = 0;
+  bool have = false;
+  std::vector<void*> bufs;
+  void* alloc(size_t bytes) {
+    bufs.push_back(dev_alloc(bytes));
+    return bufs.back();
+  }
+  template <class T>
+  T* alloc_n(size_t count) {
+    return static_cast<T*>(alloc(sizeof(T) * (count ? count : 1)));
+  }
+  void open(int device) {
+    select_device(device);
+    s = make_stream();
+    have = true;
+  }
+  ~JpegScope() {
+    if (have) {
+      try {
+        stream_sync(s);
+      } catch (...) {
+      }
+      destroy_stream(s);
+    }
+    for (void* p : bufs) dev_free(p);
+  }
+};
+
+// The per-file table and block / row runs of one call (kernels.h, JpegDecFile)
+struct JpegLayout {
+  std::vector<JpegDecFile> tab;
+  std::vector<int> blk0, row0, quant;
+  long long blocks = 0, rows = 0, pixels = 0;
+};
+
+JpegLayout jpeg_layout(const JpegInput* const* files, int n) {
+  JpegLayout L;
+  L.tab.resize(n);
+  L.blk0.resize(n + 1);
+  L.row0.resize(n + 1);
+  L.quant.assign(static_cast<size_t>(n) * 3 * 64, 1);
   for (int i = 0; i < n; ++i) {
     const JpegInput& j = *files[i];
-    JpegDecFile& d = tab[i];
+    JpegDecFile& d = L.tab[i];
     d.w = j.width;
     d.h = j.height;
     d.ncomp = static_cast<int>(j.components.size());
@@ -3007,56 +3050,60 @@ void jpeg_decode_rgb(const JpegInput* const* files, int n, int device, uint8_t* 
     d.vs = j.max_v;
     d.cw = (d.w + d.hs - 1) / d.hs;
     d.ch = (d.h + d.vs - 1) / d.vs;
-    blk0[i] = static_cast<int>(blocks);
+    L.blk0[i] = static_cast<int>(L.blocks);
     for (int c = 0; c < 4; ++c) {
-      d.blk0[c] = static_cast<int>(blocks);
+      d.blk0[c] = static_cast<int>(L.blocks);
       if (c >= d.ncomp) continue;
       const JpegComponent& comp = j.components[c];
       d.bw[c] = comp.width_in_blocks;
-      memcpy(&quant[(3 * i + c) * 64], j.quant[comp.quant_idx].values, 64 * sizeof(int));
-      blocks += static_cast<long long>(comp.width_in_blocks) * comp.height_in_blocks;
+      memcpy(&L.quant[(3 * i + c) * 64], j.quant[comp.quant_idx].values, 64 * sizeof(int));
+      L.blocks += static_cast<long long>(comp.width_in_blocks) * comp.height_in_blocks;
     }
-    d.row0 = static_cast<int>(rows);
-    rows += d.h;
+    d.row0 = static_cast<int>(L.rows);
+    L.rows += d.h;
     d.out = nullptr;
-    pixels += static_cast<long long>(d.w) * d.h;
-    if (blocks > (1LL << 30) || rows > (1LL << 30))
+    L.pixels += static_cast<long long>(d.w) * d.h;
+    if (L.blocks > (1LL << 30) || L.rows > (1LL << 30))
       throw std::runtime_error("jpeg_decode_rgb: more than 2^30 blocks or rows in one call");
   }
-  blk0[n] = static_cast<int>(blocks);
-  row0[n] = static_cast<int>(rows);
-  for (int i = 0; i < n; ++i) row0[i] = tab[i].row0;
-  out_bytes = 3 * pixels;
-  std::vector<int16_t> coeffs(static_cast<size_t>(blocks) * 64);
+  L.blk0[n] = static_cast<int>(L.blocks);
+  L.row0[n] = static_cast<int>(L.rows);
+  for (int i = 0; i < n; ++i) L.row0[i] = L.tab[i].row0;
+  return L;
+}
+
+// The tail both entries share: the IDCT of every block of the call, then upsampling and colour conversion
+// of every row into the files' outputs
+void jpeg_idct_upsample(Stream s, const JpegDecFile* d_tab, const int* d_blk0, const int* d_row0, const int* d_quant,
+                        const int16_t* d_coeffs, uint8_t* d_samples, int n, const JpegLayout& L) {
+  launch_1d(s, JpegIdctIslow{d_coeffs, d_quant, d_tab, d_blk0, n, d_samples}, static_cast<int>(L.blocks),
+            "jpeg_idct_islow");
+  JpegUpsampleYccRgb up{d_tab, d_row0, n, d_samples, 1};
+#if defined(GB200_HOSTSIM)
+  launch_2d(s, up, 1, static_cast<int>(L.rows));
+#else
+  up.lanes = 32;
+  note_launch("jpeg_upsample_ycc_rgb", s, static_cast<double>(L.pixels));
+  k_jpeg_rows<<<cdiv(static_cast<int>(L.rows), 8), 256, 0, s>>>(up, static_cast<int>(L.rows));
+  note_launch_end("jpeg_upsample_ycc_rgb", s);
+#endif
+}
+}  // namespace
+
+void jpeg_decode_rgb(const JpegInput* const* files, int n, int device, uint8_t* const* out, bool out_on_device,
+                     Stream stream) {
+  JpegLayout L = jpeg_layout(files, n);
+  std::vector<JpegDecFile>& tab = L.tab;
+  const long long out_bytes = 3 * L.pixels;
+  std::vector<int16_t> coeffs(static_cast<size_t>(L.blocks) * 64);
   for (int i = 0; i < n; ++i)
     for (int c = 0; c < tab[i].ncomp; ++c) {
       const std::vector<int16_t>& v = files[i]->components[c].coeffs;
       memcpy(&coeffs[static_cast<size_t>(tab[i].blk0[c]) * 64], v.data(), v.size() * sizeof(int16_t));
     }
 
-  // everything acquired is handed back on every path; buffers only once the stream is idle
-  struct Scope {
-    Stream s = 0;
-    bool have = false;
-    std::vector<void*> bufs;
-    void* alloc(size_t bytes) {
-      bufs.push_back(dev_alloc(bytes));
-      return bufs.back();
-    }
-    ~Scope() {
-      if (have) {
-        try {
-          stream_sync(s);
-        } catch (...) {
-        }
-        destroy_stream(s);
-      }
-      for (void* p : bufs) dev_free(p);
-    }
-  } sc;
-  select_device(device);
-  sc.s = make_stream();
-  sc.have = true;
+  JpegScope sc;
+  sc.open(device);
   const Stream s = sc.s;
   uint8_t* staged = nullptr;
   if (out_on_device) {
@@ -3072,29 +3119,469 @@ void jpeg_decode_rgb(const JpegInput* const* files, int n, int device, uint8_t* 
   JpegDecFile* d_tab = static_cast<JpegDecFile*>(sc.alloc(sizeof(JpegDecFile) * n));
   int* d_blk0 = static_cast<int*>(sc.alloc(sizeof(int) * (n + 1)));
   int* d_row0 = static_cast<int*>(sc.alloc(sizeof(int) * (n + 1)));
-  int* d_quant = static_cast<int*>(sc.alloc(sizeof(int) * quant.size()));
+  int* d_quant = static_cast<int*>(sc.alloc(sizeof(int) * L.quant.size()));
   int16_t* d_coeffs = static_cast<int16_t*>(sc.alloc(sizeof(int16_t) * coeffs.size()));
-  uint8_t* d_samples = static_cast<uint8_t*>(sc.alloc(static_cast<size_t>(blocks) * 64));
+  uint8_t* d_samples = static_cast<uint8_t*>(sc.alloc(static_cast<size_t>(L.blocks) * 64));
   h2d(d_tab, tab.data(), sizeof(JpegDecFile) * n, s);
-  h2d(d_blk0, blk0.data(), sizeof(int) * (n + 1), s);
-  h2d(d_row0, row0.data(), sizeof(int) * (n + 1), s);
-  h2d(d_quant, quant.data(), sizeof(int) * quant.size(), s);
+  h2d(d_blk0, L.blk0.data(), sizeof(int) * (n + 1), s);
+  h2d(d_row0, L.row0.data(), sizeof(int) * (n + 1), s);
+  h2d(d_quant, L.quant.data(), sizeof(int) * L.quant.size(), s);
   h2d(d_coeffs, coeffs.data(), sizeof(int16_t) * coeffs.size(), s);
   if (out_on_device) stream_wait(s, stream);
-  launch_1d(s, JpegIdctIslow{d_coeffs, d_quant, d_tab, d_blk0, n, d_samples}, static_cast<int>(blocks),
-            "jpeg_idct_islow");
-  JpegUpsampleYccRgb up{d_tab, d_row0, n, d_samples, 1};
-#if defined(GB200_HOSTSIM)
-  launch_2d(s, up, 1, static_cast<int>(rows));
-#else
-  up.lanes = 32;
-  note_launch("jpeg_upsample_ycc_rgb", s, static_cast<double>(pixels));
-  k_jpeg_rows<<<cdiv(static_cast<int>(rows), 8), 256, 0, s>>>(up, static_cast<int>(rows));
-  note_launch_end("jpeg_upsample_ycc_rgb", s);
-#endif
+  jpeg_idct_upsample(s, d_tab, d_blk0, d_row0, d_quant, d_coeffs, d_samples, n, L);
   if (!out_on_device)
     for (int i = 0; i < n; ++i) d2h(out[i], tab[i].out, static_cast<size_t>(3) * tab[i].w * tab[i].h, s);
   stream_sync(s);
+}
+
+// ---------------------------------------------------------------------------
+// JPEG entropy decoding on the device (JpegSegEnd .. JpegDcChunkApply in kernels.h)
+namespace {
+
+// Files the device path takes are shorter than this: bit positions in a restart interval stay below 2^31.
+constexpr size_t kJpegMaxDeviceBytes = size_t(1) << 28;
+// Synchronisation rounds after the first: an exact state moves on by at least one subsequence per round,
+// so the bound covers 64 subsequences or 2^16 bits, whichever is more; files whose states still change
+// then are decoded on the host.
+int jpeg_max_sync_rounds(int S) { return std::max(64, 65536 / S); }
+// What the device files of one call may add up to (scan bytes, subsequences, DC chunks); files beyond it
+// are decoded on the host.  Keeps every flat index of jpeg_entropy_decode below 2^31.
+constexpr long long kJpegCallBudget = 1LL << 30;
+
+// The shape the device path takes: a file shorter than kJpegMaxDeviceBytes with a sequential 8-bit frame
+// (read_jpeg_header checked the precision) of one component, or of three in a sampling libjpeg_decodable
+// accepts, whose first scan carries every component with Ss = 0, Se = 63, Ah = Al = 0
+bool jpeg_device_shape(const JpegScanHeader& h, size_t len) {
+  if (len >= kJpegMaxDeviceBytes) return false;
+  const JpegInput& j = h.jpg;
+  const int n = static_cast<int>(j.components.size());
+  std::string why;
+  if (j.progressive || !libjpeg_decodable(j, &why)) return false;  // no coefficients: the layout checks only
+  const JpegScanSpec& sp = h.scan;
+  if (sp.ncomp != n || sp.ss != 0 || sp.se != 63 || sp.ah != 0 || sp.al != 0) return false;
+  int slots = 0;
+  for (const JpegComponent& c : j.components) slots += n > 1 ? c.h_samp * c.v_samp : 1;
+  return slots <= kJpegMaxSlots;
+}
+
+// MCUs of the first scan, as scan() (jpeg_in.cc) counts them
+void jpeg_scan_mcus(const JpegScanHeader& h, int* mcus_per_row, int* mcus) {
+  const JpegInput& j = h.jpg;
+  *mcus_per_row = j.mcu_cols;
+  int mcu_rows = j.mcu_rows;
+  if (h.scan.ncomp == 1) {
+    const JpegComponent& c = j.components[h.scan.comp[0]];
+    *mcus_per_row = (j.width * c.h_samp + 8 * j.max_h - 1) / (8 * j.max_h);
+    mcu_rows = (j.height * c.v_samp + 8 * j.max_v - 1) / (8 * j.max_v);
+  }
+  *mcus = *mcus_per_row * mcu_rows;
+}
+
+// Upper bounds of what one file adds to jpeg_entropy_decode's flat ranges: scan bytes, subsequences, DC chunks
+void jpeg_device_cost(const JpegScanHeader& h, size_t len, int S, long long cost[3]) {
+  int mpr = 0, mcus = 0;
+  jpeg_scan_mcus(h, &mpr, &mcus);
+  const int R = h.restart_interval;
+  const long long nint = R > 0 ? (mcus + R - 1) / R : 1;
+  long long per_mcu = 0;
+  for (int si = 0; si < h.scan.ncomp; ++si) {
+    const JpegComponent& c = h.jpg.components[h.scan.comp[si]];
+    per_mcu += h.scan.ncomp > 1 ? c.h_samp * c.v_samp : 1;
+  }
+  cost[0] = std::max(0LL, static_cast<long long>(len) - 2 - static_cast<long long>(h.scan_start));
+  cost[1] = (8 * cost[0] + S - 1) / S + nint;
+  cost[2] = nint * h.scan.ncomp + mcus * per_mcu / kJpegDcChunk + 1;
+}
+
+// The decoder's copy of a DHT table (JpegHuffDev, kernels.h): decode_symbol over the first 9 bits in `fast`
+void jpeg_build_huff(const JpegHuffTable& t, JpegHuffDev* o) {
+  memset(o, 0, sizeof(*o));
+  memcpy(o->max_code, t.max_code, sizeof(o->max_code));
+  memcpy(o->val_offset, t.val_offset, sizeof(o->val_offset));
+  memcpy(o->symbols, t.symbols, sizeof(o->symbols));
+  o->num_symbols = t.num_symbols;
+  for (int w = 0; w < 512; ++w) {
+    uint16_t e = 0;
+    for (int l = 1; l <= 9; ++l) {
+      const int code = w >> (9 - l);
+      if (t.max_code[l] >= 0 && code <= t.max_code[l]) {
+        const int idx = t.val_offset[l] + code;
+        e = idx < t.num_symbols ? static_cast<uint16_t>(0x8000 | (l << 8) | t.symbols[idx]) : 0x4000;
+        break;
+      }
+    }
+    o->fast[w] = e;
+  }
+}
+
+struct JpegDeviceFile {
+  const uint8_t* data;  // device memory
+  size_t len;
+  const JpegScanHeader* hdr;
+  const JpegDecFile* layout;  // blk0 of each component
+};
+
+// Entropy-decodes the files into d_coeffs (zeroed, laid out as `layout` says) on s; d_status[i] receives
+// the kJpegBad* flags of file i.  Returns the number of synchronisation rounds after the first.
+int jpeg_entropy_decode(const std::vector<JpegDeviceFile>& fs, int16_t* d_coeffs, int S, Stream s, JpegScope* sc,
+                        unsigned* d_status) {
+  const int n = static_cast<int>(fs.size());
+  if (n == 0) return 0;
+  if (S < 8) throw std::runtime_error("jpeg entropy decode: subsequences of fewer than 8 bits");
+  std::vector<JpegScanFile> tab(n);
+  std::vector<int> byte0(n + 1), int0(n + 1);
+  std::vector<unsigned> end(n);
+  std::map<std::string, int> lut_ids;
+  std::vector<JpegHuffDev> luts;
+  std::vector<JpegDcTask> tasks;
+  std::vector<int> chunk0;
+  long long bytes = 0, intervals = 0, subs = 0, chunks = 0;
+  auto lut = [&](const JpegHuffTable& t) {
+    std::string key(reinterpret_cast<const char*>(t.max_code), sizeof(t.max_code));
+    key.append(reinterpret_cast<const char*>(t.val_offset), sizeof(t.val_offset));
+    key.append(reinterpret_cast<const char*>(t.symbols), t.num_symbols);
+    key.append(1, static_cast<char>(t.num_symbols & 255)).append(1, static_cast<char>(t.num_symbols >> 8));
+    auto it = lut_ids.find(key);
+    if (it != lut_ids.end()) return it->second;
+    const int id = static_cast<int>(lut_ids.size());
+    lut_ids[key] = id;
+    luts.resize(luts.size() + 1);
+    jpeg_build_huff(t, &luts.back());
+    return id;
+  };
+  for (int i = 0; i < n; ++i) {
+    const JpegScanHeader& h = *fs[i].hdr;
+    const JpegInput& j = h.jpg;
+    JpegScanFile& d = tab[i];
+    memset(&d, 0, sizeof(d));
+    d.data = fs[i].data;
+    d.len = static_cast<long long>(fs[i].len);
+    d.s0 = static_cast<int>(h.scan_start);
+    const long long nb = std::max(0LL, d.len - 2 - d.s0);
+    byte0[i] = static_cast<int>(bytes);
+    bytes += nb;
+    end[i] = static_cast<unsigned>(d.len >= 2 ? d.len - 2 : 0);
+    const bool inter = h.scan.ncomp > 1;
+    jpeg_scan_mcus(h, &d.mcus_per_row, &d.mcus);
+    d.R = h.restart_interval;
+    d.nint = d.R > 0 ? (d.mcus + d.R - 1) / d.R : 1;
+    d.int0 = static_cast<int>(intervals);
+    int0[i] = d.int0;
+    for (int si = 0; si < h.scan.ncomp; ++si) {
+      const int c = h.scan.comp[si];
+      const JpegComponent& comp = j.components[c];
+      d.comp_h[c] = inter ? comp.h_samp : 1;
+      d.comp_v[c] = inter ? comp.v_samp : 1;
+      d.bw[c] = comp.width_in_blocks;
+      d.blk0[c] = fs[i].layout->blk0[c];
+      const int dc = lut(h.dc[h.scan.dc_tbl[si]]), ac = lut(h.ac[h.scan.ac_tbl[si]]);
+      for (int iy = 0; iy < d.comp_v[c]; ++iy)
+        for (int ix = 0; ix < d.comp_h[c]; ++ix) {
+          d.slot_comp[d.nslot] = c;
+          d.slot_ix[d.nslot] = ix;
+          d.slot_iy[d.nslot] = iy;
+          d.slot_dc[d.nslot] = dc;
+          d.slot_ac[d.nslot] = ac;
+          ++d.nslot;
+        }
+    }
+    for (d.period = 1; d.period < d.nslot; ++d.period) {
+      if (d.nslot % d.period) continue;
+      bool same = true;
+      for (int k = d.period; k < d.nslot && same; ++k)
+        same = d.slot_dc[k] == d.slot_dc[k % d.period] && d.slot_ac[k] == d.slot_ac[k % d.period];
+      if (same) break;
+    }
+    for (int k = 0; k < d.nint; ++k) {
+      const int nmcu = d.R > 0 ? std::min(d.R, d.mcus - k * d.R) : d.mcus;
+      for (int si = 0; si < h.scan.ncomp; ++si) {
+        const int c = h.scan.comp[si];
+        JpegDcTask t{i, d.int0 + k, c, nmcu * d.comp_h[c] * d.comp_v[c]};
+        tasks.push_back(t);
+        chunk0.push_back(static_cast<int>(chunks));
+        chunks += (t.nblk + kJpegDcChunk - 1) / kJpegDcChunk;
+      }
+    }
+    intervals += d.nint;
+    subs += (8 * nb + S - 1) / S + d.nint;
+  }
+  byte0[n] = static_cast<int>(bytes);
+  int0[n] = static_cast<int>(intervals);
+  chunk0.push_back(static_cast<int>(chunks));
+  if (bytes >= (1LL << 31) - 1 || subs >= (1LL << 31) - 1 || chunks >= (1LL << 31) - 1)
+    throw std::runtime_error("jpeg entropy decode: more than 2^31 scan bytes or subsequences in one call");
+  // (the entries keep their device files within kJpegCallBudget and kJpegMaxDeviceBytes, far below that)
+  const int B = static_cast<int>(bytes), NI = static_cast<int>(intervals), U = static_cast<int>(subs);
+  const int NT = static_cast<int>(tasks.size()), NC = static_cast<int>(chunks);
+
+  const int scan_max = std::max(std::max(B, U), std::max(NI, NC)) + 1;
+  unsigned* sums = sc->alloc_n<unsigned>((scan_max + 1023) / 1024 + 2);
+  unsigned long long* d_total = sc->alloc_n<unsigned long long>(1);
+  JpegScanFile* d_tab = sc->alloc_n<JpegScanFile>(n);
+  int* d_byte0 = sc->alloc_n<int>(n + 1);
+  int* d_int0 = sc->alloc_n<int>(n + 1);
+  unsigned* d_end = sc->alloc_n<unsigned>(n);
+  JpegHuffDev* d_luts = sc->alloc_n<JpegHuffDev>(luts.size());
+  uint8_t* d_zz = sc->alloc_n<uint8_t>(64);
+  unsigned* keep = sc->alloc_n<unsigned>(B + 1);
+  unsigned* rst = sc->alloc_n<unsigned>(B + 1);
+  unsigned* cpos = sc->alloc_n<unsigned>(B + 1);
+  unsigned* ridx = sc->alloc_n<unsigned>(B + 1);
+  uint8_t* comp = sc->alloc_n<uint8_t>(B);
+  long long* istart = sc->alloc_n<long long>(NI);
+  JpegInterval* ivs = sc->alloc_n<JpegInterval>(NI);
+  unsigned* nsub = sc->alloc_n<unsigned>(NI + 1);
+  unsigned* sub0 = sc->alloc_n<unsigned>(NI + 1);
+  unsigned long long* exit_a = sc->alloc_n<unsigned long long>(U);
+  unsigned long long* exit_b = sc->alloc_n<unsigned long long>(U);
+  unsigned long long* entry = sc->alloc_n<unsigned long long>(U);
+  unsigned* count = sc->alloc_n<unsigned>(U + 1);
+  unsigned* bscan = sc->alloc_n<unsigned>(U + 1);
+  unsigned* changed = sc->alloc_n<unsigned>(1);
+  JpegDcTask* d_tasks = sc->alloc_n<JpegDcTask>(NT);
+  int* d_chunk0 = sc->alloc_n<int>(NT + 1);
+  unsigned* csum = sc->alloc_n<unsigned>(NC + 1);
+  unsigned* cscan = sc->alloc_n<unsigned>(NC + 1);
+  uint8_t zz[64];
+  for (int k = 0; k < 64; ++k) zz[k] = static_cast<uint8_t>(zigzag_to_natural()[k]);
+  h2d(d_tab, tab.data(), sizeof(JpegScanFile) * n, s);
+  h2d(d_byte0, byte0.data(), sizeof(int) * (n + 1), s);
+  h2d(d_int0, int0.data(), sizeof(int) * (n + 1), s);
+  h2d(d_end, end.data(), sizeof(unsigned) * n, s);
+  h2d(d_luts, luts.data(), sizeof(JpegHuffDev) * luts.size(), s);
+  h2d(d_zz, zz, 64, s);
+  h2d(d_tasks, tasks.data(), sizeof(JpegDcTask) * NT, s);
+  h2d(d_chunk0, chunk0.data(), sizeof(int) * (NT + 1), s);
+  dev_zero(keep + B, sizeof(unsigned), s);
+  dev_zero(rst + B, sizeof(unsigned), s);
+  dev_zero(istart, sizeof(long long) * std::max(NI, 1), s);
+  dev_zero(nsub + NI, sizeof(unsigned), s);
+  dev_zero(count, sizeof(unsigned) * (U + 1), s);
+  dev_zero(csum + NC, sizeof(unsigned), s);
+
+  // 4.1: segment pass
+  launch_1d(s, JpegSegEnd{d_tab, d_byte0, n, d_end}, B, "jpeg_seg_end");
+  launch_1d(s, JpegSegFlags{d_tab, d_byte0, n, d_end, keep, rst}, B, "jpeg_seg_flags");
+  exclusive_scan_device(s, keep, cpos, B + 1, sums, d_total);
+  exclusive_scan_device(s, rst, ridx, B + 1, sums, d_total);
+  launch_1d(s, JpegSegCompact{d_tab, d_byte0, n, keep, cpos, rst, ridx, comp, istart, d_status}, B, "jpeg_seg_compact");
+  launch_1d(s, JpegIntervals{d_tab, d_byte0, d_int0, n, d_end, cpos, ridx, istart, S, ivs, nsub, d_status}, NI,
+            "jpeg_intervals");
+  exclusive_scan_device(s, nsub, sub0, NI + 1, sums, d_total);
+
+  // 4.2: speculative decode, synchronised until no exit state changes, or for jpeg_max_sync_rounds(S) rounds,
+  // the last of which flags the files that have not converged (kJpegBadSync)
+  const JpegSubs subsq{d_tab, ivs, NI, sub0, d_luts, comp, S};
+  launch_1d(s, JpegHuffSync{subsq, 0, exit_b, exit_a, entry, count, changed, nullptr}, U, "jpeg_huff_sync");
+  int rounds = 0;
+  for (;;) {
+    ++rounds;
+    const bool last = rounds == jpeg_max_sync_rounds(S);
+    dev_zero(changed, sizeof(unsigned), s);
+    launch_1d(s, JpegHuffSync{subsq, rounds, exit_a, exit_b, entry, count, changed, last ? d_status : nullptr}, U,
+              "jpeg_huff_sync");
+    std::swap(exit_a, exit_b);
+    unsigned h_changed = 0;
+    d2h(&h_changed, changed, sizeof(unsigned), s);
+    if (!h_changed || last) break;
+  }
+  exclusive_scan_device(s, count, bscan, U + 1, sums, d_total);
+  launch_1d(s, JpegHuffWrite{subsq, entry, bscan, d_zz, d_coeffs, d_status}, U, "jpeg_huff_write");
+  launch_1d(s, JpegDcChunkSum{d_tab, ivs, d_tasks, d_chunk0, NT, d_coeffs, csum}, NC, "jpeg_dc_sum");
+  exclusive_scan_device(s, csum, cscan, NC + 1, sums, d_total);
+  launch_1d(s, JpegDcChunkApply{d_tab, ivs, d_tasks, d_chunk0, NT, d_coeffs, cscan, d_status}, NC, "jpeg_dc_apply");
+  return rounds;
+}
+
+std::string jpeg_file_reason(const std::string& who, int i, const std::string& why) {
+  return who + ": file " + std::to_string(i) + ": " + why;
+}
+
+// The host path of one file: read_jpeg and the checks of gb200_jpeg_decode_rgb, then the output size;
+// "" where the file is accepted
+std::string jpeg_host_check(const std::vector<uint8_t>& b, int width, int height, JpegInput* jpg) {
+  std::string why;
+  if (!read_jpeg(b.data(), b.size(), jpg, &why)) return why;
+  int w = 0, h = 0;
+  if (!read_jpeg_dimensions(b.data(), b.size(), &w, &h) || w != jpg->width || h != jpg->height)
+    return "the frame size differs from what gb200_jpeg_dimensions reads";
+  if (width != jpg->width || height != jpg->height)
+    return "the output is " + std::to_string(width) + "x" + std::to_string(height) + ", the frame " +
+           std::to_string(jpg->width) + "x" + std::to_string(jpg->height);
+  if (!libjpeg_decodable(*jpg, &why)) return why;
+  return "";
+}
+
+constexpr size_t kJpegFirstPrefix = 4096;
+}  // namespace
+
+void jpeg_dimensions_from_device(const uint8_t* const* jpeg, const size_t* len, int n, int device, Stream stream,
+                                 int* width, int* height) {
+  JpegScope sc;
+  sc.open(device);
+  stream_wait(sc.s, stream);
+  std::vector<uint8_t> b;
+  for (int i = 0; i < n; ++i) {
+    width[i] = height[i] = 0;
+    for (size_t m = std::min(kJpegFirstPrefix, len[i]);; m = std::min(2 * m, len[i])) {
+      b.resize(m);
+      if (m) d2h(b.data(), jpeg[i], m, sc.s);
+      int w = 0, h = 0;
+      if (read_jpeg_dimensions(b.data(), m, &w, &h)) {
+        width[i] = w;
+        height[i] = h;
+        break;
+      }
+      if (m == len[i]) break;
+    }
+  }
+}
+
+void jpeg_decode_rgb_from_device(const char* who, const uint8_t* const* jpeg, const size_t* len, int n, int device,
+                                 const int* width, const int* height, uint8_t* const* out, Stream stream) {
+  JpegScope sc;
+  sc.open(device);
+  const Stream s = sc.s;
+  stream_wait(s, stream);
+  // headers, from prefixes of 4 KiB doubling; each round covers every file still short of its first SOS
+  std::vector<JpegScanHeader> hdr(n);
+  std::vector<std::vector<uint8_t> > pre(n);
+  std::vector<char> head_ok(n, 0), pending(n, 1);
+  for (size_t m = kJpegFirstPrefix;; m *= 2) {
+    bool more = false;
+    for (int i = 0; i < n; ++i) {
+      if (!pending[i]) continue;
+      const size_t k = std::min(m, len[i]);
+      pre[i].resize(k);
+      if (k) d2h(pre[i].data(), jpeg[i], k, s);
+      if (read_jpeg_header(pre[i].data(), k, &hdr[i])) {
+        head_ok[i] = 1;
+        pending[i] = 0;
+      } else if (k == len[i]) {
+        pending[i] = 0;
+      } else {
+        more = true;
+      }
+    }
+    if (!more) break;
+  }
+  std::vector<char> dev(n, 0);
+  std::vector<std::string> why(n);
+  std::vector<JpegInput> host(n);
+  std::vector<char> host_ok(n, 0);
+  auto host_path = [&](int i) {
+    std::vector<uint8_t> b(len[i]);
+    if (len[i]) d2h(b.data(), jpeg[i], len[i], s);
+    why[i] = jpeg_host_check(b, width[i], height[i], &host[i]);
+    host_ok[i] = why[i].empty();
+  };
+  long long budget[3] = {0, 0, 0};
+  for (int i = 0; i < n; ++i) {
+    int w = 0, h = 0;
+    dev[i] = head_ok[i] && jpeg_device_shape(hdr[i], len[i]) &&
+             read_jpeg_dimensions(pre[i].data(), pre[i].size(), &w, &h) && w == hdr[i].jpg.width &&
+             h == hdr[i].jpg.height;
+    if (dev[i]) {
+      long long cost[3];
+      jpeg_device_cost(hdr[i], len[i], kJpegSubBits, cost);
+      for (int k = 0; k < 3; ++k) dev[i] = dev[i] && budget[k] + cost[k] < kJpegCallBudget;
+      if (dev[i])
+        for (int k = 0; k < 3; ++k) budget[k] += cost[k];
+    }
+    if (!dev[i]) host_path(i);
+  }
+  static const JpegInput kEmpty;
+  std::vector<const JpegInput*> lay(n);
+  for (int i = 0; i < n; ++i) lay[i] = dev[i] ? &hdr[i].jpg : (host_ok[i] ? &host[i] : &kEmpty);
+  JpegLayout L = jpeg_layout(lay.data(), n);
+  std::vector<int> check(n);
+  std::vector<JpegDeviceFile> fs;
+  for (int i = 0; i < n; ++i) {
+    check[i] = dev[i];
+    if (check[i]) fs.push_back(JpegDeviceFile{jpeg[i], len[i], &hdr[i], &L.tab[i]});
+  }
+  for (int i = 0; i < n; ++i) L.tab[i].out = out[i];
+  JpegDecFile* d_tab = sc.alloc_n<JpegDecFile>(n);
+  int* d_blk0 = sc.alloc_n<int>(n + 1);
+  int* d_row0 = sc.alloc_n<int>(n + 1);
+  int* d_quant = sc.alloc_n<int>(L.quant.size());
+  int* d_check = sc.alloc_n<int>(n);
+  unsigned* d_status = sc.alloc_n<unsigned>(n);
+  int16_t* d_coeffs = sc.alloc_n<int16_t>(static_cast<size_t>(L.blocks) * 64);
+  h2d(d_tab, L.tab.data(), sizeof(JpegDecFile) * n, s);
+  h2d(d_blk0, L.blk0.data(), sizeof(int) * (n + 1), s);
+  h2d(d_row0, L.row0.data(), sizeof(int) * (n + 1), s);
+  h2d(d_quant, L.quant.data(), sizeof(int) * L.quant.size(), s);
+  h2d(d_check, check.data(), sizeof(int) * n, s);
+  if (!fs.empty()) {
+    dev_zero(d_coeffs, sizeof(int16_t) * 64 * static_cast<size_t>(L.blocks), s);
+    // the status words of the device files, in call order
+    unsigned* st = sc.alloc_n<unsigned>(fs.size());
+    dev_zero(st, sizeof(unsigned) * fs.size(), s);
+    jpeg_entropy_decode(fs, d_coeffs, kJpegSubBits, s, &sc, st);
+    std::vector<unsigned> zeros(n, 0);
+    h2d(d_status, zeros.data(), sizeof(unsigned) * n, s);
+    std::vector<unsigned> hs(fs.size());
+    // scatter the per-device-file words to call order through the host: one small copy each way
+    d2h(hs.data(), st, sizeof(unsigned) * fs.size(), s);
+    launch_1d(s, JpegRangeCheck{d_coeffs, d_quant, d_tab, d_blk0, n, d_check, d_status}, static_cast<int>(L.blocks),
+              "jpeg_range_check");
+    std::vector<unsigned> range(n);
+    d2h(range.data(), d_status, sizeof(unsigned) * n, s);
+    for (int i = 0, k = 0; i < n; ++i) {
+      if (!check[i]) continue;
+      const unsigned flags = hs[k++] | range[i];
+      if (flags) {
+        // read_jpeg decides, with its own reasons in the host entry's order (the output size among them)
+        host_path(i);
+        if (host_ok[i]) {
+          for (size_t c = 0; c < host[i].components.size(); ++c) {
+            const std::vector<int16_t>& v = host[i].components[c].coeffs;
+            h2d(d_coeffs + static_cast<size_t>(L.tab[i].blk0[c]) * 64, v.data(), v.size() * sizeof(int16_t), s);
+          }
+        }
+      } else if (width[i] != hdr[i].jpg.width || height[i] != hdr[i].jpg.height) {
+        // read_jpeg accepts the file, so the size is the first reason jpeg_host_check would give
+        why[i] = "the output is " + std::to_string(width[i]) + "x" + std::to_string(height[i]) + ", the frame " +
+                 std::to_string(hdr[i].jpg.width) + "x" + std::to_string(hdr[i].jpg.height);
+      }
+    }
+  }
+  for (int i = 0; i < n; ++i)
+    if (!why[i].empty()) throw std::runtime_error(jpeg_file_reason(who, i, why[i]));
+  for (int i = 0; i < n; ++i)
+    if (!dev[i])
+      for (size_t c = 0; c < host[i].components.size(); ++c) {
+        const std::vector<int16_t>& v = host[i].components[c].coeffs;
+        h2d(d_coeffs + static_cast<size_t>(L.tab[i].blk0[c]) * 64, v.data(), v.size() * sizeof(int16_t), s);
+      }
+  uint8_t* d_samples = sc.alloc_n<uint8_t>(static_cast<size_t>(L.blocks) * 64);
+  jpeg_idct_upsample(s, d_tab, d_blk0, d_row0, d_quant, d_coeffs, d_samples, n, L);
+  stream_sync(s);
+}
+
+bool jpeg_debug_entropy_decode(const uint8_t* data, size_t len, int S, std::vector<int16_t>* coeffs) {
+  JpegScanHeader hdr;
+  if (!read_jpeg_header(data, len, &hdr) || !jpeg_device_shape(hdr, len)) return false;
+  const JpegInput* one = &hdr.jpg;
+  JpegLayout L = jpeg_layout(&one, 1);
+  JpegScope sc;
+  sc.open(0);
+  const Stream s = sc.s;
+  uint8_t* d_data = sc.alloc_n<uint8_t>(len);
+  h2d(d_data, data, len, s);
+  int16_t* d_coeffs = sc.alloc_n<int16_t>(static_cast<size_t>(L.blocks) * 64);
+  unsigned* d_status = sc.alloc_n<unsigned>(1);
+  dev_zero(d_coeffs, sizeof(int16_t) * 64 * static_cast<size_t>(L.blocks), s);
+  dev_zero(d_status, sizeof(unsigned), s);
+  std::vector<JpegDeviceFile> fs{JpegDeviceFile{d_data, len, &hdr, &L.tab[0]}};
+  jpeg_entropy_decode(fs, d_coeffs, S, s, &sc, d_status);
+  unsigned status = 0;
+  d2h(&status, d_status, sizeof(unsigned), s);
+  if (status) return false;
+  coeffs->resize(static_cast<size_t>(L.blocks) * 64);
+  d2h(coeffs->data(), d_coeffs, sizeof(int16_t) * coeffs->size(), s);
+  return true;
 }
 
 }  // namespace gb200

@@ -25,6 +25,32 @@ struct JpegInput;
 void jpeg_decode_rgb(const JpegInput* const* files, int n, int device, uint8_t* const* out, bool out_on_device,
                      Stream stream);
 
+// Subsequence length, in bits, of the speculative Huffman decode (JpegHuffSync in kernels.h).
+constexpr int kJpegSubBits = 1024;
+
+// Frame size of n files in memory of `device`, read from prefixes copied to the host (4 KiB, doubling) after
+// the work queued on `stream`; 0 x 0 where no frame size can be read.
+void jpeg_dimensions_from_device(const uint8_t* const* jpeg, const size_t* len, int n, int device, Stream stream,
+                                 int* width, int* height);
+// jpeg_decode_rgb for n files in memory of `device`, into out[i] ([height[i]][width[i]][3], memory of
+// `device`) after the work queued on `stream`.  Each file's header is read from a prefix copied to the
+// host; a sequential file of the plain shape (jpeg_device_shape in pipeline.cu) is entropy-decoded on the
+// device while the call's budget lasts; any other file, or one the device flags (an error, or a decode
+// that did not converge in jpeg_max_sync_rounds, pipeline.cu), is copied back and read by read_jpeg.  A refusal
+// throws "<who>: file i: <reason>" for the lowest such i, with read_jpeg / libjpeg_decodable's reasons,
+// before any output is written.
+void jpeg_decode_rgb_from_device(const char* who, const uint8_t* const* jpeg, const size_t* len, int n, int device,
+                                 const int* width, const int* height, uint8_t* const* out, Stream stream);
+// Test hook: the segment pass and the speculative decode with subsequences of S bits on one file in host
+// memory, uploaded first.  True with read_jpeg's coefficient layout (components one after another) in
+// *coeffs where the device path takes the file and finds no error; false where it goes to the host path.
+bool jpeg_debug_entropy_decode(const uint8_t* data, size_t len, int S, std::vector<int16_t>* coeffs);
+
+// Exclusive prefix sum of n values on stream s (three launches), the total to device memory; sums holds
+// ceil(n / 1024) values.  ImageContext's scans use it.
+void exclusive_scan_device(Stream s, const unsigned int* in, unsigned int* out, int n, unsigned int* sums,
+                           unsigned long long* d_total);
+
 // An 8-bit image of 1 (gray), 2 (gray + alpha), 3 (RGB) or 4 (RGBA) channels in any layout with
 // non-negative strides: sample (y, x, c) is at byte y * stride[0] + x * stride[1] + c * stride[2] of data.
 struct ImageView {

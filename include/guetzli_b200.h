@@ -313,9 +313,36 @@ int gb200_jpeg_decode_rgb(const uint8_t* const* jpeg, const size_t* len, int n, 
 int gb200_jpeg_decode_rgb_device(const uint8_t* const* jpeg, const size_t* len, int n, int device,
                                  uint8_t* const* out_dev, void* stream);
 
+/* gb200_jpeg_dimensions for n files whose bytes are in device memory of `device`, read after the work queued
+ * on `stream`: a prefix of each file is copied to the host (4 KiB, doubling until the frame header is in
+ * it).  A file without a readable frame size gets 0 x 0.  Returns 1 on success. */
+int gb200_jpeg_dimensions_from_device(const uint8_t* const* jpeg_dev, const size_t* len, int n, int device,
+                                      void* stream, int* width, int* height);
+/* gb200_jpeg_decode_rgb_device for n files whose bytes are in device memory of `device`: the same pixels,
+ * into out_dev[i] of width[i] x height[i] x 3 bytes, which must be the frame's size.  Everything is read
+ * after the work queued on `stream` so far, and the outputs are written when the call returns.  Each
+ * file's header is parsed on the host from a copied prefix.  A sequential (SOF0 / SOF1) file under 256 MiB
+ * whose first scan carries every component in one pass (Ss = 0, Se = 63, Ah = Al = 0) and whose scan data
+ * ends in EOI, with RSTn in order, is Huffman-decoded on the device, up to 2^30 scan bytes per call; every
+ * other file, one the device finds an error in, and one whose speculative decode has not converged
+ * within its rounds, is copied back and read as gb200_jpeg_decode_rgb reads it.  A file of len 0 may have
+ * a null pointer.  Refusals are those of
+ * gb200_jpeg_decode_rgb, with the same reasons ("jpeg_decode_rgb_from_device: file i: <reason>"), plus a
+ * width or height other than the frame's; host, managed and other devices' pointers are refused too.  No
+ * output is written unless every file is accepted.  Returns 1 on success. */
+int gb200_jpeg_decode_rgb_from_device(const uint8_t* const* jpeg_dev, const size_t* len, int n, int device,
+                                      const int* width, const int* height, uint8_t* const* out_dev, void* stream);
+
 /* test hook: ReadJpeg(JPEG_READ_ALL) alone.  dims = {w, h, ncomp, wb0, hb0, wb1, hb1, ...} (11 ints);
  * out receives the quantised coefficients of all components, concatenated. */
 int gb200_debug_read_jpeg(const uint8_t* jpeg_in, size_t jpeg_len, int* dims, int16_t* out, size_t out_cap);
+/* test hook: the device path's entropy decoding (segment pass, speculative Huffman decode with subsequences
+ * of S bits, DC prefix sums) of one file in host memory, uploaded first (on the CPU port: run as host loops).
+ * *status = 1 where the device path takes the file and finds no error, with the coefficients in out as
+ * gb200_debug_read_jpeg gives them; 0 where the file goes to the host path, out untouched.  Returns 1 on
+ * success. */
+int gb200_debug_entropy_decode(const uint8_t* jpeg_in, size_t jpeg_len, int S, int16_t* out, size_t out_cap,
+                               int* status);
 
 /* ---- one image tiled over the GPUs of a node (BASELINE configs[3]) ------------
  * One process per GPU.  Rank 0 obtains an id, the host application distributes it

@@ -40,6 +40,24 @@ for fx in ("prog444_q85", "restart444", "meta_kept", "sub420"):
             b = b[:rng.integers(4, len(b))]
         gb.api.read_jpeg(bytes(b), lib=lib)
 print("damaged jpeg files ok", flush=True)
+# the device path's entropy decoding (segment pass, speculative decode, DC sums) as host loops, on baseline
+# files cut after their SOS header and with single scan bytes changed: read_jpeg's coefficients or the host path
+for fx in ("tiny444", "sub420"):
+    base = open(os.path.join(ROOT, "tests", "golden", "jpeg", fx + ".jpg"), "rb").read()
+    sos = base.find(b"\xff\xda")
+    start = sos + 2 + ((base[sos + 2] << 8) | base[sos + 3])
+    variants = [base[:k] for k in range(start, len(base))]
+    for k in range(start, len(base) - 2):
+        for x in (0x01, 0x80, 0xff):
+            v = bytearray(base)
+            v[k] ^= x
+            variants.append(bytes(v))
+    for i, b in enumerate(variants):
+        taken, coeffs = gb.api.entropy_decode(b, 33 if i % 2 else 1024, lib=lib)
+        if taken:
+            ok, _, want = gb.api.read_jpeg(b, lib=lib)
+            assert ok and np.array_equal(coeffs[:want.size], want), (fx, i)
+print("device entropy decoding of damaged files ok", flush=True)
 a = synth.gradnoise(20, 33, 2).astype(np.float32).transpose(2, 0, 1)
 gb.api.butteraugli_diffmap(a, a[:, ::-1].copy(), lib=lib)
 rgb = np.ascontiguousarray(np.tile(synth.noise(64, 64, 3), (1, 2, 1)))
