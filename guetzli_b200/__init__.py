@@ -9,10 +9,10 @@ from .api import (Params, ProcessStats, process, process_image, process_jpeg, bu
                   DeviceImage, load_library, library_path, write_jpeg, counters,
                   process_tiled_threads, process_tiled, dist_unique_id, dist_init, dist_shutdown,
                   last_error, Comparator, ComparatorSet, ButteraugliBatch, adaptive_quantization,
-                  butteraugli_srgb, decode_jpeg)
+                  butteraugli_srgb, decode_jpeg, heatmap, heatmap_thresholds)
 
 __all__ = ["Params", "ProcessStats", "process", "process_image", "process_jpeg", "butteraugli_score_for_quality",
            "DeviceImage", "load_library", "library_path", "write_jpeg", "counters",
            "process_tiled_threads", "process_tiled", "dist_unique_id", "dist_init", "dist_shutdown", "last_error",
            "Comparator", "ComparatorSet", "ButteraugliBatch", "adaptive_quantization", "butteraugli_srgb",
-           "decode_jpeg"]
+           "decode_jpeg", "heatmap", "heatmap_thresholds"]

@@ -7,6 +7,7 @@ CUDA-only: importing works anywhere, but calling fails loudly without the built
 extension or without a GPU -- there is no CPU fallback in the product.
 """
 import ctypes as C
+import math
 import os
 from dataclasses import dataclass, field
 
@@ -168,6 +169,25 @@ def load_library(path=None):
         getattr(lib, entry).argtypes = set_diffmap
         getattr(lib, entry + "_device").argtypes = set_diffmap + [C.c_void_p]
     lib.gb200_butteraugli_comparator_set_destroy.argtypes = [C.c_void_p]
+    lib.gb200_butteraugli_comparator_create_device.restype = C.c_void_p
+    lib.gb200_butteraugli_comparator_create_device.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
+                                                               C.c_void_p]
+    lib.gb200_butteraugli_comparator_create_srgb_device.restype = C.c_void_p
+    lib.gb200_butteraugli_comparator_create_srgb_device.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
+                                                                    C.c_int, C.c_void_p]
+    lib.gb200_butteraugli_comparator_set_create_device.restype = C.c_void_p
+    lib.gb200_butteraugli_comparator_set_create_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                                                   C.c_int, C.c_int, C.c_void_p]
+    lib.gb200_butteraugli_comparator_set_create_srgb_device.restype = C.c_void_p
+    lib.gb200_butteraugli_comparator_set_create_srgb_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p,
+                                                                        C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                                                        C.c_void_p]
+    lib.gb200_butteraugli_comparator_mask_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.gb200_butteraugli_adaptive_quantization_device.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                                                   C.c_void_p, C.c_void_p]
+    heatmap = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_double, C.c_double, C.c_void_p, C.c_int]
+    lib.gb200_butteraugli_heatmap.argtypes = heatmap
+    lib.gb200_butteraugli_heatmap_device.argtypes = heatmap + [C.c_void_p]
     _libs[path] = lib
     return lib
 
@@ -632,7 +652,9 @@ class Comparator(_Handle):
     """butteraugli::ButteraugliComparator (butteraugli.h:425) on one GPU: the original rgb0, planar
     linear RGB float32 [3][h][w], nominally in 0..255 and at least 8x8, stays resident and is scored
     against any number of images, up to `capacity` (1..16383) of them per diffmap() call in one pass of
-    the Compare chain.  Used by one thread at a time.  Values outside 0..255 (ringing below 0, highlights above 255) are scored as the reference scores
+    the Compare chain.  rgb0 may be a numpy array or a float32 CUDA tensor on the comparator's device,
+    read after the work queued on that device's current torch stream and copied on the device; either
+    way it may be changed or freed once the comparator is made.  Used by one thread at a time.  Values outside 0..255 (ringing below 0, highlights above 255) are scored as the reference scores
     them, bit for bit; this is tested from -300 to 4500.  NaN and infinities must not be passed: the
     reference's result is undefined for them."""
 
@@ -641,13 +663,22 @@ class Comparator(_Handle):
     def __init__(self, rgb0, device=0, capacity=1, lib=None):
         self.lib = lib or load_library()
         self.channels = 0  # made from float planes
-        a = np.ascontiguousarray(rgb0, dtype=np.float32)
-        if a.ndim != 3 or a.shape[0] != 3:
-            raise ValueError(f"rgb0 must be planar [3][h][w], got shape {a.shape}")
-        _, self.h, self.w = a.shape
         self.device, self.capacity = device, int(capacity)
-        self._h = self.lib.gb200_butteraugli_comparator_create_batch(a.ctypes.data, self.w, self.h, self.capacity,
-                                                                     device)
+        if _is_torch_tensor(rgb0) and rgb0.is_cuda:
+            import torch
+            if rgb0.dtype != torch.float32 or rgb0.ndim != 3 or rgb0.shape[0] != 3:
+                raise ValueError(f"rgb0 must be float32 planar [3][h][w], got {rgb0.dtype} {tuple(rgb0.shape)}")
+            t = rgb0.contiguous()
+            _, self.h, self.w = t.shape
+            self._h = self.lib.gb200_butteraugli_comparator_create_device(
+                t.data_ptr(), self.w, self.h, self.capacity, device, torch.cuda.current_stream(t.device).cuda_stream)
+        else:
+            a = np.ascontiguousarray(rgb0, dtype=np.float32)
+            if a.ndim != 3 or a.shape[0] != 3:
+                raise ValueError(f"rgb0 must be planar [3][h][w], got shape {a.shape}")
+            _, self.h, self.w = a.shape
+            self._h = self.lib.gb200_butteraugli_comparator_create_batch(a.ctypes.data, self.w, self.h,
+                                                                         self.capacity, device)
         if not self._h:
             raise RuntimeError("gb200_butteraugli_comparator_create failed: " + _err(self.lib))
 
@@ -656,14 +687,35 @@ class Comparator(_Handle):
         """A comparator whose original is an 8-bit sRGB image, uint8 [h][w][C] in host memory with C = 3
         (RGB) or 4 (RGBA), at least 8x8, scored as butteraugli_srgb scores it.  With C = 4 the original
         is kept twice, laid over black and over white.  diffmap() then takes uint8 [h][w][C] or
-        [n][h][w][C] with the same C, numpy or CUDA tensors, and nothing else; mask() refuses RGBA."""
+        [n][h][w][C] with the same C, numpy or CUDA tensors, and nothing else; mask() refuses RGBA.
+        An original in CUDA memory goes to from_srgb_device."""
+        a, _ = _srgb_images("img0", img0, (3,), cuda_ok=False)
+        return cls._from_srgb(a, False, capacity, device, lib)
+
+    @classmethod
+    def from_srgb_device(cls, img0, capacity=1, device=0, lib=None):
+        """from_srgb with the original a uint8 CUDA tensor [h][w][C] on the comparator's device, converted where it
+        lies after the work queued on that device's current torch stream; no pixel goes through the host.  The
+        comparator is the one from_srgb makes of the same bytes, and img0 may be changed or freed once it is made."""
+        a, cuda = _srgb_images("img0", img0, (3,))
+        if not cuda:
+            raise ValueError(f"img0 must be a CUDA tensor, got {type(img0).__name__} (from_srgb takes host memory)")
+        return cls._from_srgb(a, True, capacity, device, lib)
+
+    @classmethod
+    def _from_srgb(cls, a, cuda, capacity, device, lib):
         self = cls.__new__(cls)
         self.lib = lib or load_library()
-        a, _ = _srgb_images("img0", img0, (3,), cuda_ok=False)
         self.h, self.w, self.channels = a.shape
         self.device, self.capacity = device, int(capacity)
-        self._h = self.lib.gb200_butteraugli_comparator_create_srgb(a.ctypes.data, self.w, self.h, self.channels,
-                                                                    self.capacity, device)
+        if cuda:
+            import torch
+            self._h = self.lib.gb200_butteraugli_comparator_create_srgb_device(
+                a.data_ptr(), self.w, self.h, self.channels, self.capacity, device,
+                torch.cuda.current_stream(a.device).cuda_stream)
+        else:
+            self._h = self.lib.gb200_butteraugli_comparator_create_srgb(a.ctypes.data, self.w, self.h, self.channels,
+                                                                        self.capacity, device)
         if not self._h:
             raise RuntimeError("gb200_butteraugli_comparator_create_srgb failed: " + _err(self.lib))
         return self
@@ -746,12 +798,19 @@ class Comparator(_Handle):
                                                                         score.ctypes.data))
         return (dm[0], float(score[0])) if single else (dm, score)
 
-    def mask(self):
-        """ButteraugliComparator::Mask -> (mask, mask_dc), float32 [3][h][w] each."""
-        m = np.empty((3, self.h, self.w), dtype=np.float32)
-        mdc = np.empty_like(m)
-        self._ck(self.lib.gb200_butteraugli_comparator_mask(self._h, m.ctypes.data, mdc.ctypes.data))
+    def mask(self, cuda=False):
+        """ButteraugliComparator::Mask -> (mask, mask_dc), float32 [3][h][w] each: numpy arrays, or with
+        cuda=True tensors on the comparator's device, written in order on its current torch stream."""
+        [m, mdc], [mp, mdcp], stream = _outputs(self._torch_device() if cuda else None, [(3, self.h, self.w)] * 2)
+        if cuda:
+            self._ck(self.lib.gb200_butteraugli_comparator_mask_device(self._h, mp, mdcp, stream))
+        else:
+            self._ck(self.lib.gb200_butteraugli_comparator_mask(self._h, mp, mdcp))
         return m, mdc
+
+    def _torch_device(self):
+        import torch
+        return torch.device("cuda", self.device)
 
 
 class ButteraugliBatch(_Handle):
@@ -914,8 +973,10 @@ class ButteraugliBatch(_Handle):
 
 class ComparatorSet(_Handle):
     """Many resident originals of sizes of their own, each scored against any number of candidates: the
-    originals rgb0s, a sequence of planar linear RGB float32 [3][h_i][w_i] in host memory, each at least 8x8,
-    are analysed once on one GPU and kept there (40 bytes per pixel).  diffmap() scores up to `capacity`
+    originals rgb0s, a sequence of planar linear RGB float32 [3][h_i][w_i], each at least 8x8, are analysed
+    once on one GPU and kept there (40 bytes per pixel).  They are all numpy arrays, or all CUDA tensors on the
+    set's device, read in place after the work queued on its current torch stream; either way they may be
+    changed or freed once the set is made.  diffmap() scores up to `capacity`
     (1..16383) candidates per call, each against the original it names, in one pass of the Compare chain;
     each result is bit for bit ButteraugliBatch.diffmap_sizes' on the pair (original, candidate), whatever
     else the call holds.  Used by one thread at a time."""
@@ -927,8 +988,8 @@ class ComparatorSet(_Handle):
 
     @classmethod
     def from_srgb(cls, img0s, capacity=1, device=0, lib=None):
-        """A set of 8-bit sRGB originals, uint8 [h_i][w_i][C_i] in host memory with C_i = 3 (RGB) or 4
-        (RGBA), each at least 8x8, scored as butteraugli_srgb scores them (an RGBA original is kept twice,
+        """A set of 8-bit sRGB originals, uint8 [h_i][w_i][C_i] with C_i = 3 (RGB) or 4 (RGBA), all numpy
+        arrays or all CUDA tensors on the set's device (as in the constructor), each at least 8x8, scored as butteraugli_srgb scores them (an RGBA original is kept twice,
         laid over black and over white).  diffmap() then takes uint8 [h][w][C] candidates with their
         original's shape, and nothing else."""
         self = cls.__new__(cls)
@@ -939,9 +1000,9 @@ class ComparatorSet(_Handle):
         self.lib = lib or load_library()
         self.device, self.capacity, self.srgb = device, int(capacity), srgb
         name = "img0s" if srgb else "rgb0s"
-        n, _, ptrs, self.shapes = _sizes_items(
+        n, dev, ptrs, self.shapes = _sizes_items(
             (name,), (items,), lambda n: None if n >= 1 else "a set holds at least 1 original, got 0",
-            "uint8" if srgb else "float32", _interleaved_error if srgb else _planar_error, device, cuda_ok=False)
+            "uint8" if srgb else "float32", _interleaved_error if srgb else _planar_error, device)
         hw = [s[:2] if srgb else s[1:] for s in self.shapes]
         for i, (h, w) in enumerate(hw):
             if not (8 <= h < 65536 and 8 <= w < 65536):
@@ -949,14 +1010,15 @@ class ComparatorSet(_Handle):
         hs = np.array([x[0] for x in hw], dtype=np.int32)
         ws = np.array([x[1] for x in hw], dtype=np.int32)
         P = C.c_void_p * n
-        if srgb:
-            chs = np.array([s[2] for s in self.shapes], dtype=np.int32)
-            self._h = self.lib.gb200_butteraugli_comparator_set_create_srgb(ws.ctypes.data, hs.ctypes.data,
-                                                                            chs.ctypes.data, P(*ptrs), n,
-                                                                            self.capacity, device)
+        chs = np.array([s[2] for s in self.shapes], dtype=np.int32) if srgb else None
+        args = (ws.ctypes.data, hs.ctypes.data) + ((chs.ctypes.data,) if srgb else ()) + (P(*ptrs), n,
+                                                                                          self.capacity, device)
+        entry = "gb200_butteraugli_comparator_set_create" + ("_srgb" if srgb else "")
+        if dev is not None:
+            import torch
+            self._h = getattr(self.lib, entry + "_device")(*args, torch.cuda.current_stream(dev).cuda_stream)
         else:
-            self._h = self.lib.gb200_butteraugli_comparator_set_create(ws.ctypes.data, hs.ctypes.data, P(*ptrs), n,
-                                                                       self.capacity, device)
+            self._h = getattr(self.lib, entry)(*args)
         if not self._h:
             raise RuntimeError("gb200_butteraugli_comparator_set_create failed: " + _err(self.lib))
 
@@ -1002,11 +1064,24 @@ class ComparatorSet(_Handle):
 
 def adaptive_quantization(rgb, device=0, lib=None):
     """butteraugli::ButteraugliAdaptiveQuantization: rgb planar linear RGB float32 [3][h][w], nominally
-    in 0..255 -> quant [h][w] float32.  Raises ValueError below 16x16, where the reference returns
-    false.  Values outside 0..255 (ringing below 0, highlights above 255) are scored as the reference scores
+    in 0..255 -> quant [h][w] float32.  A CUDA tensor is read on its own device after the work queued on
+    its current torch stream, and quant comes back as a tensor there (`device` is then not used).  Raises
+    ValueError below 16x16, where the reference returns false.  Values outside 0..255 (ringing below 0, highlights above 255) are scored as the reference scores
     them, bit for bit; this is tested from -300 to 4500.  NaN and infinities must not be passed: the
     reference's result is undefined for them."""
     lib = lib or load_library()
+    if _is_torch_tensor(rgb) and rgb.is_cuda:
+        import torch
+        if rgb.dtype != torch.float32 or rgb.ndim != 3 or rgb.shape[0] != 3:
+            raise ValueError(f"rgb must be float32 planar [3][h][w], got {rgb.dtype} {tuple(rgb.shape)}")
+        t = rgb.contiguous()
+        _, h, w = t.shape
+        if w < 16 or h < 16:
+            raise ValueError(f"adaptive quantization needs at least 16x16 pixels, got {w}x{h}")
+        [quant], [qp], stream = _outputs(t.device, [(h, w)])
+        if not lib.gb200_butteraugli_adaptive_quantization_device(t.data_ptr(), w, h, t.device.index, qp, stream):
+            raise RuntimeError(_err(lib))
+        return quant
     a = np.ascontiguousarray(rgb, dtype=np.float32)
     if a.ndim != 3 or a.shape[0] != 3:
         raise ValueError(f"rgb must be planar [3][h][w], got shape {a.shape}")
@@ -1017,6 +1092,88 @@ def adaptive_quantization(rgb, device=0, lib=None):
     if not lib.gb200_butteraugli_adaptive_quantization(a.ctypes.data, w, h, device, quant.ctypes.data):
         raise RuntimeError(_err(lib))
     return quant
+
+
+def heatmap_thresholds():
+    """The butteraugli tool's heat-map thresholds (butteraugli_main.cc:423-424): (good, bad) =
+    (ButteraugliFuzzyInverse(1.5), ButteraugliFuzzyInverse(0.5))."""
+    return _fuzzy_inverse(1.5), _fuzzy_inverse(0.5)
+
+
+def _fuzzy_inverse(seek):
+    # ButteraugliFuzzyClass / ButteraugliFuzzyInverse (butteraugli.cc:1902, :1923) in the same double arithmetic,
+    # as the butteraugli CLI states them (cli/butteraugli.cc)
+    def fuzzy_class(score):
+        width_up, width_down, m0, scaler = 6.07887388532, 5.50793514384, 2.0, 0.840253347958
+        if score < 1.0:
+            v = m0 / (1.0 + math.exp((score - 1.0) * width_down))
+            v -= 1.0
+            v *= 2.0 - scaler
+            return v + scaler
+        return m0 / (1.0 + math.exp((score - 1.0) * width_up)) * scaler
+    pos, r = 0.0, 1.0
+    while r >= 1e-10:
+        pos += -r if fuzzy_class(pos) < seek else r
+        r *= 0.5
+    return pos
+
+
+def heatmap(diffmap, good=None, bad=None, device=0, lib=None):
+    """butteraugli::CreateHeatMapImage (butteraugli.cc:1979): a diffmap float32 [h][w] -> its heat map, uint8
+    [h][w][3], the reference's bytes exactly.  good, bad: the thresholds, 0 < good < bad; None for either takes
+    the butteraugli tool's (heatmap_thresholds()).
+
+    A numpy array gives a numpy array, made on GPU `device`; a CUDA tensor gives a tensor on its device, made
+    after the work queued on that device's current torch stream.  A list (or tuple) of maps of sizes of their
+    own, all numpy arrays or all CUDA tensors, gives a list, made in one launch."""
+    lib = lib or load_library()
+    tool_good, tool_bad = heatmap_thresholds()
+    good = tool_good if good is None else float(good)
+    bad = tool_bad if bad is None else float(bad)
+    many = isinstance(diffmap, (list, tuple))
+    maps = list(diffmap) if many else [diffmap]
+    if not maps:
+        raise ValueError("heatmap needs at least 1 map, got an empty list")
+    cuda = _is_torch_tensor(maps[0]) and maps[0].is_cuda
+    items = []
+    for i, m in enumerate(maps):
+        name = f"diffmap[{i}]" if many else "diffmap"
+        if cuda != (_is_torch_tensor(m) and m.is_cuda):
+            raise ValueError("the maps must all be CUDA tensors or all host arrays")
+        if cuda:
+            import torch
+            if m.dtype != torch.float32:
+                raise ValueError(f"{name} must be float32, got {m.dtype}")
+            m = m.contiguous()
+        else:
+            m = np.asarray(m.numpy() if _is_torch_tensor(m) else m)
+            if m.dtype != np.float32:
+                raise ValueError(f"{name} must be float32, got {m.dtype}")
+            m = np.ascontiguousarray(m)
+        if m.ndim != 2 or m.shape[0] < 1 or m.shape[1] < 1:
+            raise ValueError(f"{name} must be [h][w] with h, w >= 1, got shape {tuple(m.shape)}")
+        items.append(m)
+    n = len(items)
+    hs = np.array([m.shape[0] for m in items], dtype=np.int32)
+    ws = np.array([m.shape[1] for m in items], dtype=np.int32)
+    P = C.c_void_p * n
+    if cuda:
+        import torch
+        dev = items[0].device
+        for i, m in enumerate(items):
+            if m.device != dev:
+                raise ValueError(f"the maps must be on one device: diffmap[{i}] is on {m.device}, not {dev}")
+        out = [torch.empty((m.shape[0], m.shape[1], 3), dtype=torch.uint8, device=dev) for m in items]
+        ok = lib.gb200_butteraugli_heatmap_device(ws.ctypes.data, hs.ctypes.data, P(*[m.data_ptr() for m in items]),
+                                                  n, good, bad, P(*[o.data_ptr() for o in out]), dev.index,
+                                                  torch.cuda.current_stream(dev).cuda_stream)
+    else:
+        out = [np.empty((m.shape[0], m.shape[1], 3), dtype=np.uint8) for m in items]
+        ok = lib.gb200_butteraugli_heatmap(ws.ctypes.data, hs.ctypes.data, P(*[m.ctypes.data for m in items]), n,
+                                           good, bad, P(*[o.ctypes.data for o in out]), device)
+    if not ok:
+        raise RuntimeError(_err(lib))
+    return out if many else out[0]
 
 
 def counters(lib=None):

@@ -178,8 +178,21 @@ void Butteraugli::release() {
   have_stream_ = false;
 }
 
-void Butteraugli::analyse_original(const float* linear_rgb) {
-  if (linear_rgb != nullptr) r_.upload_planes(linear_rgb, lin_, 3);
+void Butteraugli::lin_from_device(const float* linear_rgb, Stream caller) {
+  const size_t row = sizeof(float) * g_.w, pitch = sizeof(float) * g_.pitch;
+  stream_wait(s_, caller);
+  // [3][h][w] -> [3][h][pitch]: a plane is h rows of pitch, so the three planes are 3h rows
+  d2d_2d(lin_, pitch, linear_rgb, row, row, static_cast<size_t>(3) * g_.h, s_);
+}
+
+void Butteraugli::analyse_original(const float* linear_rgb, bool device, Stream caller) {
+  if (linear_rgb != nullptr) {
+    if (device) {
+      lin_from_device(linear_rgb, caller);
+    } else {
+      r_.upload_planes(linear_rgb, lin_, 3);
+    }
+  }
   opsin(lin_, xyb_);
   separate(xyb_, ps0_);
   fused_sup0(1, 0);
@@ -194,12 +207,10 @@ float Butteraugli::compare_linear(const float* linear_rgb) {
 
 float Butteraugli::compare_linear_device(const float* linear_rgb, float* diffmap, Stream caller) {
   bind();
-  const size_t row = sizeof(float) * g_.w, pitch = sizeof(float) * g_.pitch;
-  stream_wait(s_, caller);
-  // [3][h][w] -> [3][h][pitch]: a plane is h rows of pitch, so the three planes are 3h rows
-  d2d_2d(lin_, pitch, linear_rgb, row, row, static_cast<size_t>(3) * g_.h, s_);
+  lin_from_device(linear_rgb, caller);
   const float m = compare();
   if (diffmap != nullptr) {
+    const size_t row = sizeof(float) * g_.w, pitch = sizeof(float) * g_.pitch;
     d2d_2d(diffmap, row, dm_, pitch, row, g_.h, s_);
     stream_sync(s_);
   }
@@ -333,9 +344,17 @@ void Butteraugli::srgb_backgrounds(int n, int channels, int only, float* diffmap
   }
 }
 
-void Butteraugli::analyse_original_srgb(const uint8_t* img0, int channels, int background) {
+void Butteraugli::analyse_original_srgb(const uint8_t* img0, int channels, int background, bool device,
+                                        Stream caller) {
   check_channels(channels);
   bind();
+  if (device) {  // converted where it lies
+    stream_wait(s_, caller);
+    srgb_to_linear(img0, 1, channels, background, lin_, g_.pitch);
+    analyse_original();
+    stream_sync(s_);
+    return;
+  }
   const size_t bytes = static_cast<size_t>(g_.w) * g_.h * channels;
   uint8_t* u8 = static_cast<uint8_t*>(dev_alloc(bytes));
   try {
@@ -421,7 +440,7 @@ void Butteraugli::compare_batch_sizes_srgb(const int* w, const int* h, const int
 
 // ---- comparator sets (butteraugli.h) ----
 ComparatorSet::ComparatorSet(const int* w, const int* h, const int* channels, const void* const* img0, int count,
-                             int capacity, int device)
+                             int capacity, int device, bool on_device, Stream caller)
     : w_(w, w + count), h_(h, h + count) {
   if (channels != nullptr) {
     channels_.assign(channels, channels + count);
@@ -430,6 +449,7 @@ ComparatorSet::ComparatorSet(const int* w, const int* h, const int* channels, co
   ba_.reset(new Butteraugli(*std::max_element(w_.begin(), w_.end()), *std::max_element(h_.begin(), h_.end()),
                             capacity, device, Butteraugli::Slots::kPairs));
 #if defined(GB200_HOSTSIM)
+  if (on_device) throw std::runtime_error("the CPU port has no device memory");
   for (int i = 0; i < count; ++i) {
     const size_t in = static_cast<size_t>(w[i]) * h[i] * (srgb() ? channels[i] : 3 * sizeof(float));
     const unsigned char* p = static_cast<const unsigned char*>(img0[i]);
@@ -452,6 +472,7 @@ ComparatorSet::ComparatorSet(const int* w, const int* h, const int* channels, co
   ba_->bind();
   store_ = dev_alloc(bytes);
   try {
+    if (on_device) stream_wait(ba_->region().s, caller);
     unsigned char* base = static_cast<unsigned char*>(store_);
     // mixed passes of up to `capacity` originals: every original over black, then the RGBA ones over white
     for (int bg = 0; bg < 2; ++bg) {
@@ -472,7 +493,7 @@ ComparatorSet::ComparatorSet(const int* w, const int* h, const int* channels, co
           to[j] = reinterpret_cast<float*>(base + at_[bg][i]);
         }
         ba_->analyse_originals(cw.data(), ch.data(), srgb() ? cc.data() : nullptr, in.data(), static_cast<int>(m),
-                               bg == 0 ? 0 : 255, to.data());
+                               bg == 0 ? 0 : 255, to.data(), on_device);
       }
     }
   } catch (...) {
@@ -533,11 +554,19 @@ void ComparatorSet::compare(const int* original, const void* const* img1, int n,
 #endif
 }
 
-void Butteraugli::adaptive_quantization(const float* linear_rgb, float* quant) {
+void Butteraugli::adaptive_quantization(const float* linear_rgb, float* quant, bool device, Stream caller) {
   bind();
-  r_.upload_planes(linear_rgb, lin_, 3);
+  if (!device) {
+    r_.upload_planes(linear_rgb, lin_, 3);
+    mask_planes(lin_);
+    r_.download_planes(mask_ + g_.plane, quant, 1);
+    return;
+  }
+  lin_from_device(linear_rgb, caller);
   mask_planes(lin_);
-  r_.download_planes(mask_ + g_.plane, quant, 1);
+  const size_t row = sizeof(float) * g_.w, pitch = sizeof(float) * g_.pitch;
+  d2d_2d(quant, row, mask_ + g_.plane, pitch, row, g_.h, s_);
+  stream_sync(s_);
 }
 
 void Butteraugli::compare_begin() {

@@ -410,21 +410,38 @@ int gb200_butteraugli_comparator_diffmap_device(gb200_butteraugli_comparator* c,
   });
 }
 
+namespace {
 // The comparator with `capacity` candidate slots: ButteraugliComparator::ButteraugliComparator(rgb0) once
-// (capacity 1: the single-image metric)
-gb200_butteraugli_comparator* gb200_butteraugli_comparator_create_batch(const float* rgb0, int w, int h, int capacity,
-                                                                        int device) {
+// (capacity 1: the single-image metric); on_device: rgb0 in memory of `device`, read after `stream`'s work
+gb200_butteraugli_comparator* comparator_create(const float* rgb0, int w, int h, int capacity, int device,
+                                                bool on_device, void* stream) {
   gb200_butteraugli_comparator* c = nullptr;
   guarded([&]() {
     if (rgb0 == nullptr) throw std::runtime_error("butteraugli comparator: no image");
     check_create("butteraugli comparator", "image", w, h, capacity);
+    if (on_device) {
+      const void* ptrs[1] = {rgb0};
+      const char* what[1] = {"rgb0"};
+      check_device_pointers("butteraugli comparator", device, ptrs, what, 1);
+    }
     std::unique_ptr<gb200::Butteraugli> ba(
         new gb200::Butteraugli(w, h, capacity, device, gb200::Butteraugli::Slots::kCandidates));
-    ba->analyse_original(rgb0);
+    ba->analyse_original(rgb0, on_device, caller_stream(stream));
     c = new gb200_butteraugli_comparator;
     c->ba = ba.release();
   });
   return c;
+}
+}  // namespace
+
+gb200_butteraugli_comparator* gb200_butteraugli_comparator_create_batch(const float* rgb0, int w, int h, int capacity,
+                                                                        int device) {
+  return comparator_create(rgb0, w, h, capacity, device, false, nullptr);
+}
+
+gb200_butteraugli_comparator* gb200_butteraugli_comparator_create_device(const float* rgb0_dev, int w, int h,
+                                                                         int capacity, int device, void* stream) {
+  return comparator_create(rgb0_dev, w, h, capacity, device, true, stream);
 }
 
 namespace {
@@ -672,20 +689,27 @@ int gb200_butteraugli_batch_diffmap_sizes_srgb_device(gb200_butteraugli_batch* b
   return batch_diffmap_sizes_srgb(b, w, h, channels, img0_dev, img1_dev, n, diffmap_dev, score, true, stream);
 }
 
-gb200_butteraugli_comparator* gb200_butteraugli_comparator_create_srgb(const uint8_t* img0, int w, int h, int channels,
-                                                                       int capacity, int device) {
+namespace {
+gb200_butteraugli_comparator* comparator_create_srgb(const uint8_t* img0, int w, int h, int channels, int capacity,
+                                                     int device, bool on_device, void* stream) {
   gb200_butteraugli_comparator* c = nullptr;
   if (!channels_ok("butteraugli comparator", channels)) return nullptr;
   guarded([&]() {
     if (img0 == nullptr) throw std::runtime_error("butteraugli comparator: no image");
     check_create("butteraugli comparator", "image", w, h, capacity);
+    if (on_device) {
+      const void* ptrs[1] = {img0};
+      const char* what[1] = {"img0"};
+      check_device_pointers("butteraugli comparator", device, ptrs, what, 1);
+    }
+    const gb200::Stream caller = caller_stream(stream);
     const gb200::Butteraugli::Slots kind = gb200::Butteraugli::Slots::kCandidates;
     std::unique_ptr<gb200::Butteraugli> black(new gb200::Butteraugli(w, h, capacity, device, kind));
-    black->analyse_original_srgb(img0, channels, 0);
+    black->analyse_original_srgb(img0, channels, 0, on_device, caller);
     std::unique_ptr<gb200::Butteraugli> white;
     if (channels == 4) {  // a second resident original, laid over white
       white.reset(new gb200::Butteraugli(w, h, capacity, device, kind));
-      white->analyse_original_srgb(img0, channels, 255);
+      white->analyse_original_srgb(img0, channels, 255, on_device, caller);
     }
     c = new gb200_butteraugli_comparator;
     c->ba = black.release();
@@ -693,6 +717,18 @@ gb200_butteraugli_comparator* gb200_butteraugli_comparator_create_srgb(const uin
     c->channels = channels;
   });
   return c;
+}
+}  // namespace
+
+gb200_butteraugli_comparator* gb200_butteraugli_comparator_create_srgb(const uint8_t* img0, int w, int h, int channels,
+                                                                       int capacity, int device) {
+  return comparator_create_srgb(img0, w, h, channels, capacity, device, false, nullptr);
+}
+
+gb200_butteraugli_comparator* gb200_butteraugli_comparator_create_srgb_device(const uint8_t* img0_dev, int w, int h,
+                                                                              int channels, int capacity, int device,
+                                                                              void* stream) {
+  return comparator_create_srgb(img0_dev, w, h, channels, capacity, device, true, stream);
 }
 
 int gb200_butteraugli_comparator_diffmap_srgb(gb200_butteraugli_comparator* c, const uint8_t* img1, int n,
@@ -711,7 +747,8 @@ namespace {
 const char* const kSet = "butteraugli comparator set";
 
 gb200_butteraugli_comparator_set* set_create(const int* w, const int* h, const int* channels, const void* const* img0,
-                                             int count, int capacity, int device, bool srgb) {
+                                             int count, int capacity, int device, bool srgb, bool on_device = false,
+                                             void* stream = nullptr) {
   if (w == nullptr || h == nullptr || img0 == nullptr || (srgb && channels == nullptr)) {
     g_err = std::string(kSet) + (srgb ? ": no sizes, no channels or no images" : ": no sizes or no images");
     return nullptr;
@@ -736,8 +773,14 @@ gb200_butteraugli_comparator_set* set_create(const int* w, const int* h, const i
   gb200_butteraugli_comparator_set* s = nullptr;
   guarded([&]() {
     check_capacity(kSet, capacity);
-    std::unique_ptr<gb200::ComparatorSet> set(new gb200::ComparatorSet(w, h, srgb ? channels : nullptr, img0, count,
-                                                                       capacity, device));
+    if (on_device)
+      for (int i = 0; i < count; ++i) {
+        const std::string name = std::string(srgb ? "img0" : "rgb0") + "[" + std::to_string(i) + "]";
+        const char* what[1] = {name.c_str()};
+        check_device_pointers(kSet, device, &img0[i], what, 1);
+      }
+    std::unique_ptr<gb200::ComparatorSet> set(new gb200::ComparatorSet(
+        w, h, srgb ? channels : nullptr, img0, count, capacity, device, on_device, caller_stream(stream)));
     s = new gb200_butteraugli_comparator_set;
     s->set = set.release();
   });
@@ -787,6 +830,21 @@ gb200_butteraugli_comparator_set* gb200_butteraugli_comparator_set_create_srgb(c
   return set_create(w, h, channels, reinterpret_cast<const void* const*>(img0), count, capacity, device, true);
 }
 
+gb200_butteraugli_comparator_set* gb200_butteraugli_comparator_set_create_device(const int* w, const int* h,
+                                                                                 const float* const* rgb0_dev,
+                                                                                 int count, int capacity, int device,
+                                                                                 void* stream) {
+  return set_create(w, h, nullptr, reinterpret_cast<const void* const*>(rgb0_dev), count, capacity, device, false,
+                    true, stream);
+}
+
+gb200_butteraugli_comparator_set* gb200_butteraugli_comparator_set_create_srgb_device(
+    const int* w, const int* h, const int* channels, const uint8_t* const* img0_dev, int count, int capacity,
+    int device, void* stream) {
+  return set_create(w, h, channels, reinterpret_cast<const void* const*>(img0_dev), count, capacity, device, true,
+                    true, stream);
+}
+
 int gb200_butteraugli_comparator_set_diffmap(gb200_butteraugli_comparator_set* s, const int* original,
                                              const float* const* rgb1, int n, float* const* diffmap, double* score) {
   return set_diffmap(s, original, reinterpret_cast<const void* const*>(rgb1), n, diffmap, score, false, false, nullptr);
@@ -818,8 +876,9 @@ void gb200_butteraugli_comparator_set_destroy(gb200_butteraugli_comparator_set* 
   delete s;
 }
 
+namespace {
 // ButteraugliComparator::Mask (b/butteraugli.cc:793)
-int gb200_butteraugli_comparator_mask(gb200_butteraugli_comparator* c, float* mask, float* mask_dc) {
+int comparator_mask(gb200_butteraugli_comparator* c, float* mask, float* mask_dc, bool device, void* stream) {
   if (c == nullptr || mask == nullptr || mask_dc == nullptr) {
     g_err = "butteraugli comparator: no comparator or no output";
     return 0;
@@ -828,11 +887,18 @@ int gb200_butteraugli_comparator_mask(gb200_butteraugli_comparator* c, float* ma
     g_err = "butteraugli comparator: an RGBA comparator has two originals (over black and over white), no one mask";
     return 0;
   }
-  return guarded([&]() { c->ba->mask(mask, mask_dc); });
+  return guarded([&]() {
+    if (device) {
+      const void* ptrs[2] = {mask, mask_dc};
+      const char* what[2] = {"mask", "mask_dc"};
+      check_device_pointers("butteraugli comparator", c->ba->device(), ptrs, what, 2);
+    }
+    c->ba->mask(mask, mask_dc, device, caller_stream(stream));
+  });
 }
 
 // butteraugli::ButteraugliAdaptiveQuantization (b/butteraugli.cc:1880)
-int gb200_butteraugli_adaptive_quantization(const float* rgb, int w, int h, int device, float* quant) {
+int adaptive_quantization(const float* rgb, int w, int h, int device, float* quant, bool on_device, void* stream) {
   if (rgb == nullptr || quant == nullptr) {
     g_err = "butteraugli adaptive quantization: no image or no output";
     return 0;
@@ -842,10 +908,88 @@ int gb200_butteraugli_adaptive_quantization(const float* rgb, int w, int h, int 
     return 0;
   }
   return guarded([&]() {
+    if (on_device) {  // the quantization field depends on the image alone: no analysis of it is needed
+      const void* ptrs[2] = {rgb, quant};
+      const char* what[2] = {"rgb", "quant"};
+      check_device_pointers("butteraugli adaptive quantization", device, ptrs, what, 2);
+      gb200::Butteraugli ba(w, h, device, nullptr);
+      ba.adaptive_quantization(rgb, quant, true, caller_stream(stream));
+      return;
+    }
     gb200::Butteraugli ba(w, h, device, nullptr);
     ba.analyse_original(rgb);
     ba.adaptive_quantization(rgb, quant);
   });
+}
+
+// CreateHeatMapImage (b/butteraugli.cc:1979) of n maps in one launch
+int heatmap(const int* w, const int* h, const float* const* diffmap, int n, double good, double bad,
+            uint8_t* const* rgb, int device, bool on_device, void* stream) {
+  const char* const who = "butteraugli heatmap";
+  if (w == nullptr || h == nullptr || diffmap == nullptr || rgb == nullptr) {
+    g_err = std::string(who) + ": no sizes, no maps or no outputs";
+    return 0;
+  }
+  if (n < 1) {
+    g_err = std::string(who) + ": n = " + std::to_string(n) + ", a call takes at least 1 map";
+    return 0;
+  }
+  if (!(good > 0) || !(bad > good)) {
+    g_err = std::string(who) + ": the thresholds must satisfy 0 < good < bad, got good = " + std::to_string(good) +
+            ", bad = " + std::to_string(bad);
+    return 0;
+  }
+  for (int i = 0; i < n; ++i) {
+    const std::string map = std::string(who) + ": map " + std::to_string(i);
+    if (w[i] < 1 || h[i] < 1) {
+      g_err = map + " is " + std::to_string(w[i]) + "x" + std::to_string(h[i]) + ", a map has at least 1x1 pixels";
+      return 0;
+    }
+    if (diffmap[i] == nullptr || rgb[i] == nullptr) {
+      g_err = map + " has a null pointer";
+      return 0;
+    }
+  }
+  return guarded([&]() {
+    if (on_device)
+      for (int i = 0; i < n; ++i) {
+        const std::string k = "[" + std::to_string(i) + "]";
+        const std::string names[2] = {"diffmap" + k, "rgb" + k};
+        const void* ptrs[2] = {diffmap[i], rgb[i]};
+        const char* what[2] = {names[0].c_str(), names[1].c_str()};
+        check_device_pointers(who, device, ptrs, what, 2);
+      }
+    gb200::butteraugli_heatmap(w, h, diffmap, n, good, bad, rgb, on_device, device, caller_stream(stream));
+  });
+}
+}  // namespace
+
+int gb200_butteraugli_comparator_mask(gb200_butteraugli_comparator* c, float* mask, float* mask_dc) {
+  return comparator_mask(c, mask, mask_dc, false, nullptr);
+}
+
+int gb200_butteraugli_comparator_mask_device(gb200_butteraugli_comparator* c, float* mask_dev, float* mask_dc_dev,
+                                             void* stream) {
+  return comparator_mask(c, mask_dev, mask_dc_dev, true, stream);
+}
+
+int gb200_butteraugli_adaptive_quantization(const float* rgb, int w, int h, int device, float* quant) {
+  return adaptive_quantization(rgb, w, h, device, quant, false, nullptr);
+}
+
+int gb200_butteraugli_adaptive_quantization_device(const float* rgb_dev, int w, int h, int device, float* quant_dev,
+                                                   void* stream) {
+  return adaptive_quantization(rgb_dev, w, h, device, quant_dev, true, stream);
+}
+
+int gb200_butteraugli_heatmap(const int* w, const int* h, const float* const* diffmap, int n, double good, double bad,
+                              uint8_t* const* rgb, int device) {
+  return heatmap(w, h, diffmap, n, good, bad, rgb, device, false, nullptr);
+}
+
+int gb200_butteraugli_heatmap_device(const int* w, const int* h, const float* const* diffmap_dev, int n, double good,
+                                     double bad, uint8_t* const* rgb_dev, int device, void* stream) {
+  return heatmap(w, h, diffmap_dev, n, good, bad, rgb_dev, device, true, stream);
 }
 
 int gb200_jpeg_dimensions(const uint8_t* jpeg_in, size_t jpeg_len, int* width, int* height) {

@@ -728,6 +728,60 @@ struct SrgbToLinear {
   }
 };
 
+// ScoreToRgb's colour table (b/butteraugli.cc:1940), rows 0..9 as halves (0, 1 or 2) of r, g and b, six bits
+// a row; rows 10 and 11 are white
+constexpr unsigned long long heat_row(int row, int r, int g, int b) {
+  return static_cast<unsigned long long>(r | g << 2 | b << 4) << (6 * row);
+}
+constexpr unsigned long long kHeatHalves = heat_row(0, 0, 0, 0) | heat_row(1, 0, 0, 2) | heat_row(2, 0, 2, 2) |
+                                           heat_row(3, 0, 2, 0) | heat_row(4, 2, 2, 0) | heat_row(5, 2, 0, 0) |
+                                           heat_row(6, 2, 0, 2) | heat_row(7, 1, 1, 2) | heat_row(8, 2, 1, 1) |
+                                           heat_row(9, 2, 2, 1);
+GB_HD double heat_level(int row, int c) {
+  return 0.5 * (row >= 10 ? 2 : static_cast<int>((kHeatHalves >> (6 * row + 2 * c)) & 3));
+}
+
+// ScoreToRgb (b/butteraugli.cc:1938) in its double arithmetic and order, up to v.  Its byte
+// (uint8_t)(255 * pow(v, 0.5) + 0.5) is the largest k with steps[k] <= v, steps the host-pow table
+// heat_byte_steps() (tables.h): IEEE sqrt differs from the host's pow in one byte (DESIGN.md §3).  NaN scores have
+// no defined colour.
+GB_HD void score_to_rgb(double score, double good, double bad, const double* steps, uint8_t* rgb) {
+  if (score < good) {
+    score = (score / good) * 0.3;
+  } else if (score < bad) {
+    score = 0.3 + (score - good) / (bad - good) * 0.15;
+  } else {
+    score = 0.45 + (score - bad) / (bad * 12) * 0.5;
+  }
+  score = hd_min<double>(hd_max<double>(score * 11, 0.0), 10);
+  const int ix = static_cast<int>(score);
+  const double mix = score - ix;
+  for (int i = 0; i < 3; ++i) {
+    const double v = mix * heat_level(ix + 1, i) + (1 - mix) * heat_level(ix, i);
+    int k = 0;
+    for (int step = 128; step > 0; step >>= 1)
+      if (k + step <= 255 && steps[k + step] <= v) k += step;
+    rgb[i] = static_cast<uint8_t>(k);
+  }
+}
+
+// CreateHeatMapImage (b/butteraugli.cc:1979) of n diffmaps of sizes of their own, flat over all their pixels:
+// pixel i of the call is pixel i - px0[f] of map f = jpeg_find(px0, n, i), map f [h][w] floats into rgb[f]
+// [h][w][3] bytes.
+struct HeatMap {
+  const float* const* dm;
+  uint8_t* const* rgb;
+  const int* px0;        // [n + 1]
+  const double* steps;   // [256] heat_byte_steps()
+  int n;
+  double good, bad;
+  GB_HD void operator()(int i) const {
+    const int f = jpeg_find(px0, n, i);
+    const int p = i - px0[f];
+    score_to_rgb(dm[f][p], good, bad, steps, rgb[f] + 3 * static_cast<size_t>(p));
+  }
+};
+
 // a8: ApplyGlobalQuantization on top of CopyFromJpegData with unit quant
 // (g/output_image.cc:211-243): cand = Quantize(orig, q[c][k]).
 struct QuantizeCoeffs {

@@ -885,26 +885,27 @@ void Butteraugli::fused_mixed_run(const int* w, const int* h, const std::vector<
 }
 
 void Butteraugli::analyse_originals(const int* w, const int* h, const int* channels, const void* const* img0, int n,
-                                    int background, float* const* store) {
+                                    int background, float* const* store, bool device) {
   check_sizes(w, h, n);
   bind();
   if (mixed_ == nullptr) mixed_ = new Mixed();
   Mixed& mx = *mixed_;
   if (channels != nullptr && t_.srgb_lin == nullptr) t_.srgb_lin = upload_srgb_lin(s_, &owned_, nullptr);
-  // the originals packed and uploaded in one copy
-  std::vector<size_t> at(n + 1, 0);
-  for (int i = 0; i < n; ++i)
-    at[i + 1] = at[i] + static_cast<size_t>(w[i]) * h[i] * (channels != nullptr ? channels[i] : 3 * sizeof(float));
-  mx.stage_in = grow(mx.stage_in, &mx.stage_in_bytes, at[n]);
-  mx.host_in.resize(at[n]);
-  std::vector<const void*> p0(n);
+  std::vector<const void*> p0(img0, img0 + n);
   std::vector<int> all(n);
-  for (int i = 0; i < n; ++i) {
-    memcpy(&mx.host_in[at[i]], img0[i], at[i + 1] - at[i]);
-    p0[i] = mx.stage_in + at[i];
-    all[i] = i;
+  for (int i = 0; i < n; ++i) all[i] = i;
+  if (!device) {  // the originals packed and uploaded in one copy
+    std::vector<size_t> at(n + 1, 0);
+    for (int i = 0; i < n; ++i)
+      at[i + 1] = at[i] + static_cast<size_t>(w[i]) * h[i] * (channels != nullptr ? channels[i] : 3 * sizeof(float));
+    mx.stage_in = grow(mx.stage_in, &mx.stage_in_bytes, at[n]);
+    mx.host_in.resize(at[n]);
+    for (int i = 0; i < n; ++i) {
+      memcpy(&mx.host_in[at[i]], img0[i], at[i + 1] - at[i]);
+      p0[i] = mx.stage_in + at[i];
+    }
+    h2d(mx.stage_in, mx.host_in.data(), at[n], s_);
   }
-  h2d(mx.stage_in, mx.host_in.data(), at[n], s_);
   MixSrc src;
   src.img[0] = p0.data();
   src.channels = channels;
@@ -961,14 +962,23 @@ void Butteraugli::mask_planes(const float* xy) {
         "mask_planes");
 }
 
-void Butteraugli::mask(float* mask, float* mask_dc) {
+void Butteraugli::mask(float* mask, float* mask_dc, bool device, Stream caller) {
   bind();
+  if (device) stream_wait(s_, caller);
   // MaskPsychoImage(pi0_, pi0_) (b/butteraugli.cc:753): the mixed X and Y planes go to xyb_, which
   // every Compare rewrites before reading it
   r_.px(MaskPsychoMix{ps0_, xyb_, g_}, "mask_psycho_mix");
   mask_planes(xyb_);
-  r_.download_planes(mask_, mask, 3);
-  r_.download_planes(mask_ + 3 * g_.plane, mask_dc, 3);
+  if (!device) {
+    r_.download_planes(mask_, mask, 3);
+    r_.download_planes(mask_ + 3 * g_.plane, mask_dc, 3);
+    return;
+  }
+  // [3][h][pitch] -> [3][h][w], each group as 3h rows
+  const size_t row = sizeof(float) * g_.w, pitch = sizeof(float) * g_.pitch, rows = static_cast<size_t>(3) * g_.h;
+  d2d_2d(mask, row, mask_, pitch, row, rows, s_);
+  d2d_2d(mask_dc, row, mask_ + 3 * g_.plane, pitch, row, rows, s_);
+  stream_sync(s_);
 }
 
 void Butteraugli::srgb_to_linear(const uint8_t* src, int n, int channels, int background, float* dst, int pitch) {
@@ -3131,6 +3141,60 @@ void jpeg_decode_rgb(const JpegInput* const* files, int n, int device, uint8_t* 
   jpeg_idct_upsample(s, d_tab, d_blk0, d_row0, d_quant, d_coeffs, d_samples, n, L);
   if (!out_on_device)
     for (int i = 0; i < n; ++i) d2h(out[i], tab[i].out, static_cast<size_t>(3) * tab[i].w * tab[i].h, s);
+  stream_sync(s);
+}
+
+// ---------------------------------------------------------------------------
+// Heat maps (HeatMap in kernels.h)
+void butteraugli_heatmap(const int* w, const int* h, const float* const* diffmap, int n, double good, double bad,
+                         uint8_t* const* rgb, bool on_device, int device, Stream stream) {
+  std::vector<int> px0(n + 1, 0);
+  for (int i = 0; i < n; ++i) {
+    const long long end = px0[i] + static_cast<long long>(w[i]) * h[i];
+    if (end > 0x7fffffffLL) throw std::runtime_error("butteraugli heatmap: more than 2^31 - 1 pixels in one call");
+    px0[i + 1] = static_cast<int>(end);
+  }
+  const size_t total = static_cast<size_t>(px0[n]);
+  JpegScope sc;  // a stream and buffers, handed back on every path
+  sc.open(device);
+  const Stream s = sc.s;
+  std::vector<const float*> in(diffmap, diffmap + n);
+  std::vector<uint8_t*> out(rgb, rgb + n);
+  uint8_t* staged = nullptr;
+  if (on_device) {
+    stream_wait(s, stream);
+  } else {  // the maps packed and uploaded in one copy, the heat maps back in one
+    std::vector<float> packed(total);
+    for (int i = 0; i < n; ++i) memcpy(&packed[px0[i]], diffmap[i], sizeof(float) * (px0[i + 1] - px0[i]));
+    float* d_in = sc.alloc_n<float>(total);
+    h2d(d_in, packed.data(), sizeof(float) * total, s);
+    staged = sc.alloc_n<uint8_t>(3 * total);
+    for (int i = 0; i < n; ++i) {
+      in[i] = d_in + px0[i];
+      out[i] = staged + 3 * static_cast<size_t>(px0[i]);
+    }
+  }
+  // one table: the byte steps, input pointers, output pointers, first pixels
+  const std::vector<double>& steps = heat_byte_steps();
+  const size_t at_in = sizeof(double) * steps.size(), ptrs = sizeof(void*) * n, at_px0 = at_in + 2 * ptrs;
+  std::vector<unsigned char> tab(at_px0 + sizeof(int) * (n + 1));
+  memcpy(tab.data(), steps.data(), at_in);
+  memcpy(tab.data() + at_in, in.data(), ptrs);
+  memcpy(tab.data() + at_in + ptrs, out.data(), ptrs);
+  memcpy(tab.data() + at_px0, px0.data(), sizeof(int) * (n + 1));
+  unsigned char* d_tab = sc.alloc_n<unsigned char>(tab.size());
+  h2d(d_tab, tab.data(), tab.size(), s);
+  launch_1d(s,
+            HeatMap{reinterpret_cast<const float* const*>(d_tab + at_in),
+                    reinterpret_cast<uint8_t* const*>(d_tab + at_in + ptrs), reinterpret_cast<const int*>(d_tab + at_px0),
+                    reinterpret_cast<const double*>(d_tab), n, good, bad},
+            px0[n], "butteraugli_heatmap");
+  if (!on_device) {
+    std::vector<uint8_t> back(3 * total);
+    d2h(back.data(), staged, back.size(), s);
+    for (int i = 0; i < n; ++i)
+      memcpy(rgb[i], &back[3 * static_cast<size_t>(px0[i])], 3 * static_cast<size_t>(px0[i + 1] - px0[i]));
+  }
   stream_sync(s);
 }
 

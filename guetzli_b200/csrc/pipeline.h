@@ -25,6 +25,13 @@ struct JpegInput;
 void jpeg_decode_rgb(const JpegInput* const* files, int n, int device, uint8_t* const* out, bool out_on_device,
                      Stream stream);
 
+// CreateHeatMapImage (b/butteraugli.cc:1979) of n diffmaps, map i [h[i]][w[i]] floats into rgb[i] [h[i]][w[i]][3]
+// bytes, with one launch of HeatMap (kernels.h) on `device` for all of them.  Host maps go up in one copy and
+// come back in one; with on_device, diffmap[i] and rgb[i] are memory of `device`, read after the work queued on
+// `stream` so far.  Either way the outputs are written when this returns.
+void butteraugli_heatmap(const int* w, const int* h, const float* const* diffmap, int n, double good, double bad,
+                         uint8_t* const* rgb, bool on_device, int device, Stream stream);
+
 // Subsequence length, in bits, of the speculative Huffman decode (JpegHuffSync in kernels.h).
 constexpr int kJpegSubBits = 1024;
 

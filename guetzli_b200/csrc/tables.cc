@@ -63,6 +63,31 @@ const int* natural_to_zigzag() {
   return zz.to_zigzag;
 }
 
+const std::vector<double>& heat_byte_steps() {
+  static const std::vector<double> steps = [] {
+    const auto byte_of = [](uint64_t bits) {
+      double v;
+      memcpy(&v, &bits, sizeof(v));
+      return static_cast<uint8_t>(255 * pow(v, 0.5) + 0.5);
+    };
+    // bisection on the bit patterns, which order non-negative doubles as their values: byte_of(lo) < k <= byte_of(hi)
+    uint64_t zero = 0, one;
+    const double d1 = 1.0;
+    memcpy(&one, &d1, sizeof(one));
+    std::vector<double> t(256, 0.0);
+    for (int k = 1; k <= 255; ++k) {
+      uint64_t lo = zero, hi = one;
+      while (hi - lo > 1) {
+        const uint64_t mid = lo + (hi - lo) / 2;
+        (byte_of(mid) >= k ? hi : lo) = mid;
+      }
+      memcpy(&t[k], &hi, sizeof(double));
+    }
+    return t;
+  }();
+  return steps;
+}
+
 double distance_for_quality(double quality) {
   // quality.cc:78 -- clamp to [70,110], linear interpolation between integers.
   if (quality < 70) quality = 70;

@@ -88,5 +88,9 @@ const float* upload_srgb_lin(Stream s, std::vector<void*>* owned, HostTables* ho
 const int* zigzag_to_natural();  // [64] JPEG zig-zag scan position -> natural index
 const int* natural_to_zigzag();  // [64] inverse
 double distance_for_quality(double quality);  // quality.cc:78
+// ScoreToRgb's output byte (uint8_t)(255 * pow(v, 0.5) + 0.5) (butteraugli.cc:1973) as steps: [k], k = 1..255,
+// is the least double v in [0, 1] whose byte is at least k, found with the host's pow; [0] is 0.  The byte of v
+// is then the largest k with steps[k] <= v (HeatMap, kernels.h).
+const std::vector<double>& heat_byte_steps();
 
 }  // namespace gb200

@@ -133,6 +133,11 @@ int gb200_butteraugli_comparator_diffmap_device(gb200_butteraugli_comparator* c,
                                                 float* diffmap_dev, double* score, void* stream);
 /* ButteraugliComparator::Mask (butteraugli.cc:793): mask and mask_dc, [3][h][w] each, host memory. */
 int gb200_butteraugli_comparator_mask(gb200_butteraugli_comparator* c, float* mask, float* mask_dc);
+/* The same into mask_dev and mask_dc_dev, device memory of the comparator's device, written after the work
+ * queued on `stream` so far and written when the call returns.  A host pointer or memory of another device is
+ * refused, nothing runs. */
+int gb200_butteraugli_comparator_mask_device(gb200_butteraugli_comparator* c, float* mask_dev, float* mask_dc_dev,
+                                             void* stream);
 void gb200_butteraugli_comparator_destroy(gb200_butteraugli_comparator* c);
 /* A comparator that scores up to `capacity` images per call against its original, all of them in one
  * pass of the Compare chain, one launch per stage; the original is analysed once, here (DESIGN.md §4).
@@ -141,6 +146,13 @@ void gb200_butteraugli_comparator_destroy(gb200_butteraugli_comparator* c);
  * failure (gb200_last_error), with nothing left allocated. */
 gb200_butteraugli_comparator* gb200_butteraugli_comparator_create_batch(const float* rgb0, int w, int h, int capacity,
                                                                         int device);
+/* The same comparator made from an original rgb0_dev [3][h][w] in device memory of `device`, read after the
+ * work queued on `stream` so far (a cudaStream_t, NULL = the legacy default stream) and copied on the device:
+ * no pixel crosses PCIe.  The caller may free or overwrite rgb0_dev once this returns.  A host, managed or
+ * other device's pointer is refused, nothing runs.  NULL on failure, with nothing left allocated; otherwise
+ * the comparator is the one gb200_butteraugli_comparator_create_batch makes, bit for bit. */
+gb200_butteraugli_comparator* gb200_butteraugli_comparator_create_device(const float* rgb0_dev, int w, int h,
+                                                                         int capacity, int device, void* stream);
 /* ButteraugliComparator::Diffmap (butteraugli.cc:799) and ButteraugliScoreFromDiffmap (butteraugli.cc:1623)
  * for each image: rgb1 [n][3][h][w] in host memory, 1 <= n <= capacity; diffmap (may be NULL) receives
  * [n][h][w], score (may be NULL) [n], the maximum of each diffmap.  Each image gets the bits that
@@ -237,6 +249,11 @@ int gb200_butteraugli_batch_diffmap_sizes_srgb_device(gb200_butteraugli_batch* b
  * entries below); the float entries refuse it, and gb200_butteraugli_comparator_mask refuses an RGBA one. */
 gb200_butteraugli_comparator* gb200_butteraugli_comparator_create_srgb(const uint8_t* img0, int w, int h, int channels,
                                                                        int capacity, int device);
+/* The same from img0_dev [h][w][channels] in device memory of `device`, converted where it lies after the
+ * work queued on `stream` so far, as gb200_butteraugli_comparator_create_device reads its original. */
+gb200_butteraugli_comparator* gb200_butteraugli_comparator_create_srgb_device(const uint8_t* img0_dev, int w, int h,
+                                                                              int channels, int capacity, int device,
+                                                                              void* stream);
 /* img1 [n][h][w][channels] in host memory, 1 <= n <= capacity; diffmap (may be NULL) [n][h][w], score
  * (may be NULL) [n].  A comparator made from float planes refuses it. */
 int gb200_butteraugli_comparator_diffmap_srgb(gb200_butteraugli_comparator* c, const uint8_t* img1, int n,
@@ -268,6 +285,18 @@ gb200_butteraugli_comparator_set* gb200_butteraugli_comparator_set_create_srgb(c
                                                                                const int* channels,
                                                                                const uint8_t* const* img0, int count,
                                                                                int capacity, int device);
+/* The same two with the originals in device memory of `device` (w, h and channels stay host arrays), read in
+ * place by the packing launch after the work queued on `stream` so far (a cudaStream_t, NULL = the legacy
+ * default stream), in the same mixed passes as from host memory.  The caller may free or overwrite them once
+ * this returns.  A host, managed or other device's pointer is refused, naming it (rgb0[i] / img0[i]), and
+ * nothing runs.  The set is the one the host entry makes, bit for bit. */
+gb200_butteraugli_comparator_set* gb200_butteraugli_comparator_set_create_device(const int* w, const int* h,
+                                                                                 const float* const* rgb0_dev,
+                                                                                 int count, int capacity, int device,
+                                                                                 void* stream);
+gb200_butteraugli_comparator_set* gb200_butteraugli_comparator_set_create_srgb_device(
+    const int* w, const int* h, const int* channels, const uint8_t* const* img0_dev, int count, int capacity,
+    int device, void* stream);
 /* original: host array [n]; rgb1[i]: [3][h][w] of original[i]'s size, in host memory; diffmap (may be NULL,
  * and so may its entries) [i]: [h][w]; score (may be NULL) [n].  A set made from 8-bit images refuses it. */
 int gb200_butteraugli_comparator_set_diffmap(gb200_butteraugli_comparator_set* s, const int* original,
@@ -293,6 +322,25 @@ void gb200_butteraugli_comparator_set_destroy(gb200_butteraugli_comparator_set* 
 /* butteraugli::ButteraugliAdaptiveQuantization (butteraugli.cc:1880): the Y plane of Mask(rgb, rgb),
  * [h][w] into quant.  rgb in host memory.  Fails below 16x16, where the reference returns false. */
 int gb200_butteraugli_adaptive_quantization(const float* rgb, int w, int h, int device, float* quant);
+/* The same with rgb_dev [3][h][w] and quant_dev [h][w] in device memory of `device`, read and written after the
+ * work queued on `stream` so far; quant_dev is written when the call returns.  A host, managed or other device's
+ * pointer is refused, nothing runs. */
+int gb200_butteraugli_adaptive_quantization_device(const float* rgb_dev, int w, int h, int device, float* quant_dev,
+                                                   void* stream);
+
+/* butteraugli::CreateHeatMapImage (butteraugli.cc:1979) of n maps of sizes of their own, on `device`, with one
+ * launch for all of them: diffmap[i] [h[i]][w[i]] floats -> rgb[i] [h[i]][w[i]][3] bytes, the reference's
+ * ScoreToRgb bytes exactly.  The butteraugli tool's thresholds are good = ButteraugliFuzzyInverse(1.5) and
+ * bad = ButteraugliFuzzyInverse(0.5) (butteraugli_main.cc:423-424); any 0 < good < bad is taken, anything
+ * else refused.  Maps are at least 1x1, at most 2^31 - 1 pixels in all.  Host memory here, uploaded in one
+ * copy; the heat maps come back in one.  A NaN in a map has no defined colour.  Returns 1 on success. */
+int gb200_butteraugli_heatmap(const int* w, const int* h, const float* const* diffmap, int n, double good, double bad,
+                              uint8_t* const* rgb, int device);
+/* The same with diffmap_dev[i] and rgb_dev[i] in device memory of `device` (w, h stay host arrays), read and
+ * written after the work queued on `stream` so far, written when the call returns.  A host, managed or other
+ * device's pointer is refused, nothing runs. */
+int gb200_butteraugli_heatmap_device(const int* w, const int* h, const float* const* diffmap_dev, int n, double good,
+                                     double bad, uint8_t* const* rgb_dev, int device, void* stream);
 
 /* ReadJpeg(JPEG_READ_HEADER) as the CLI uses it (guetzli/guetzli.cc:306): frame size only. */
 int gb200_jpeg_dimensions(const uint8_t* jpeg_in, size_t jpeg_len, int* width, int* height);

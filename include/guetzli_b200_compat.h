@@ -211,6 +211,23 @@ inline bool ButteraugliAdaptiveQuantization(size_t xsize, size_t ysize, const st
   return true;
 }
 
+// butteraugli::CreateHeatMapImage (butteraugli.cc:1979), same arguments: *heatmap is resized to 3 * xsize * ysize
+// and receives the reference's bytes.  The butteraugli tool passes good = ButteraugliFuzzyInverse(1.5) and
+// bad = ButteraugliFuzzyInverse(0.5).  The device is GUETZLI_B200_DEVICE (environment), default 0.  False where
+// the reference's behaviour is undefined or the call fails: distmap not xsize * ysize, an empty map, thresholds
+// not 0 < good < bad.
+inline bool CreateHeatMapImage(const std::vector<float>& distmap, double good_threshold, double bad_threshold,
+                               size_t xsize, size_t ysize, std::vector<uint8_t>* heatmap) {
+  if (xsize < 1 || ysize < 1 || xsize >= 65536 || ysize >= 65536 || distmap.size() != xsize * ysize) return false;
+  int device = 0;
+  if (const char* e = getenv("GUETZLI_B200_DEVICE")) device = atoi(e);
+  heatmap->resize(3 * xsize * ysize);
+  const int w = static_cast<int>(xsize), h = static_cast<int>(ysize);
+  const float* in = distmap.data();
+  uint8_t* out = heatmap->data();
+  return gb200_butteraugli_heatmap(&w, &h, &in, 1, good_threshold, bad_threshold, &out, device) != 0;
+}
+
 }  // namespace guetzli_b200
 
 #endif  // GUETZLI_B200_COMPAT_H_

@@ -66,7 +66,14 @@ every round:
                     per original
 
 It reports the device memory each holds after gb200_trim_memory, the bytes each host mode uploads per
-candidate, and whether every mode's scores are equal."""
+candidate, and whether every mode's scores are equal.
+
+With --device-originals, the originals of the same sweeps go into a ComparatorSet from numpy arrays and from CUDA
+tensors (8-bit sRGB, the kodak sweep with alpha on every other original), and the two are timed alternately: ms per
+set made (the set's device memory is reused through the library's cache after the first), the host-to-device and
+device-to-host bytes of each, and whether both sets score a call of candidates alike.  Then heat maps of the tool's
+thresholds: one 1920x1080 map and 64 such maps in one call, from CUDA tensors and from numpy arrays, against the
+reference's host loop (butteraugli::CreateHeatMapImage through oracle/_ref, where build() made it)."""
 import argparse
 import json
 import os
@@ -115,6 +122,8 @@ def main():
                     help="pairs per call of a set whose largest size is 1920x1080 (the arena of 256 such slots "
                          "does not fit in 80 GB)")
     ap.add_argument("--set", action="store_true", help="time the comparator-set sweeps and nothing else")
+    ap.add_argument("--device-originals", action="store_true",
+                    help="time set creation from host arrays against CUDA tensors, and heat maps, and nothing else")
     ap.add_argument("--out", default=None, help="also write the JSON result here")
     args = ap.parse_args()
 
@@ -125,6 +134,11 @@ def main():
     dev = torch.device("cuda", args.device)
     torch.cuda.set_device(dev)
 
+    if args.device_originals:
+        result = {"device_originals": bench_device_originals(args, dev, torch), "heatmap": bench_heatmap(args, dev, torch)}
+        result.update(gpu_info(args.device))
+        emit(result, args.out)
+        return
     if args.set:
         result = {"set": bench_set(args, dev, torch)}
         result.update(gpu_info(args.device))
@@ -536,6 +550,81 @@ def bench_set(args, dev, torch):
                      "h2d_kib_per_candidate": {m: round(h2d[m] / 1024, 1) for m in ("set_host", "sizes_host")},
                      "scores_identical": all(v == scores["set_cuda"] for v in scores.values()),
                      "device_memory": memory}
+    return out
+
+
+def bench_device_originals(args, dev, torch):
+    out = {}
+    for name, (shapes, _) in set_workloads().items():
+        orig = [synth.gradnoise(h, w, 100 + i) for i, (h, w) in enumerate(shapes)]
+        if name == "kodak":
+            orig = [np.ascontiguousarray(np.dstack([x, synth.noise(x.shape[0], x.shape[1], 7)[..., :1]]))
+                    if i % 2 else x for i, x in enumerate(orig)]
+        orig_dev = [torch.from_numpy(x).to(dev) for x in orig]
+        cap = min(args.sizes_capacity, len(orig))
+        index = list(range(cap))
+        cands = [orig_dev[i].flip(1).contiguous() for i in index]
+        torch.cuda.synchronize(dev)
+        modes = {"from_host": orig, "from_cuda": orig_dev}
+        moved, scores = {}, {}
+        for m, src in modes.items():  # also the warm-up
+            c0 = gb.counters()
+            s = gb.ComparatorSet.from_srgb(src, capacity=cap, device=args.device)
+            torch.cuda.synchronize(dev)
+            c1 = gb.counters()
+            moved[m] = {"h2d_bytes": c1[1] - c0[1], "d2h_bytes": c1[2] - c0[2]}
+            scores[m] = s.diffmap(index, cands)[1].tolist()
+            s.close()
+        ms = {m: [] for m in modes}
+        for _ in range(args.rounds):
+            for m, src in modes.items():
+                torch.cuda.synchronize(dev)
+                t0 = time.perf_counter()
+                s = gb.ComparatorSet.from_srgb(src, capacity=cap, device=args.device)
+                torch.cuda.synchronize(dev)
+                ms[m].append((time.perf_counter() - t0) * 1e3)
+                s.close()
+        out[name] = {"originals": len(orig), "pixels": sum(x.shape[0] * x.shape[1] for x in orig),
+                     "input_bytes": sum(x.nbytes for x in orig), "capacity": cap,
+                     "ms_per_set": {m: {"median": round(statistics.median(v), 2), "min": round(min(v), 2),
+                                        "max": round(max(v), 2)} for m, v in ms.items()},
+                     "bytes_moved": moved, "scores_identical": scores["from_host"] == scores["from_cuda"]}
+    return out
+
+
+def bench_heatmap(args, dev, torch):
+    import ctypes as C
+    ref_path = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "oracle", "_ref", "libguetzli_ref.so")
+    ref = C.CDLL(ref_path) if os.path.exists(ref_path) else None
+    out = {}
+    for n in (1, 64):
+        maps = [(synth.noise(1080, 1920, 300 + i)[..., 0].astype(np.float32) / 64.0) for i in range(n)]
+        maps_dev = [torch.from_numpy(m).to(dev) for m in maps]
+        torch.cuda.synchronize(dev)
+        modes = {"cuda": lambda: gb.heatmap(maps_dev, device=args.device),
+                 "host_arrays": lambda: gb.heatmap(maps, device=args.device)}
+        rgb = np.empty((1080, 1920, 3), np.uint8)
+        if ref is not None:
+            def reference():
+                for m in maps:
+                    ref.gref_heatmap(m.ctypes.data, 1920, 1080, rgb.ctypes.data)
+            modes["reference_host_loop"] = reference
+        got = {m: f() for m, f in modes.items()}  # also the warm-up
+        same = all(np.array_equal(a.cpu().numpy(), b) for a, b in zip(got["cuda"], got["host_arrays"]))
+        if ref is not None:
+            ref.gref_heatmap(maps[-1].ctypes.data, 1920, 1080, rgb.ctypes.data)
+            same = same and np.array_equal(got["host_arrays"][-1], rgb)
+        ms = {m: [] for m in modes}
+        for _ in range(args.rounds):
+            for m, f in modes.items():
+                torch.cuda.synchronize(dev)
+                t0 = time.perf_counter()
+                f()
+                torch.cuda.synchronize(dev)
+                ms[m].append((time.perf_counter() - t0) * 1e3)
+        out[f"{n}x1920x1080"] = {"ms_per_call": {m: {"median": round(statistics.median(v), 2), "min": round(min(v), 2),
+                                                     "max": round(max(v), 2)} for m, v in ms.items()},
+                                 "bytes_identical": same, "reference": ref is not None}
     return out
 
 
