@@ -60,6 +60,7 @@ def load_library(path=None):
                                       C.c_void_p, P(P(C.c_uint8)), P(C.c_size_t), P(_CStats)]
     lib.gb200_process_jpeg.argtypes = [P(_CParams), C.c_void_p, C.c_size_t, C.c_int, _LOG_FN,
                                        C.c_void_p, P(P(C.c_uint8)), P(C.c_size_t), P(_CStats)]
+    lib.gb200_process_jpeg_from_device.argtypes = lib.gb200_process_jpeg.argtypes + [C.c_void_p]
     process_image = [P(_CParams), C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, _LOG_FN, C.c_void_p,
                      P(P(C.c_uint8)), P(C.c_size_t), P(_CStats)]
     lib.gb200_process_image.argtypes = process_image
@@ -111,6 +112,7 @@ def load_library(path=None):
                                                       C.c_void_p, C.c_void_p, C.c_void_p]
     lib.gb200_debug_entropy_decode.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_size_t,
                                                P(C.c_int)]
+    lib.gb200_debug_jpeg_seed.argtypes = lib.gb200_debug_entropy_decode.argtypes
     lib.gb200_butteraugli_diffmap.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                               P(C.c_double)]
     lib.gb200_butteraugli_comparator_create.restype = C.c_void_p
@@ -358,17 +360,35 @@ def process_image(params, stats, image, device=0, lib=None):
 
 def process_jpeg(params, stats, jpeg_in, device=0, lib=None):
     """guetzli::Process(params, stats, jpeg_in, &out) (processor.cc:890): JPEG input
-    (4:4:4 YCbCr).  Returns (ok, jpeg_bytes) like process()."""
+    (4:4:4 YCbCr).  Returns (ok, jpeg_bytes) like process().
+
+    jpeg_in: the file as a bytes-like object in host memory, encoded on cuda:`device`, or as a contiguous 1-D
+    torch.uint8 CUDA tensor, encoded on the tensor's own device after the work queued on that device's current
+    torch stream (gb200_process_jpeg_from_device: a sequential 4:4:4 file is Huffman-decoded there, and only
+    its bytes after EOI and one coefficient plane come back).  Both give the same result for the same bytes.
+    Other tensors raise ValueError."""
     lib = lib or load_library()
-    buf = np.frombuffer(bytes(jpeg_in), dtype=np.uint8)
     cp, cs = _cparams(params), _CStats()
     cb = _log_sink(stats)
     out, out_len = C.POINTER(C.c_uint8)(), C.c_size_t()
-    ok = lib.gb200_process_jpeg(C.byref(cp), buf.ctypes.data if buf.size else None, buf.size, device, cb, None,
-                                C.byref(out), C.byref(out_len), C.byref(cs))
+    if _is_torch_tensor(jpeg_in):
+        import torch
+        t = jpeg_in
+        if not t.is_cuda or t.dtype != torch.uint8 or t.dim() != 1 or not t.is_contiguous():
+            raise ValueError(f"process_jpeg: the file must be a contiguous 1-D torch.uint8 CUDA tensor, got "
+                             f"{t.dtype} {tuple(t.shape)} on {t.device}")
+        ok = lib.gb200_process_jpeg_from_device(C.byref(cp), t.data_ptr() if t.numel() else None, t.numel(),
+                                                t.device.index, cb, None, C.byref(out), C.byref(out_len),
+                                                C.byref(cs), torch.cuda.current_stream(t.device).cuda_stream)
+    else:
+        buf = np.frombuffer(bytes(jpeg_in), dtype=np.uint8)
+        ok = lib.gb200_process_jpeg(C.byref(cp), buf.ctypes.data if buf.size else None, buf.size, device, cb, None,
+                                    C.byref(out), C.byref(out_len), C.byref(cs))
     data = _take(lib, out, out_len)
     _fill_stats(stats, cs)
     if not ok and not data:
+        if "device memory" in _err(lib):  # a pointer the device entry refused
+            raise RuntimeError(_err(lib))
         _raise_device_error(lib)
     return bool(ok), data
 
@@ -476,6 +496,21 @@ def entropy_decode(jpeg_in, S, lib=None, cap=1 << 24):
                                           C.byref(status)):
         raise RuntimeError(_err(lib))
     return bool(status.value), (out if status.value else None)
+
+
+def jpeg_seed(jpeg_in, S, lib=None, cap=1 << 24):
+    """The seeding of process_jpeg's device route on one file with subsequences of S bits (test hook) ->
+    (route, dq): route 0 where the file goes to the host route, 1 where the device route takes it and it is
+    sane, 2 where it is taken and fails the sanity check; dq the [3][blocks][64] coefficients times their
+    quant steps (int16) at the start of a buffer of cap values, or None for route 0."""
+    lib = lib or load_library()
+    buf = np.frombuffer(bytes(jpeg_in), dtype=np.uint8)
+    out = np.zeros(cap, dtype=np.int16)
+    status = C.c_int()
+    if not lib.gb200_debug_jpeg_seed(buf.ctypes.data if buf.size else None, buf.size, S, out.ctypes.data, cap,
+                                     C.byref(status)):
+        raise RuntimeError(_err(lib))
+    return status.value, (out if status.value else None)
 
 
 def read_jpeg(jpeg_in, lib=None, cap=1 << 24):

@@ -342,6 +342,27 @@ int gb200_process_jpeg(const gb200_params* params, const uint8_t* jpeg_in, size_
   return (guarded_ok && ok) ? 1 : 0;
 }
 
+int gb200_process_jpeg_from_device(const gb200_params* params, const uint8_t* jpeg_dev, size_t jpeg_len, int device,
+                                   gb200_log_fn log, void* log_user, uint8_t** out, size_t* out_len,
+                                   gb200_stats* stats, void* stream) {
+  *out = nullptr;
+  *out_len = 0;
+  bool ok = false;
+  int guarded_ok = guarded([&]() {
+    // an empty file may have no bytes at all; it is then refused as gb200_process_jpeg refuses it
+    const void* ptrs[1] = {jpeg_len ? jpeg_dev : nullptr};
+    const char* what[1] = {"jpeg"};
+    check_device_pointers("process_jpeg_from_device", device, ptrs, what, 1);
+    gb200::SearchStats st;
+    std::string jpeg, err;
+    ok = gb200::process_jpeg_from_device(to_search_params(params), jpeg_dev, jpeg_len, device, caller_stream(stream),
+                                         log, log_user, &jpeg, &st, &err);
+    if (!ok) g_err = err;
+    take_jpeg(jpeg, st, out, out_len, stats);
+  });
+  return (guarded_ok && ok) ? 1 : 0;
+}
+
 // butteraugli::ButteraugliInterface (b/butteraugli.cc:1858) on the device kernels.
 int gb200_butteraugli_diffmap(const float* rgb0, const float* rgb1, int w, int h, int device, float* diffmap,
                               double* score) {
@@ -1093,6 +1114,18 @@ int gb200_debug_entropy_decode(const uint8_t* jpeg_in, size_t jpeg_len, int S, i
       if (c.size() > out_cap) throw std::runtime_error("debug_entropy_decode: out is too small");
       memcpy(out, c.data(), c.size() * sizeof(int16_t));
     }
+  });
+}
+
+int gb200_debug_jpeg_seed(const uint8_t* jpeg_in, size_t jpeg_len, int S, int16_t* dq, size_t dq_cap, int* status) {
+  return guarded([&]() {
+    if (jpeg_in == nullptr || dq == nullptr || status == nullptr)
+      throw std::runtime_error("debug_jpeg_seed: null argument");
+    if (S < 8) throw std::runtime_error("debug_jpeg_seed: subsequences of fewer than 8 bits");
+    std::vector<int16_t> c;
+    *status = gb200::jpeg_debug_seed_route(jpeg_in, jpeg_len, S, &c);
+    if (c.size() > dq_cap) throw std::runtime_error("debug_jpeg_seed: dq is too small");
+    memcpy(dq, c.data(), c.size() * sizeof(int16_t));
   });
 }
 

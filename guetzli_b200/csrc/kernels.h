@@ -679,6 +679,24 @@ struct JpegRangeCheck {
   }
 };
 
+// The encoder's JPEG input from one device-decoded 4:4:4 file, per coefficient of [3][nblocks][64]:
+// RemoveOriginalQuantization (g/processor.cc:82), dq = coef * q, and CheckJpegSanity's bound (:106),
+// |coef * q| <= 4096 as a 64-bit product, whose breach flags the file (kJpegBadSanity).  The int16 store
+// is exact wherever the bound holds, and the encoder reads dq only then.
+constexpr unsigned kJpegBadSanity = 16u;
+struct JpegDequantSanity {
+  const int16_t* coeffs;  // [3][nblocks][64], quantised, natural order
+  const int* quant;       // [3][64], natural order
+  int nblocks;
+  int16_t* dq;
+  unsigned* status;
+  GB_HD void operator()(int i) const {
+    const long long v = static_cast<long long>(coeffs[i]) * quant[(i / (64 * nblocks)) * 64 + (i & 63)];
+    dq[i] = static_cast<int16_t>(v);
+    if (v > 4096 || v < -4096) hd_atomic_or(status, kJpegBadSanity);
+  }
+};
+
 // Original image u8 sRGB -> linear float planes (g/butteraugli_comparator.cc:33).
 struct LinearizeRgb {
   const uint8_t* rgb;

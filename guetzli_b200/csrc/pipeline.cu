@@ -12,6 +12,7 @@
 
 #include <algorithm>
 #include <map>
+#include <memory>
 #include <stdexcept>
 
 #include "block_math.h"
@@ -1073,6 +1074,14 @@ ImageContext::ImageContext(const int16_t* dq_coeffs, int w, int h, int device, b
   guarded_init(nullptr, dq_coeffs, prepare_now);
 }
 
+ImageContext::ImageContext(const int16_t* dq_dev, Stream stream, int w, int h, int device, bool prepare_now)
+    : ba_(w, h, device, nullptr) {
+  from_coeffs_ = true;
+  dq_on_device_ = true;
+  dq_stream_ = stream;
+  guarded_init(nullptr, dq_dev, prepare_now);
+}
+
 ImageContext::ImageContext(const ImageView& view, int w, int h, int device, bool prepare_now)
     : ba_(w, h, device, nullptr) {
   guarded_init(nullptr, nullptr, prepare_now, &view);
@@ -1148,8 +1157,11 @@ void ImageContext::init(const uint8_t* rgb, const int16_t* dq_coeffs, bool prepa
   render_all_ = true;
   num_dirty_ = 0;
   d_dirty_ = static_cast<int*>(own(sizeof(int) * g_.nblocks));
-  if (from_coeffs_) {
-    h2d(d_orig_, dq_coeffs, static_cast<size_t>(3) * g_.nblocks * 64 * sizeof(int16_t), s_);
+  if (dq_on_device_) {
+    stream_wait(s_, dq_stream_);
+    d2d(d_orig_, dq_coeffs, ncoef * sizeof(int16_t), s_);
+  } else if (from_coeffs_) {
+    h2d(d_orig_, dq_coeffs, ncoef * sizeof(int16_t), s_);
   } else if (view != nullptr) {
     ingest(*view);
   } else {
@@ -3286,9 +3298,11 @@ struct JpegDeviceFile {
 };
 
 // Entropy-decodes the files into d_coeffs (zeroed, laid out as `layout` says) on s; d_status[i] receives
-// the kJpegBad* flags of file i.  Returns the number of synchronisation rounds after the first.
+// the kJpegBad* flags of file i, and d_end[i] (if given; else scratch) the offset of the marker that ends
+// file i's scan data, EOI where no kJpegBadSegment is raised.  Returns the number of synchronisation rounds
+// after the first.
 int jpeg_entropy_decode(const std::vector<JpegDeviceFile>& fs, int16_t* d_coeffs, int S, Stream s, JpegScope* sc,
-                        unsigned* d_status) {
+                        unsigned* d_status, unsigned* d_end = nullptr) {
   const int n = static_cast<int>(fs.size());
   if (n == 0) return 0;
   if (S < 8) throw std::runtime_error("jpeg entropy decode: subsequences of fewer than 8 bits");
@@ -3384,7 +3398,7 @@ int jpeg_entropy_decode(const std::vector<JpegDeviceFile>& fs, int16_t* d_coeffs
   JpegScanFile* d_tab = sc->alloc_n<JpegScanFile>(n);
   int* d_byte0 = sc->alloc_n<int>(n + 1);
   int* d_int0 = sc->alloc_n<int>(n + 1);
-  unsigned* d_end = sc->alloc_n<unsigned>(n);
+  if (d_end == nullptr) d_end = sc->alloc_n<unsigned>(n);
   JpegHuffDev* d_luts = sc->alloc_n<JpegHuffDev>(luts.size());
   uint8_t* d_zz = sc->alloc_n<uint8_t>(64);
   unsigned* keep = sc->alloc_n<unsigned>(B + 1);
@@ -3477,7 +3491,116 @@ std::string jpeg_host_check(const std::vector<uint8_t>& b, int width, int height
 }
 
 constexpr size_t kJpegFirstPrefix = 4096;
+
+// The headers of n files in device memory (read_jpeg_header), from prefixes copied to the host on s, 4 KiB
+// doubling; each round covers every file still short of its first SOS.  (*head_ok)[i] where file i's was read.
+void jpeg_read_headers(const uint8_t* const* jpeg, const size_t* len, int n, Stream s, std::vector<JpegScanHeader>* hdr,
+                       std::vector<std::vector<uint8_t> >* pre, std::vector<char>* head_ok) {
+  std::vector<char> pending(n, 1);
+  for (size_t m = kJpegFirstPrefix;; m *= 2) {
+    bool more = false;
+    for (int i = 0; i < n; ++i) {
+      if (!pending[i]) continue;
+      const size_t k = std::min(m, len[i]);
+      std::vector<uint8_t>& p = (*pre)[i];
+      p.resize(k);
+      if (k) d2h(p.data(), jpeg[i], k, s);
+      if (read_jpeg_header(p.data(), k, &(*hdr)[i])) {
+        (*head_ok)[i] = 1;
+        pending[i] = 0;
+      } else if (k == len[i]) {
+        pending[i] = 0;
+      } else {
+        more = true;
+      }
+    }
+    if (!more) break;
+  }
+}
+
+// Whether the device route of process_jpeg_from_device takes a file whose header was read: the shape the
+// entropy decode takes, within one call's budget, and a frame the encoder would encode
+bool jpeg_seed_takes(const JpegScanHeader& h, size_t len, int S, bool (*encodable)(const JpegInput&)) {
+  if (!jpeg_device_shape(h, len) || !encodable(h.jpg)) return false;
+  long long cost[3];
+  jpeg_device_cost(h, len, S, cost);
+  return cost[0] < kJpegCallBudget && cost[1] < kJpegCallBudget && cost[2] < kJpegCallBudget;
+}
+
+// The device route's work on one file the route takes (d_data: its len bytes in device memory), on sc->s:
+// the entropy decode, then JpegDequantSanity into *dq ([3][nblocks][64], sc's memory).  kHost where the
+// decode flags the file or finds more than EOI after its scan; else kInsane or kTaken, with the offset of
+// EOI in *eoi.
+JpegSeed::Route jpeg_seed_decode(const uint8_t* d_data, size_t len, const JpegScanHeader& hdr, int S, JpegScope* sc,
+                                 int16_t** dq, size_t* eoi) {
+  const Stream s = sc->s;
+  const JpegInput* one = &hdr.jpg;
+  const JpegLayout L = jpeg_layout(&one, 1);
+  const size_t ncoef = static_cast<size_t>(L.blocks) * 64;
+  int16_t* d_coeffs = sc->alloc_n<int16_t>(ncoef);
+  *dq = sc->alloc_n<int16_t>(ncoef);
+  int* d_quant = sc->alloc_n<int>(3 * 64);
+  unsigned* d_words = sc->alloc_n<unsigned>(2);  // the status word, the end of the scan data
+  dev_zero(d_coeffs, sizeof(int16_t) * ncoef, s);
+  dev_zero(d_words, sizeof(unsigned), s);
+  h2d(d_quant, L.quant.data(), sizeof(int) * 3 * 64, s);
+  std::vector<JpegDeviceFile> fs{JpegDeviceFile{d_data, len, &hdr, &L.tab[0]}};
+  jpeg_entropy_decode(fs, d_coeffs, S, s, sc, d_words, d_words + 1);
+  launch_1d(s, JpegDequantSanity{d_coeffs, d_quant, static_cast<int>(L.blocks / 3), *dq, d_words},
+            static_cast<int>(ncoef), "jpeg_dequant_sanity");
+  unsigned words[2];
+  d2h(words, d_words, sizeof(words), s);
+  if (words[0] & ~kJpegBadSanity) return JpegSeed::kHost;
+  *eoi = words[1];
+  return words[0] ? JpegSeed::kInsane : JpegSeed::kTaken;
+}
 }  // namespace
+
+void jpeg_seed_from_device(const uint8_t* jpeg, size_t len, int device, Stream stream, int S,
+                           bool (*encodable)(const JpegInput&), JpegSeed* out) {
+  auto sc = std::make_shared<JpegScope>();
+  sc->open(device);
+  const Stream s = sc->s;
+  stream_wait(s, stream);
+  std::vector<JpegScanHeader> hdr(1);
+  std::vector<std::vector<uint8_t> > pre(1);
+  std::vector<char> head_ok(1, 0);
+  jpeg_read_headers(&jpeg, &len, 1, s, &hdr, &pre, &head_ok);
+  out->route = JpegSeed::kHost;
+  int16_t* dq = nullptr;
+  size_t eoi = 0;
+  if (head_ok[0] && jpeg_seed_takes(hdr[0], len, S, encodable))
+    out->route = jpeg_seed_decode(jpeg, len, hdr[0], S, sc.get(), &dq, &eoi);
+  if (out->route == JpegSeed::kHost) {
+    out->file.resize(len);
+    d2h(out->file.data(), jpeg, len, s);
+    return;
+  }
+  out->hdr = std::move(hdr[0]);
+  out->tail.resize(len - eoi - 2);
+  if (!out->tail.empty()) d2h(&out->tail[0], jpeg + eoi + 2, out->tail.size(), s);
+  out->dq = dq;
+  out->stream = s;
+  out->keep = sc;
+}
+
+JpegSeed::Route jpeg_debug_seed(const uint8_t* data, size_t len, int S, bool (*encodable)(const JpegInput&),
+                                std::vector<int16_t>* dq) {
+  JpegScanHeader hdr;
+  if (!read_jpeg_header(data, len, &hdr) || !jpeg_seed_takes(hdr, len, S, encodable)) return JpegSeed::kHost;
+  JpegScope sc;
+  sc.open(0);
+  uint8_t* d_data = sc.alloc_n<uint8_t>(len);
+  h2d(d_data, data, len, sc.s);
+  int16_t* d_dq = nullptr;
+  size_t eoi = 0;
+  const JpegSeed::Route r = jpeg_seed_decode(d_data, len, hdr, S, &sc, &d_dq, &eoi);
+  if (r != JpegSeed::kHost) {
+    dq->resize(static_cast<size_t>(hdr.jpg.components[0].width_in_blocks) * hdr.jpg.components[0].height_in_blocks * 192);
+    d2h(dq->data(), d_dq, sizeof(int16_t) * dq->size(), sc.s);
+  }
+  return r;
+}
 
 void jpeg_dimensions_from_device(const uint8_t* const* jpeg, const size_t* len, int n, int device, Stream stream,
                                  int* width, int* height) {
@@ -3507,28 +3630,10 @@ void jpeg_decode_rgb_from_device(const char* who, const uint8_t* const* jpeg, co
   sc.open(device);
   const Stream s = sc.s;
   stream_wait(s, stream);
-  // headers, from prefixes of 4 KiB doubling; each round covers every file still short of its first SOS
   std::vector<JpegScanHeader> hdr(n);
   std::vector<std::vector<uint8_t> > pre(n);
-  std::vector<char> head_ok(n, 0), pending(n, 1);
-  for (size_t m = kJpegFirstPrefix;; m *= 2) {
-    bool more = false;
-    for (int i = 0; i < n; ++i) {
-      if (!pending[i]) continue;
-      const size_t k = std::min(m, len[i]);
-      pre[i].resize(k);
-      if (k) d2h(pre[i].data(), jpeg[i], k, s);
-      if (read_jpeg_header(pre[i].data(), k, &hdr[i])) {
-        head_ok[i] = 1;
-        pending[i] = 0;
-      } else if (k == len[i]) {
-        pending[i] = 0;
-      } else {
-        more = true;
-      }
-    }
-    if (!more) break;
-  }
+  std::vector<char> head_ok(n, 0);
+  jpeg_read_headers(jpeg, len, n, s, &hdr, &pre, &head_ok);
   std::vector<char> dev(n, 0);
   std::vector<std::string> why(n);
   std::vector<JpegInput> host(n);

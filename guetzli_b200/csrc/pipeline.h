@@ -6,10 +6,12 @@
 #pragma once
 #include <stdint.h>
 
+#include <memory>
 #include <string>
 #include <vector>
 
 #include "butteraugli.h"
+#include "jpeg_in.h"
 
 namespace gb200 {
 
@@ -53,6 +55,34 @@ void jpeg_decode_rgb_from_device(const char* who, const uint8_t* const* jpeg, co
 // *coeffs where the device path takes the file and finds no error; false where it goes to the host path.
 bool jpeg_debug_entropy_decode(const uint8_t* data, size_t len, int S, std::vector<int16_t>* coeffs);
 
+// What the device route of process_jpeg_from_device (search.cc) makes of one file in device memory.
+struct JpegSeed {
+  // kTaken: read_jpeg accepts the file, check_jpeg_sanity too, and dq holds its coefficients; kInsane: read_jpeg
+  // accepts it, check_jpeg_sanity does not; kHost: the device route does not decide, `file` holds the file
+  enum Route { kHost, kInsane, kTaken };
+  Route route = kHost;
+  JpegScanHeader hdr;         // kTaken, kInsane: frame, quant tables, APPn / COM of the file
+  std::string tail;           // kTaken: the bytes after EOI
+  std::vector<uint8_t> file;  // kHost: the whole file, copied back
+  // kTaken: [3][nblocks][64] coefficients times their quant steps, device memory written by the work queued
+  // on `stream`; both stay valid while `keep` is held
+  const int16_t* dq = nullptr;
+  Stream stream = 0;
+  std::shared_ptr<void> keep;
+};
+// The device route for one file of len bytes in memory of `device`, read after the work queued on `stream`.
+// Its header is read from prefixes copied to the host (as jpeg_decode_rgb_from_device reads them); a file
+// that jpeg_device_shape takes within one call's budget and that `encodable` accepts is entropy-decoded with
+// subsequences of S bits and dequantised and checked by JpegDequantSanity (kernels.h) on the device, and
+// only its tail comes back.  Any other file, and any the decode flags or whose scan is followed by more than
+// EOI, is copied back whole (kHost).
+void jpeg_seed_from_device(const uint8_t* jpeg, size_t len, int device, Stream stream, int S,
+                           bool (*encodable)(const JpegInput&), JpegSeed* out);
+// Test hook: the same route on len bytes in host memory, uploaded first; *dq receives the plane where the
+// file is taken (kTaken or kInsane).
+JpegSeed::Route jpeg_debug_seed(const uint8_t* data, size_t len, int S, bool (*encodable)(const JpegInput&),
+                                std::vector<int16_t>* dq);
+
 // Exclusive prefix sum of n values on stream s (three launches), the total to device memory; sums holds
 // ceil(n / 1024) values.  ImageContext's scans use it.
 void exclusive_scan_device(Stream s, const unsigned int* in, unsigned int* out, int n, unsigned int* sums,
@@ -84,6 +114,9 @@ class ImageContext {
   // JPEG input (4:4:4): the original is given as dequantised DCT coefficients
   // [3][nblocks][64]; its pixels (DecodeJpegToRGB) are rendered on the device.
   ImageContext(const int16_t* dq_coeffs, int w, int h, int device, bool prepare_now, Comm* comm);
+  // The same coefficients in memory of `device`, copied into the context on its own stream after the work
+  // queued on `stream` so far; the copy is done when the constructor returns.
+  ImageContext(const int16_t* dq_dev, Stream stream, int w, int h, int device, bool prepare_now);
   // An 8-bit view (ImageView) turned into the packed RGB of the first constructor on the device, as the
   // guetzli tool turns PNG layouts into RGB (IngestU8, kernels.h); everything after that is the RGB path.
   // A device view is read in place after the work queued on its stream; a host view's span is uploaded
@@ -314,6 +347,8 @@ class ImageContext {
   void gather_reserve(size_t n);
   void gather_fetch(size_t n, std::vector<int16_t>* coeffs, std::vector<int>* cursor, std::vector<int>* in_bulk);
   bool from_coeffs_ = false;  // original given as coefficients (JPEG input)
+  bool dq_on_device_ = false;  // JPEG input in device memory, written by the work queued on dq_stream_
+  Stream dq_stream_ = 0;
   void guarded_init(const uint8_t* rgb, const int16_t* dq_coeffs, bool prepare_now, const ImageView* view = nullptr);
   void init(const uint8_t* rgb, const int16_t* dq_coeffs, bool prepare_now, const ImageView* view);
   void ingest(const ImageView& view);

@@ -1323,9 +1323,13 @@ static bool check_params(const SearchParams& params, std::string* err) {
 // Flat coefficient indices and the candidate-list offsets are 32-bit: refuse larger images up
 // front with a clear message instead of overflowing after all device memory is allocated.
 // (The scan's 32-bit bit offsets are checked where the scan size is known, jpeg_encode_scan.)
-bool image_size_supported(int w, int h, std::string* err) {
+static bool image_size_fits(int w, int h) {
   const long long nblocks = static_cast<long long>((w + 7) / 8) * ((h + 7) / 8);
-  if (nblocks * 192 >= (1ll << 31)) {
+  return nblocks * 192 < (1ll << 31);
+}
+
+bool image_size_supported(int w, int h, std::string* err) {
+  if (!image_size_fits(w, h)) {
     char buf[160];
     snprintf(buf, sizeof(buf), "guetzli_b200: image too large (%d x %d): at most %lld 8x8 blocks are supported\n", w, h,
              (1ll << 31) / 192 - 1);
@@ -1418,6 +1422,82 @@ bool process_resident_impl(const SearchParams& params, ImageContext* ctx, const 
 }
 }  // namespace
 
+namespace {
+bool refuse(const char* msg, std::string* err) {
+  *err = msg;
+  fputs(msg, stderr);
+  return false;
+}
+const char kCantRead[] = "Can't read jpg data from input file\n";
+const char kInsane[] = "Unsupported input JPEG (unexpectedly large coefficient values).\n";
+
+// What the search needs of a 4:4:4 file besides its coefficients: quant tables, component ids and metadata
+// as read, the bytes after EOI (jpg's own tail_data when the whole file was read)
+void jpeg_source(const SearchParams& params, const JpegInput& jpg, const std::string& tail, JpegSource* src) {
+  for (int c = 0; c < 3; ++c) {
+    const JpegComponent& comp = jpg.components[c];
+    memcpy(src->q_in[c], jpg.quant[comp.quant_idx].values, sizeof(src->q_in[c]));
+    src->layout.comp_id[c] = comp.id;
+    src->layout.comp_table[c] = comp.quant_idx;
+  }
+  src->layout.num_tables = static_cast<int>(jpg.quant.size());
+  for (int i = 0; i < src->layout.num_tables; ++i) {
+    memcpy(src->layout.table[i], jpg.quant[i].values, sizeof(src->layout.table[i]));
+    src->layout.precision[i] = jpg.quant[i].precision;
+    src->layout.index[i] = jpg.quant[i].index;
+  }
+  src->meta.strip = params.clear_metadata;
+  src->meta.app_data = jpg.app_data;
+  src->meta.com_data = jpg.com_data;
+  src->meta.tail_data = tail;
+}
+
+// Process(jpeg bytes) (g/processor.cc:890-924) once ReadJpeg has accepted the file
+bool process_jpeg_input(const SearchParams& params, const JpegInput& jpg, int device, LogSink log, void* log_user,
+                        std::string* jpeg_out, SearchStats* st, std::string* err) {
+  if (!check_jpeg_sanity(jpg)) return refuse(kInsane, err);
+  const size_t ncomp = jpg.components.size();
+  const bool decodable = ncomp == 1 || (ncomp == 3 && has_ycbcr_color_space(jpg) && (jpg.is_420() || jpg.is_444()));
+  if (!decodable)
+    return refuse(
+        "Unsupported input JPEG file (e.g. unsupported downsampling mode).\nPlease provide the input image as a PNG "
+        "file.\n",
+        err);
+  if (!check_params(params, err)) return false;
+  if (ncomp != 3 || !has_ycbcr_color_space(jpg)) return refuse("Only YUV color space input jpeg is supported\n", err);
+  if (!jpg.is_444())
+    return refuse("guetzli_b200: YUV420 JPEG input is outside the GPU hot path (DESIGN.md); provide 4:4:4 or PNG\n",
+                  err);
+
+  if (!image_size_supported(jpg.width, jpg.height, err)) return false;
+  Clock::time_point t0 = Clock::now();
+  const long long h2d0 = h2d_bytes_total();
+  JpegSource src;
+  jpeg_source(params, jpg, jpg.tail_data, &src);
+  const int nblocks = jpg.components[0].width_in_blocks * jpg.components[0].height_in_blocks;
+  // RemoveOriginalQuantization (g/processor.cc:82): coefficients times their quant step
+  std::vector<int16_t> dq(static_cast<size_t>(3) * nblocks * 64);
+  for (int c = 0; c < 3; ++c) {
+    const JpegComponent& comp = jpg.components[c];
+    const int* q = jpg.quant[comp.quant_idx].values;
+    int16_t* dst = &dq[static_cast<size_t>(c) * nblocks * 64];
+    for (size_t i = 0; i < comp.coeffs.size(); ++i) dst[i] = static_cast<int16_t>(comp.coeffs[i] * q[i & 63]);
+  }
+  ImageContext ctx(dq.data(), jpg.width, jpg.height, device, false, nullptr);
+  st->ms_device_setup = ms_since(t0);
+  const bool ok = process_resident_impl(params, &ctx, &src, log, log_user, jpeg_out, st, err);
+  st->h2d_bytes = h2d_bytes_total() - h2d0;
+  st->ms_total = ms_since(t0);
+  return ok;
+}
+
+// The files process_jpeg_input encodes once check_params passes: 4:4:4, YCbCr as the reference guesses it
+// (not libjpeg_ycbcr), of a size the device lists index
+bool jpeg_encodable(const JpegInput& j) {
+  return j.is_444() && has_ycbcr_color_space(j) && image_size_fits(j.width, j.height);
+}
+}  // namespace
+
 // Process(jpeg bytes), g/processor.cc:890-924.
 bool process_jpeg(const SearchParams& params, const uint8_t* data, size_t len, int device, LogSink log,
                   void* log_user, std::string* jpeg_out, SearchStats* stats, std::string* err) {
@@ -1425,59 +1505,60 @@ bool process_jpeg(const SearchParams& params, const uint8_t* data, size_t len, i
   SearchStats* st = stats ? stats : &local;
   *st = SearchStats();
   jpeg_out->clear();
-  auto fail = [err](const char* msg) {
-    *err = msg;
-    fputs(msg, stderr);
-    return false;
-  };
   JpegInput jpg;
   std::string why;
-  if (data == nullptr || !read_jpeg(data, len, &jpg, &why)) return fail("Can't read jpg data from input file\n");
-  if (!check_jpeg_sanity(jpg)) return fail("Unsupported input JPEG (unexpectedly large coefficient values).\n");
-  const size_t ncomp = jpg.components.size();
-  const bool decodable = ncomp == 1 || (ncomp == 3 && has_ycbcr_color_space(jpg) && (jpg.is_420() || jpg.is_444()));
-  if (!decodable)
-    return fail(
-        "Unsupported input JPEG file (e.g. unsupported downsampling mode).\nPlease provide the input image as a PNG "
-        "file.\n");
-  if (!check_params(params, err)) return false;
-  if (ncomp != 3 || !has_ycbcr_color_space(jpg)) return fail("Only YUV color space input jpeg is supported\n");
-  if (!jpg.is_444())
-    return fail("guetzli_b200: YUV420 JPEG input is outside the GPU hot path (DESIGN.md); provide 4:4:4 or PNG\n");
+  if (data == nullptr || !read_jpeg(data, len, &jpg, &why)) return refuse(kCantRead, err);
+  return process_jpeg_input(params, jpg, device, log, log_user, jpeg_out, st, err);
+}
 
-  if (!image_size_supported(jpg.width, jpg.height, err)) return false;
-  Clock::time_point t0 = Clock::now();
-  const long long h2d0 = h2d_bytes_total();
+bool process_jpeg_from_device(const SearchParams& params, const uint8_t* data, size_t len, int device, Stream stream,
+                              LogSink log, void* log_user, std::string* jpeg_out, SearchStats* stats,
+                              std::string* err) {
+  SearchStats local;
+  SearchStats* st = stats ? stats : &local;
+  *st = SearchStats();
+  jpeg_out->clear();
+  const Clock::time_point t0 = Clock::now();
+  const long long h2d0 = h2d_bytes_total(), d2h0 = d2h_bytes_total();
+  auto done = [&](bool ok) {
+    st->h2d_bytes = h2d_bytes_total() - h2d0;
+    st->d2h_bytes = d2h_bytes_total() - d2h0;
+    st->ms_total = ms_since(t0);
+    return ok;
+  };
+  JpegSeed seed;
+  // an empty file has no bytes to read on the device: read_jpeg refuses it as it is
+  if (len > 0) jpeg_seed_from_device(data, len, device, stream, kJpegSubBits, jpeg_encodable, &seed);
+  if (seed.route == JpegSeed::kHost) {
+    JpegInput jpg;
+    std::string why;
+    if (!read_jpeg(seed.file.data(), seed.file.size(), &jpg, &why)) return done(refuse(kCantRead, err));
+    std::vector<uint8_t>().swap(seed.file);
+    const double read_ms = ms_since(t0);
+    const bool ok = process_jpeg_input(params, jpg, device, log, log_user, jpeg_out, st, err);
+    st->ms_device_setup += read_ms;
+    return done(ok);
+  }
+  // read_jpeg accepts the file: the sanity check, then check_params, then the rest, which the route ensures
+  if (seed.route == JpegSeed::kInsane) return done(refuse(kInsane, err));
+  if (!check_params(params, err)) return done(false);
   JpegSource src;
-  const int w = jpg.width, h = jpg.height;
-  const int nblocks = jpg.components[0].width_in_blocks * jpg.components[0].height_in_blocks;
-  // RemoveOriginalQuantization (g/processor.cc:82): coefficients times their quant step
-  std::vector<int16_t> dq(static_cast<size_t>(3) * nblocks * 64);
-  for (int c = 0; c < 3; ++c) {
-    const JpegComponent& comp = jpg.components[c];
-    const int* q = jpg.quant[comp.quant_idx].values;
-    memcpy(src.q_in[c], q, sizeof(src.q_in[c]));
-    int16_t* dst = &dq[static_cast<size_t>(c) * nblocks * 64];
-    for (size_t i = 0; i < comp.coeffs.size(); ++i) dst[i] = static_cast<int16_t>(comp.coeffs[i] * q[i & 63]);
-    src.layout.comp_id[c] = comp.id;
-    src.layout.comp_table[c] = comp.quant_idx;
-  }
-  src.layout.num_tables = static_cast<int>(jpg.quant.size());
-  for (int i = 0; i < src.layout.num_tables; ++i) {
-    memcpy(src.layout.table[i], jpg.quant[i].values, sizeof(src.layout.table[i]));
-    src.layout.precision[i] = jpg.quant[i].precision;
-    src.layout.index[i] = jpg.quant[i].index;
-  }
-  src.meta.strip = params.clear_metadata;
-  src.meta.app_data = jpg.app_data;
-  src.meta.com_data = jpg.com_data;
-  src.meta.tail_data = jpg.tail_data;
-  ImageContext ctx(dq.data(), w, h, device, false, nullptr);
+  jpeg_source(params, seed.hdr.jpg, seed.tail, &src);
+  ImageContext ctx(seed.dq, seed.stream, seed.hdr.jpg.width, seed.hdr.jpg.height, device, false);
+  seed.keep.reset();
   st->ms_device_setup = ms_since(t0);
-  const bool ok = process_resident_impl(params, &ctx, &src, log, log_user, jpeg_out, st, err);
-  st->h2d_bytes = h2d_bytes_total() - h2d0;
-  st->ms_total = ms_since(t0);
-  return ok;
+  return done(process_resident_impl(params, &ctx, &src, log, log_user, jpeg_out, st, err));
+}
+
+int jpeg_debug_seed_route(const uint8_t* data, size_t len, int S, std::vector<int16_t>* dq) {
+  switch (jpeg_debug_seed(data, len, S, jpeg_encodable, dq)) {
+    case JpegSeed::kTaken:
+      return 1;
+    case JpegSeed::kInsane:
+      return 2;
+    default:
+      return 0;
+  }
 }
 
 bool process_rgb(const SearchParams& params, const uint8_t* rgb, int w, int h, int device, LogSink log,

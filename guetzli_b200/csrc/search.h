@@ -6,6 +6,7 @@
 #include <stdint.h>
 
 #include <string>
+#include <vector>
 
 #include "backend.h"
 
@@ -58,6 +59,19 @@ bool process_rgb_tiled(const SearchParams& params, const uint8_t* rgb, int w, in
 // from the file's own coefficients and quant tables.
 bool process_jpeg(const SearchParams& params, const uint8_t* data, size_t len, int device, LogSink log,
                   void* log_user, std::string* jpeg_out, SearchStats* stats, std::string* err);
+// process_jpeg on a file of len bytes in memory of `device`, read once the work queued on `stream` so far is
+// done, with process_jpeg's result, output, trace, counters and refusals.  A sequential 4:4:4 YCbCr file the
+// encoder takes is Huffman-decoded, dequantised and checked on the device (jpeg_seed_from_device, pipeline.h);
+// any other file is copied back and goes through process_jpeg's own steps.  The stats cover the whole call:
+// ms_device_setup and ms_total from its start, h2d_bytes and d2h_bytes with the header prefixes and the file
+// or tail read back.
+bool process_jpeg_from_device(const SearchParams& params, const uint8_t* data, size_t len, int device, Stream stream,
+                              LogSink log, void* log_user, std::string* jpeg_out, SearchStats* stats,
+                              std::string* err);
+// Test hook: the device route's seeding with subsequences of S bits on host bytes (jpeg_debug_seed, pipeline.h):
+// 0 where the file goes to the host route, 1 where it is taken and sane, 2 where it is taken and fails
+// check_jpeg_sanity; *dq receives the plane where it is taken.
+int jpeg_debug_seed_route(const uint8_t* data, size_t len, int S, std::vector<int16_t>* dq);
 
 bool process_rgb(const SearchParams& params, const uint8_t* rgb, int w, int h, int device, LogSink log,
                  void* log_user, std::string* jpeg_out, SearchStats* stats, std::string* err);

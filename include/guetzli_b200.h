@@ -99,6 +99,21 @@ int gb200_process_image_device(const gb200_params* params, const uint8_t* img_de
 int gb200_process_jpeg(const gb200_params* params, const uint8_t* jpeg_in, size_t jpeg_len, int device,
                        gb200_log_fn log, void* log_user, uint8_t** out, size_t* out_len,
                        gb200_stats* stats);
+/* gb200_process_jpeg on a file held in memory of `device` (jpeg_len bytes at jpeg_dev), read once the work
+ * queued on `stream` (a cudaStream_t; NULL for the legacy default stream) so far is done.  For the same bytes
+ * it returns what gb200_process_jpeg returns: the result, the output (best-so-far bytes on failure), the
+ * --verbose trace, the iteration counters and the refusals, in the same order.  The header is read from
+ * prefixes copied to the host.  A sequential 4:4:4 YCbCr file the encoder takes (its first scan carries every
+ * component, under 256 MiB) is Huffman-decoded, dequantised and checked for coefficients beyond 4096 on the
+ * device; only its bytes after EOI and the one coefficient plane the host search keeps (384 bytes per 8x8
+ * block) come back.  Every other file (progressive, gray, subsampled, CMYK, damaged) is copied back whole
+ * and read as gb200_process_jpeg reads it.  The file may be overwritten once the call returns.  Host,
+ * managed and other-device pointers are refused before anything runs ("... is not device memory of device
+ * N"); a NULL jpeg_dev with jpeg_len 0 is refused as an unreadable file.  The stats cover the whole call,
+ * header read and decode included.  The CPU port has no device memory and refuses every call. */
+int gb200_process_jpeg_from_device(const gb200_params* params, const uint8_t* jpeg_dev, size_t jpeg_len,
+                                   int device, gb200_log_fn log, void* log_user, uint8_t** out,
+                                   size_t* out_len, gb200_stats* stats, void* stream);
 
 /* butteraugli::ButteraugliInterface(rgb0, rgb1, diffmap, diffvalue)
  * (third_party/butteraugli/butteraugli/butteraugli.cc:1858; the stand-alone `butteraugli`
@@ -391,6 +406,14 @@ int gb200_debug_read_jpeg(const uint8_t* jpeg_in, size_t jpeg_len, int* dims, in
  * success. */
 int gb200_debug_entropy_decode(const uint8_t* jpeg_in, size_t jpeg_len, int S, int16_t* out, size_t out_cap,
                                int* status);
+/* test hook: the seeding of gb200_process_jpeg_from_device's device route (entropy decode with subsequences
+ * of S bits, then JpegDequantSanity) on one file in host memory, uploaded first (on the CPU port: run as host
+ * loops).  *status = 1 where the route takes the file and it passes the sanity check, 2 where the route takes
+ * it and a coefficient times its quant step exceeds 4096 in magnitude, 0 where the file goes to the host
+ * route.  Where it is taken, dq receives [3][blocks][64] coefficients times their quant steps (natural order,
+ * stored as int16). Returns 1 on success. */
+int gb200_debug_jpeg_seed(const uint8_t* jpeg_in, size_t jpeg_len, int S, int16_t* dq, size_t dq_cap,
+                          int* status);
 
 /* ---- one image tiled over the GPUs of a node (BASELINE configs[3]) ------------
  * One process per GPU.  Rank 0 obtains an id, the host application distributes it
