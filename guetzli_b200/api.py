@@ -113,6 +113,8 @@ def load_library(path=None):
     lib.gb200_debug_entropy_decode.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_size_t,
                                                P(C.c_int)]
     lib.gb200_debug_jpeg_seed.argtypes = lib.gb200_debug_entropy_decode.argtypes
+    lib.gb200_debug_entropy_decode_flags.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_size_t,
+                                                     P(C.c_int), P(C.c_uint), P(C.c_int)]
     lib.gb200_butteraugli_diffmap.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                               P(C.c_double)]
     lib.gb200_butteraugli_comparator_create.restype = C.c_void_p
@@ -496,6 +498,27 @@ def entropy_decode(jpeg_in, S, lib=None, cap=1 << 24):
                                           C.byref(status)):
         raise RuntimeError(_err(lib))
     return bool(status.value), (out if status.value else None)
+
+
+def entropy_decode_flags(jpeg_in, S, lib=None, cap=1 << 24):
+    """entropy_decode with the reason for the path the file takes (test hook) -> (taken, flags, rounds,
+    coefficients): taken where the device path's shape takes the file; flags the OR of its kJpegBad* flags
+    (JPEG_BAD_*), the SIMD-range test of decode_jpeg included; rounds the synchronisation rounds after the
+    first; the coefficients as entropy_decode gives them where taken and flags is 0 or JPEG_BAD_RANGE, else
+    None."""
+    lib = lib or load_library()
+    buf = np.frombuffer(bytes(jpeg_in), dtype=np.uint8)
+    out = np.zeros(cap, dtype=np.int16)
+    taken, flags, rounds = C.c_int(), C.c_uint(), C.c_int()
+    if not lib.gb200_debug_entropy_decode_flags(buf.ctypes.data if buf.size else None, buf.size, S, out.ctypes.data,
+                                                cap, C.byref(taken), C.byref(flags), C.byref(rounds)):
+        raise RuntimeError(_err(lib))
+    coeffs = out if taken.value and not flags.value & ~JPEG_BAD_RANGE else None
+    return bool(taken.value), flags.value, rounds.value, coeffs
+
+
+# the kJpegBad* flags of the device path's status words (csrc/kernels.h)
+JPEG_BAD_SEGMENT, JPEG_BAD_CODE, JPEG_BAD_RANGE, JPEG_BAD_SYNC = 1, 2, 4, 8
 
 
 def jpeg_seed(jpeg_in, S, lib=None, cap=1 << 24):

@@ -1117,6 +1117,23 @@ int gb200_debug_entropy_decode(const uint8_t* jpeg_in, size_t jpeg_len, int S, i
   });
 }
 
+int gb200_debug_entropy_decode_flags(const uint8_t* jpeg_in, size_t jpeg_len, int S, int16_t* out, size_t out_cap,
+                                     int* taken, unsigned* flags, int* rounds) {
+  return guarded([&]() {
+    if (jpeg_in == nullptr || taken == nullptr || flags == nullptr || rounds == nullptr)
+      throw std::runtime_error("debug_entropy_decode_flags: null argument");
+    if (S < 8) throw std::runtime_error("debug_entropy_decode_flags: subsequences of fewer than 8 bits");
+    std::vector<int16_t> c;
+    gb200::JpegDebugDecode r;
+    gb200::jpeg_debug_entropy_decode_flags(jpeg_in, jpeg_len, S, &c, &r);
+    if (c.size() > out_cap) throw std::runtime_error("debug_entropy_decode_flags: out is too small");
+    if (!c.empty()) memcpy(out, c.data(), c.size() * sizeof(int16_t));
+    *taken = r.taken ? 1 : 0;
+    *flags = r.flags;
+    *rounds = r.rounds;
+  });
+}
+
 int gb200_debug_jpeg_seed(const uint8_t* jpeg_in, size_t jpeg_len, int S, int16_t* dq, size_t dq_cap, int* status) {
   return guarded([&]() {
     if (jpeg_in == nullptr || dq == nullptr || status == nullptr)

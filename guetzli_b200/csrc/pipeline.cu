@@ -3730,8 +3730,18 @@ void jpeg_decode_rgb_from_device(const char* who, const uint8_t* const* jpeg, co
 }
 
 bool jpeg_debug_entropy_decode(const uint8_t* data, size_t len, int S, std::vector<int16_t>* coeffs) {
+  JpegDebugDecode r;
+  jpeg_debug_entropy_decode_flags(data, len, S, coeffs, &r);
+  return r.taken && (r.flags & ~kJpegBadRange) == 0;
+}
+
+void jpeg_debug_entropy_decode_flags(const uint8_t* data, size_t len, int S, std::vector<int16_t>* coeffs,
+                                     JpegDebugDecode* r) {
+  *r = JpegDebugDecode();
+  coeffs->clear();
   JpegScanHeader hdr;
-  if (!read_jpeg_header(data, len, &hdr) || !jpeg_device_shape(hdr, len)) return false;
+  if (!read_jpeg_header(data, len, &hdr) || !jpeg_device_shape(hdr, len)) return;
+  r->taken = true;
   const JpegInput* one = &hdr.jpg;
   JpegLayout L = jpeg_layout(&one, 1);
   JpegScope sc;
@@ -3744,13 +3754,23 @@ bool jpeg_debug_entropy_decode(const uint8_t* data, size_t len, int S, std::vect
   dev_zero(d_coeffs, sizeof(int16_t) * 64 * static_cast<size_t>(L.blocks), s);
   dev_zero(d_status, sizeof(unsigned), s);
   std::vector<JpegDeviceFile> fs{JpegDeviceFile{d_data, len, &hdr, &L.tab[0]}};
-  jpeg_entropy_decode(fs, d_coeffs, S, s, &sc, d_status);
-  unsigned status = 0;
-  d2h(&status, d_status, sizeof(unsigned), s);
-  if (status) return false;
+  r->rounds = jpeg_entropy_decode(fs, d_coeffs, S, s, &sc, d_status);
+  // the SIMD-range test of jpeg_decode_rgb_from_device, on the same status word
+  JpegDecFile* d_tab = sc.alloc_n<JpegDecFile>(1);
+  int* d_blk0 = sc.alloc_n<int>(2);
+  int* d_quant = sc.alloc_n<int>(L.quant.size());
+  int* d_check = sc.alloc_n<int>(1);
+  const int check = 1;
+  h2d(d_tab, L.tab.data(), sizeof(JpegDecFile), s);
+  h2d(d_blk0, L.blk0.data(), sizeof(int) * 2, s);
+  h2d(d_quant, L.quant.data(), sizeof(int) * L.quant.size(), s);
+  h2d(d_check, &check, sizeof(int), s);
+  launch_1d(s, JpegRangeCheck{d_coeffs, d_quant, d_tab, d_blk0, 1, d_check, d_status}, static_cast<int>(L.blocks),
+            "jpeg_range_check");
+  d2h(&r->flags, d_status, sizeof(unsigned), s);
+  if (r->flags & ~kJpegBadRange) return;
   coeffs->resize(static_cast<size_t>(L.blocks) * 64);
   d2h(coeffs->data(), d_coeffs, sizeof(int16_t) * coeffs->size(), s);
-  return true;
 }
 
 }  // namespace gb200

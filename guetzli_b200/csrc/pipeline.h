@@ -54,6 +54,17 @@ void jpeg_decode_rgb_from_device(const char* who, const uint8_t* const* jpeg, co
 // memory, uploaded first.  True with read_jpeg's coefficient layout (components one after another) in
 // *coeffs where the device path takes the file and finds no error; false where it goes to the host path.
 bool jpeg_debug_entropy_decode(const uint8_t* data, size_t len, int S, std::vector<int16_t>* coeffs);
+// Test hook: the same decode, then the SIMD-range test of jpeg_decode_rgb_from_device, with why the file goes
+// where it goes: whether jpeg_device_shape takes it, the kJpegBad* flags of its status word (kernels.h), and the
+// synchronisation rounds after the first.  *coeffs as above where the file is taken and flags has no bit but
+// kJpegBadRange; else empty.
+struct JpegDebugDecode {
+  bool taken = false;
+  unsigned flags = 0;
+  int rounds = 0;
+};
+void jpeg_debug_entropy_decode_flags(const uint8_t* data, size_t len, int S, std::vector<int16_t>* coeffs,
+                                     JpegDebugDecode* r);
 
 // What the device route of process_jpeg_from_device (search.cc) makes of one file in device memory.
 struct JpegSeed {

@@ -406,6 +406,14 @@ int gb200_debug_read_jpeg(const uint8_t* jpeg_in, size_t jpeg_len, int* dims, in
  * success. */
 int gb200_debug_entropy_decode(const uint8_t* jpeg_in, size_t jpeg_len, int S, int16_t* out, size_t out_cap,
                                int* status);
+/* test hook: the same decode, then gb200_jpeg_decode_rgb_from_device's SIMD-range test, with the reason for the
+ * path a file takes.  *taken = 1 where the device path's shape takes the file; *flags = the OR of its status
+ * word's flags (1 scan data not ending in EOI or RSTn missing / out of order, 2 an error read_jpeg raises
+ * as well, 4 the SIMD-range test, 8 no convergence within the synchronisation rounds); *rounds = the
+ * synchronisation rounds after the first.  out receives the coefficients as gb200_debug_read_jpeg gives them
+ * where the file is taken and flags is 0 or 4; else it is untouched.  Returns 1 on success. */
+int gb200_debug_entropy_decode_flags(const uint8_t* jpeg_in, size_t jpeg_len, int S, int16_t* out, size_t out_cap,
+                                     int* taken, unsigned* flags, int* rounds);
 /* test hook: the seeding of gb200_process_jpeg_from_device's device route (entropy decode with subsequences
  * of S bits, then JpegDequantSanity) on one file in host memory, uploaded first (on the CPU port: run as host
  * loops).  *status = 1 where the route takes the file and it passes the sanity check, 2 where the route takes
